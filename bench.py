@@ -7,7 +7,7 @@ A "step" = one forward of the fusion layer over one batch of synthetic (ref, src
 ms_per_step = forward ms.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                  [--workload cfg2|cfg3|cfg4|cfg4_256|sweep] [--exchange peer|p2p|allgather]
+                  [--workload cfg2|cfg3|cfg4|cfg4_256|sweep] [--exchange peer|p2p|allgather] [--dump-outputs DIR]
 
 N>1 (torchrun, one rank per GPU = one camera view per GPU): every rank owns `pairs_per_gpu` frames of its view, the ranks
 exchange feature maps inside the timed region (ViewParallelFusion: peer-mapped reads over NVLink, NCCL send/recv, or NCCL
@@ -15,7 +15,7 @@ all-gather) and every rank fuses its view against its nearest-neighbour view.  W
 
 `--impl reference` times the reference's own CPU op sequence (oracle/torch_port.py, same ATen operators incl. its torch
 geometry) on the host cores with the same config / steps / warmup keys; the N=1 line of our arm also carries `cpu_baseline`
-(bounded sample of that) and `gpu_reference` (the same op sequence on the same B200: BASELINE.md B2, the >=10x target's denominator).
+(bounded sample of that) and `gpu_reference` (the same op sequence on the same GPU: BASELINE.md B2, the >=10x target's denominator).
 """
 from __future__ import annotations
 
@@ -44,7 +44,7 @@ WORKLOADS = {
                      desc="8-view synthetic, literal 256x256 feature map, C=256 K=64, one view (1 frame) per GPU, z+ZRESIDUAL eval"),
 }
 SWEEP_K, SWEEP_C = (16, 32, 64, 128), (64, 128, 256, 512)
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024
 METRIC = "epipolar_fusion_forward_views_per_sec"
 
 
@@ -65,7 +65,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
         except Exception:
             pass
-    return 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+    return 3350.0, "H100 SXM data sheet 3.35 TB/s (of fallback)"
 
 
 def make_config(args, wl, world):
@@ -80,7 +80,7 @@ def make_config(args, wl, world):
             "peer": "symmetric memory, the staging kernel reads the source view from the neighbour GPU over NVLink"}[args.exchange]
     return {"workload": wl["desc"], "pairs_per_gpu": N, "C": wl["C"], "feat_hw": [wl["H"], wl["W"]], "K": wl["K"],
             "parallelism": par,
-            "l2": "rotating %d input sets (%.0f MB > 126 MB L2), no reuse between consecutive steps" % (n_sets, n_sets * set_bytes / 1e6),
+            "l2": "rotating %d input sets (%.0f MB > 50 MB L2), no reuse between consecutive steps" % (n_sets, n_sets * set_bytes / 1e6),
             "outputs": "finalout + attn + corr_pos", "variant": args.variant}, n_sets
 
 
@@ -263,7 +263,7 @@ def run_sweep(args):
     peak, peak_src = measured_peaks()
     rows = []
     N, H, W = 4, 64, 64
-    steps, warmup = min(args.steps, 30), max(3, min(args.warmup, 10))
+    steps, warmup = args.steps, max(3, min(args.warmup, 10))
     for K in SWEEP_K:
         for C in SWEEP_C:
             cfg = epi.make_cfg(KEYPOINT=dict(HEATMAP_SIZE=(H, W), NFEATS=C), EPIPOLAR=dict(SAMPLESIZE=K, USE_CORRECT_NORMALIZE=True))
@@ -300,6 +300,30 @@ def run_sweep(args):
                       "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                       "config": {"workload": "K x C sweep (BASELINE config 5) at a 64x64 feature map, N=4 pairs; value = geometric mean",
                                  "variant": args.variant}, "peak": peak, "peak_source": peak_src, "sweep": rows}), flush=True)
+
+
+DUMP_NAMES = ("finalout", "corr_pos", "attn", "sample_locs")
+DUMP_BUDGET = 64 * 1024 * 1024          # bytes over all dumped arrays
+DUMP_PER_ARRAY = DUMP_BUDGET // len(DUMP_NAMES)
+
+
+def dump_outputs(out_dir, result):
+    """Write what the timed path returned in its last step as out_dir/<name>.npy (float32).  An array larger than its share of
+    the budget is replaced by a fixed, seeded sample of its flattened elements (the same positions on every run)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    items = result if isinstance(result, (tuple, list)) else (result,)
+    for i, t in enumerate(items):
+        if not isinstance(t, torch.Tensor):
+            continue
+        name = DUMP_NAMES[i] if len(items) == len(DUMP_NAMES) else "output%d" % i
+        a = t.detach().float().cpu().numpy().ravel()
+        cap = DUMP_PER_ARRAY // 4
+        if a.size > cap:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))
+            a = a[idx]
+            name += "_sample"
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
 
 
 def run_ours(args, wl):
@@ -397,14 +421,18 @@ def run_ours(args, wl):
         sampler.start()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
+    last = None
     for i in range(args.steps):
-        step(warmup + i)
+        last = None                     # release the previous step's outputs first: every step reuses one set of buffers
+        last = step(warmup + i)
     ev1.record()
     barrier()
     t = torch.tensor([ev0.elapsed_time(ev1)], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_step = float(t.item()) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---- correctness at N>1: the exchanged source map must give the same result as a local recompute, bit for bit ----
     parity = None
@@ -561,7 +589,11 @@ def main():
     ap.add_argument("--cpu-steps", type=int, default=8)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last step as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload == "sweep" or args.impl == "reference"):
+        ap.error("--dump-outputs writes the outputs of one workload of our implementation: not with --workload sweep or --impl reference")
     if args.workload == "sweep":
         if args.impl == "reference":
             print(json.dumps({"impl": "reference", "unavailable": "the sweep workload has no reference arm (use cfg2/cfg3)"}))

@@ -1,11 +1,11 @@
-"""B200-native epipolar-transformer fusion path (drop-in for the reference's
+"""H100-native (sm_90a) epipolar-transformer fusion path (drop-in for the reference's
 modeling/layers/epipolar.py::Epipolar + the projection helpers of vision/multiview.py).
 
     from epipolar_transformers_b200 import Epipolar, set_global_cfg
     sampler = Epipolar()                       # reads the global cfg like the reference
     out, corr_pos, attn, locs = sampler(feat_ref, feat_src, KRT_ref, KRT_src)
 
-The arithmetic runs in libepipolar_b200.so (hand-written sm_100a CUDA behind the C ABI in
+The arithmetic runs in libepipolar_b200.so (hand-written sm_90a CUDA behind the C ABI in
 include/epipolar_b200.h).  Importing this package does not need a GPU; calling the op does,
 and fails loudly if the library is missing.
 """

@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA library (sm_100a) with plain nvcc — no JIT cache, so the .so
+"""In-tree build of the CUDA library (sm_90a) with plain nvcc — no JIT cache, so the .so
 travels with the repo snapshot.  `python -m epipolar_transformers_b200.build [--force]`."""
 from __future__ import annotations
 
@@ -10,9 +10,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libepipolar_b200.so")
+STAMP = LIB + ".flags"          # the nvcc flags LIB was built with: a library built for another architecture is rebuilt
 SOURCES = ["epi_abi.cu", "epi_aux.cu", "epi_fusion_warp.cu", "epi_fusion_tile.cu", "epi_fusion_pipe.cu", "epi_fusion_bwd.cu", "epi_stage.cu", "epi_peaks.cu", "epi_zgemm.cu", "epi_umma_selftest.cu"]
 HEADERS = ["epi_common.cuh", "epi_kernels.cuh", "epi_umma.cuh", os.path.join("..", "..", "include", "epipolar_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -23,11 +24,18 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found; cannot build libepipolar_b200.so")
 
 
+def _flags_text() -> str:
+    return " ".join(NVCC_FLAGS) + "\n"
+
+
 def needs_build() -> bool:
-    if not os.path.exists(LIB):
+    if not os.path.exists(LIB) or not os.path.exists(STAMP):
         return True
+    with open(STAMP) as f:
+        if f.read() != _flags_text():
+            return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS]
+    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS] + [os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
@@ -54,7 +62,10 @@ def build(force: bool = False, verbose: bool = False, timers: bool = False) -> s
             sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s" % s)
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", lib, *objs, "-lcudart"])
+    subprocess.check_call([nvcc, *NVCC_FLAGS[:2], "-shared", "-o", lib, *objs, "-lcudart"])
+    if not timers:
+        with open(STAMP, "w") as f:
+            f.write(_flags_text())
     return lib
 
 

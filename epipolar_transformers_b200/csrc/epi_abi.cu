@@ -36,9 +36,8 @@ bool want_pipe(const EpiFusionParams *p) {
     if (p->variant != EPI_VARIANT_AUTO && p->variant != EPI_VARIANT_PIPE) return false;
     if (!epi::fusion_pipe_shape_ok(p->C, p->H, p->W, p->K, p->sample_locs_in != nullptr)) return false;
     // Automatic selection leaves one corner to the other kernels: K > 48 on maps of 2K pixels or more a side.  There a single pixel's
-    // taps (4K, sampled sparsely along a long line) already fill the 256-row union, so every work item splits down to one pixel
-    // (measured at C=256, K=64: 60-75 ns per pixel from 128x128 up, against 34-38 for the CUDA-core kernel; 7-13 ns up to 96x96, and
-    // 3-4 ns at K=32 on 128x128 .. 256x256 — tools/gpu_mapsize.py, profiles/mapsize_r2.txt).
+    // taps (4K, sampled sparsely along a long line) already fill the 256-row union, so every work item splits down to one pixel and
+    // the per-pixel CUDA-core kernel does less work (tools/gpu_mapsize.py times the kernels per map size).
     if (p->variant == EPI_VARIANT_AUTO && 4 * p->K > 192 && (p->H > p->W ? p->H : p->W) >= 2 * p->K) return false;
     return true;
 }

@@ -1,4 +1,4 @@
-// epi_common.cuh — shared device code of the epipolar fusion kernels (sm_100a).
+// epi_common.cuh — shared device code of the epipolar fusion kernels (sm_90a).
 //
 // Geometry restates grid2sample_locs (/root/reference/modeling/layers/epipolar.py:323-418) and
 // the helpers of /root/reference/vision/multiview.py (:16-21 camera_center, :25-37 normalize,
@@ -141,7 +141,7 @@ __device__ __forceinline__ Taps make_taps(float gx, float gy, int H, int W, int 
 
 // Programmatic dependent launch (the three launches of a forward are chained with
 // cudaLaunchAttributeProgrammaticStreamSerialization): a kernel's CTAs may become resident and run their prologue
-// (barrier init, TMEM allocation, tensor-map prefetch) while the previous kernel of the stream drains;
+// (barrier init, tensor-map prefetch) while the previous kernel of the stream drains;
 // pdl_wait() returns once that kernel has completed and its writes are visible.  Nothing the previous kernels
 // wrote may be read, and nothing they read may be written, before pdl_wait().
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -1,25 +1,24 @@
 // epi_fusion_pipe.cu — the fused epipolar attention kernel (default): warp-specialised, mbarrier-pipelined,
-// tcgen05/TMEM.  One persistent CTA per SM, 25 warps:
+// warpgroup MMA (wgmma).  One persistent CTA per SM, 24 warps:
 //
-//   warps  0-15  workers   scores TMEM -> table, 4-tap interpolation, ==0 mask, softmax over K (warp shuffles),
-//                          attn / corr_pos / sample_locs, β scatter, β -> bf16 (hi, lo) panels, epilogue TMEM -> global
+//   warps  0-15  workers   four warpgroups: GEMM1 (wgmma, registers -> score table), 4-tap interpolation, ==0 mask,
+//                          softmax over K, attn / corr_pos / sample_locs, β scatter, β -> bf16 (hi, lo) panels,
+//                          GEMM2 (wgmma, registers -> table) and the epilogue table -> global
 //   warps 16-19  setup     next work item: pixel list (sector order), epipolar line end points, union bitmap of the
 //                          bilinear taps of the item's pixels, prefix ranks, row list for the gathers
 //   warps 20-23  gather    16-byte cp.async (LDGSTS) of query rows and source-feature rows (bf16 hi/lo planes, pixel-major)
 //                          into 128-byte-swizzled shared-memory panels; completion through cp.async.mbarrier.arrive
-//                          (TMA tile::gather4 was measured at 7.5 B/clk/SM — profiles/gather4_probe_r2.txt — 5x too slow)
-//   warp  24     MMA       tcgen05.mma issue (one lane): GEMM1 S = F·Qᵀ and GEMM2 Oᵀ = Fᵀ·βᵀ, tcgen05.commit -> mbarriers
 //
 // Maths (identical to epi_fusion_tile.cu, restating /root/reference/modeling/layers/epipolar.py:199,210 grid_sample taps,
 // :295-307 similarity / ==0 mask / scale / softmax, :237-243 arg-max + weighted sum, :323-418 geometry):
 //   sim_k = Σ_t w_kt · (q · f[p_t])        out = Σ_p β_p · f[p],   β_p = Σ_{k,t→p} a_k w_kt
 // over the UNION of source pixels touched by the item's ≤32 epipolar lines (D ≤ 256 rows; items whose union is larger
-// are split by the setup warps).  Operands are bf16 (hi, lo) pairs: hi·hi + hi·lo + lo·hi, fp32 accumulation in TMEM.
+// are split by the setup warps).  Operands are bf16 (hi, lo) pairs: hi·hi + hi·lo + lo·hi, fp32 accumulation in registers.
 //
-// Pipeline: item j+1's gather + GEMM1 run while the workers are in item j's softmax phase; GEMM2(j) runs during
-// the workers' phase of item j+1; S and O accumulators are double-buffered in the 512 TMEM columns; the feature stages
-// are a 3-deep ring of 32 KB filled by the gather warps.  The only CTA-wide barriers are two 512-thread named barriers per item
-// among the workers; everything else is mbarrier producer/consumer hand-off.
+// Pipeline: the setup warps build item j+1 and the gather warps fill the feature ring (3 stages of 32 KB) for item j's GEMM2
+// and item j+1's GEMM1 while the workers are in item j's softmax phase.  The workers' warpgroups issue the MMAs of a stage
+// together (warpgroup wg owns 64 rows of the accumulator), wait for them and hand the stage back; the accumulators go from
+// registers straight into the shared-memory table.  Everything between the roles is mbarrier producer/consumer hand-off.
 #include <cuda_bf16.h>
 
 #include "epi_kernels.cuh"
@@ -34,10 +33,10 @@ constexpr int CHUNK = 128;         // union rows per GEMM1 accumulator (MMA M)
 constexpr int DMAX = 256;          // max union rows per item (two chunks)
 constexpr int NWORK = 16;          // worker warps
 constexpr int NT_WORK = NWORK * 32;
-constexpr int W_SETUP = 16, W_GATHER = 20, W_MMA = 24;
+constexpr int W_SETUP = 16, W_GATHER = 20;
 constexpr int NSETUP = 128;        // setup threads
 constexpr int NGATHER = 128;       // gather threads
-constexpr int NT_ALL = 800;
+constexpr int NT_ALL = 768;
 constexpr int MAXWORDS = 512;      // bitmap words: H*W <= 16384
 constexpr int MAXKPL = 4;          // samples per lane: K <= 128
 constexpr int NSTAGE = 3;
@@ -51,7 +50,7 @@ constexpr uint32_t OFF_STAGE = 0;
 constexpr uint32_t OFF_Q = NSTAGE * STAGE_BYTES;           // 4 stacked panels
 constexpr uint32_t OFF_BETA = OFF_Q + 4 * PANEL_B2;        // 4 stacked panels (256 d)
 // d-major score table T[rank][pixel]: 32 floats per row, the float4 column XOR-ed with rank % 8.  Lane <-> pixel accesses hit
-// bank (pixel-derived) regardless of each lane's rank pattern; lane <-> rank accesses (TMEM read-out) are conflict free too.
+// bank (pixel-derived) regardless of each lane's rank pattern; lane <-> rank accesses are conflict free too.
 __device__ __forceinline__ int tix(int r, int i) { return r * 32 + ((((i >> 2) ^ r) & 7) << 2) + (i & 3); }
 constexpr uint32_t OFF_TABLE = OFF_BETA + 4 * PANEL_B2;    // [DMAX][32] fp32 scores, then int32 β, then the epilogue's [32][256] transposition
 constexpr uint32_t OFF_RED = OFF_TABLE + DMAX * 32 * 4;    // softmax / arg-max split-reduction scratch [4][16][32]
@@ -87,10 +86,6 @@ struct Ctrl {
     uint64_t desc_full[NDESC], desc_free[NDESC];
     uint64_t q_full, q_empty;
     uint64_t f_full[NSTAGE], f_empty[NSTAGE];
-    uint64_t s_full[2], s_empty[2];
-    uint64_t beta_full;
-    uint64_t o_full[2], o_empty[2];
-    uint32_t tmem_base;
     int stack[16];
     int sp;
     int cur;                       // item being built: g0 | gn << 8
@@ -103,10 +98,6 @@ constexpr uint32_t SMEM_BYTES = OFF_CTRL + ((sizeof(Ctrl) + 127) / 128 * 128);
 constexpr uint32_t SMEM_ALLOC = SMEM_BYTES + 1024;         // 1024-byte alignment slack
 static_assert(SMEM_ALLOC <= 232448 - 2048, "keep head-room below the 227 KB opt-in limit");
 
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t TMEM_S = 0;       // 2 buffers x 2 chunks x 64 columns
-constexpr uint32_t TMEM_O = 256;     // 2 buffers x 2 channel halves x 64 columns
-
 __device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // Bounded mbarrier wait: a protocol bug must never hang the GPU.  On timeout the error word is set and the whole CTA
@@ -115,16 +106,6 @@ __device__ __forceinline__ void wait_n(uint64_t *bar, uint32_t n) {
     const uint32_t parity = n & 1u;
     for (uint32_t it = 0; !mbar_try_wait(bar, parity); ++it)
         if (it > (1u << 24)) __trap();
-}
-
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float *v) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                   "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr)
-                 : "memory");
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
@@ -183,9 +164,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
     // accumulator takes all 256 columns of the O region (four channel halves, single-buffered) and the epilogue runs twice.
     const bool wide = C > 256;
     const int NQH = wide ? 2 : 1;
-    auto obuf = [&](int jj) -> int { return wide ? 0 : (jj & 1); };                 // O accumulator buffer of item jj
-    auto ouse = [&](int jj) -> uint32_t { return (uint32_t)(wide ? jj : (jj >> 1)); };   // earlier uses of that buffer
-    auto ocol = [&](int jj, int h) -> uint32_t { return TMEM_O + (wide ? 0u : (uint32_t)(jj & 1) * 128u) + (uint32_t)h * 64u; };
     const GeomCfg gc = a.geom;
     const int NHW = a.N * HW;                       // plane stride (rows) of the operand buffer [ref_hi|ref_lo|src_hi|src_lo]
     constexpr int KW = 2 * KPL;                     // samples per worker warp (k = warp + 16 jj)
@@ -195,23 +173,14 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
 #ifdef EPI_PIPE_TIMERS
     if (tid == 0 && blockIdx.x < 256) { unsigned long long g; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g)); g_pipe_cta[blockIdx.x * 4] = g; }
 #endif
-    if (warp == 0) tmem_alloc(&ct.tmem_base, TMEM_COLS);
     if (tid == 32) {
         for (int i = 0; i < NDESC; i++) { mbar_init(&ct.desc_full[i], 1); mbar_init(&ct.desc_free[i], 2); }
         mbar_init(&ct.q_full, NGATHER); mbar_init(&ct.q_empty, 1);
         for (int i = 0; i < NSTAGE; i++) { mbar_init(&ct.f_full[i], NGATHER); mbar_init(&ct.f_empty[i], 1); }
-        for (int i = 0; i < 2; i++) {
-            mbar_init(&ct.s_full[i], 1); mbar_init(&ct.s_empty[i], 1);
-            mbar_init(&ct.o_full[i], 1); mbar_init(&ct.o_empty[i], NWORK);
-        }
-        mbar_init(&ct.beta_full, NWORK);
         ct.sp = 0; ct.done = 0;
         mbar_fence_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ct.tmem_base;
     pdl_wait();                                     // operand planes, pixel order, pair constants, counters: the staging launch
 #ifdef EPI_PIPE_TIMERS
     if (tid == 0 && blockIdx.x < 256) { unsigned long long g; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g)); g_pipe_cta[blockIdx.x * 4 + 1] = g; }
@@ -224,7 +193,9 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         // bank-conflict free, the K-wide softmax is a 16-way split reduction through shared memory.
         // =====================================================================================================
         const float sl2 = a.softmax_scale * 1.4426950408889634f;
-        const uint32_t tq = (uint32_t)((warp & 3) * 32) << 16;          // this warp's TMEM lane quadrant
+        const int wg = warp >> 2, t128 = tid & 127;                      // warpgroup, thread within it
+        const uint32_t sq = smem_u32(smem + OFF_Q), sb = smem_u32(smem + OFF_BETA);
+        uint32_t qcount = 0, fcount = 0;
         uint8_t *bb = smem + OFF_BETA;
         float *red_max = reinterpret_cast<float *>(smem + OFF_RED);     // [16][32]
         float *red_sum = red_max + NWORK * 32;
@@ -235,28 +206,58 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
 #pragma unroll
         for (int jj = 0; jj < KW; jj++) tkw[jj] = (float)(warp + NWORK * jj) / (float)(K - 1);
 
-        // epilogue of item j (accumulator buffer j & 1): fused feature TMEM -> table (as [pixel][channel]) -> global
+        // One feature stage of the ring: every worker waits for it, the warpgroups that own part of it issue their MMAs and wait
+        // for them, then the stage goes back to the gather warps.
+        auto consume_stage = [&]() -> uint32_t {
+            const uint32_t s = fcount % NSTAGE;
+            if (warp == 0) wait_n(&ct.f_full[s], fcount / NSTAGE);
+            named_bar(1, NT_WORK);
+            fence_proxy_async_smem();           // cp.async (generic proxy) writes -> wgmma (async proxy) reads
+            return s;
+        };
+        auto release_stage = [&](uint32_t s) {
+            named_bar(1, NT_WORK);              // the MMAs of every warpgroup on this stage have completed
+            if (tid == 0) mbar_arrive(&ct.f_empty[s]);
+            fcount++;
+        };
+
+        // GEMM2 Oᵀ = Fᵀ·βᵀ of item j, then its epilogue: fused feature -> table (as [pixel][channel]) -> global.
+        // Warpgroup wg accumulates channels (wg >> 1) * 128 + (wg & 1) * 64 .. +63 of each 256-channel part (two parts when C > 256).
         auto epilogue = [&](int j) {
             const Desc &d = desc_at(j);
+            float o0[16], o1[16];
+#pragma unroll
+            for (int e = 0; e < 16; e++) { o0[e] = 0.f; o1[e] = 0.f; }      // D == 0: all masked, zero vectors
+            if (d.D > 0) {
+                const int D16 = (d.D + 15) & ~15, nblk = (D16 + 63) >> 6;
+                for (int blk = 0; blk < nblk; blk++)
+                    for (int h = 0; h < NH; h++) {
+                        const uint32_t s = consume_stage();
+                        if ((h & 1) == (wg >> 1)) {
+                            const uint32_t sa = smem_u32(smem + OFF_STAGE + s * STAGE_BYTES) + (uint32_t)(wg & 1) * 8192u;
+                            const int nk = min(4, (D16 - blk * 64) >> 4);
+                            wg_fence();
+                            for (int kk = 0; kk < nk; kk++) {
+                                const uint64_t a_hi = make_smem_desc(sa + kk * 2048, 8192, 1024), a_lo = desc_add(a_hi, PLANE_BYTES);
+                                const uint64_t b = make_smem_desc(sb + blk * PANEL_B2 + kk * 32, 16, 1024), b_lo = desc_add(b, 4096);
+                                if (h >> 1) { wgmma_m64n32<1>(o1, a_hi, b); wgmma_m64n32<1>(o1, a_hi, b_lo); wgmma_m64n32<1>(o1, a_lo, b); }
+                                else        { wgmma_m64n32<1>(o0, a_hi, b); wgmma_m64n32<1>(o0, a_hi, b_lo); wgmma_m64n32<1>(o0, a_lo, b); }
+                            }
+                            wg_commit();
+                            wg_wait_all();
+                        }
+                        release_stage(s);
+                    }
+            }
             const int nparts = wide ? 2 : 1;
             for (int part = 0; part < nparts; part++) {
                 if (part) named_bar(1, NT_WORK);            // the first 256 channels have left the table
-                {
-                    const int h = (warp >> 2) & 1, ph = warp >> 3;
-                    const int c = h * 128 + (warp & 3) * 32 + lane;
-                    if (part * 2 + h < NH) {
-                        float v[16], v2[16];
-                        const uint32_t col = ocol(j, part * 2 + h) + (uint32_t)ph * 16u;
-                        tmem_ld_32x16(tmem + tq + col, v);
-                        tmem_ld_32x16(tmem + tq + col + 32u, v2);
-                        tmem_ld_wait();
+                if (part * 2 + (wg >> 1) < NH) {
+                    const int cb = (wg >> 1) * 128 + (wg & 1) * 64;
 #pragma unroll
-                        for (int ii = 0; ii < 16; ii++) table[(ph * 16 + ii) * 256 + c] = d.D > 0 ? v[ii] + v2[ii] : 0.f;   // D == 0: all masked
-                    }
+                    for (int e = 0; e < 16; e++) table[acc_col(t128, e) * 256 + cb + acc_row(t128, e)] = part ? o1[e] : o0[e];
                 }
-                tc_fence_before();
                 named_bar(1, NT_WORK);
-                if (part == nparts - 1 && lane == 0) mbar_arrive(&ct.o_empty[obuf(j)]);
 #pragma unroll
                 for (int u = 0; u < 2; u++) {
                     const int i = warp * 2 + u;
@@ -298,12 +299,9 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         PT_DECL;
         int j = 0;
         for (;; j++) {
-            // Only warp 0 polls the mbarriers (item descriptor, then its scores); the other 15 warps sleep in the hardware
-            // barrier instead of spinning through issue slots.  The barrier also separates item j-1's use of the table.
-            if (warp == 0) {
-                wait_n(&ct.desc_full[j % NDESC], (uint32_t)(j / NDESC));
-                if (desc_at(j).tile >= 0) wait_n(&ct.s_full[j & 1], (uint32_t)(j >> 1));
-            }
+            // Only warp 0 polls the mbarriers; the other 15 warps sleep in the hardware barrier instead of spinning through
+            // issue slots.  The barrier also separates item j-1's use of the table.
+            if (warp == 0) wait_n(&ct.desc_full[j % NDESC], (uint32_t)(j / NDESC));
             named_bar(1, NT_WORK);
             PT(0);
             if (tid == 0) TR(j, 4);
@@ -317,29 +315,47 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
             const int D = d.D, n = d.n;
             const int nch = (D + CHUNK - 1) / CHUNK;
 
-            // ---------------- B1: scores TMEM -> T[rank][pixel] ----------------
-            tc_fence_after();
+            // ---------------- B1: S = F·Qᵀ on the tensor cores -> T[rank][pixel] ----------------
+            // Warpgroup wg accumulates union rows (wg >> 1) * 128 + (wg & 1) * 64 .. +63, i.e. half of chunk wg >> 1.
             PT(2);
-            {
-                const int c = warp >> 2;
-                if (c < nch) {
-                    float v[32], v2[32];
-                    const uint32_t col = TMEM_S + (uint32_t)(j & 1) * 128u + (uint32_t)c * 64u;
-                    tmem_ld_32x32(tmem + tq + col, v);
-                    tmem_ld_32x32(tmem + tq + col + 32u, v2);
-                    tmem_ld_wait();
-                    const int r = c * CHUNK + (warp & 3) * 32 + lane;
-                    if (r < D) {
+            if (D > 0) {
+                float sacc[16];
 #pragma unroll
-                        for (int c4 = 0; c4 < 8; c4++)
-                            *reinterpret_cast<float4 *>(table + r * 32 + (((c4 ^ r) & 7) << 2)) =
-                                make_float4(v[4 * c4] + v2[4 * c4], v[4 * c4 + 1] + v2[4 * c4 + 1], v[4 * c4 + 2] + v2[4 * c4 + 2], v[4 * c4 + 3] + v2[4 * c4 + 3]);
+                for (int e = 0; e < 16; e++) sacc[e] = 0.f;
+                const int r0 = (wg >> 1) * CHUNK + (wg & 1) * 64;
+                const bool mine = r0 < D;
+                for (int qh = 0; qh < NQH; qh++) {
+                    const int npq = min(4, NP - qh * 4);
+                    if (warp == 0) wait_n(&ct.q_full, qcount);           // ordered before the MMAs by the first stage's barrier
+                    for (int c = 0; c < nch; c++)
+                        for (int kp = 0; kp < npq; kp++) {
+                            const uint32_t s = consume_stage();
+                            if (c == (wg >> 1) && mine) {
+                                const uint32_t sa = smem_u32(smem + OFF_STAGE + s * STAGE_BYTES) + (uint32_t)(wg & 1) * 8192u;
+                                wg_fence();
+#pragma unroll
+                                for (int ks = 0; ks < 4; ks++) {
+                                    const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = desc_add(a_hi, PLANE_BYTES);
+                                    const uint64_t b = make_smem_desc(sq + kp * PANEL_B2 + ks * 32, 16, 1024), b_lo = desc_add(b, 4096);
+                                    wgmma_m64n32<0>(sacc, a_hi, b); wgmma_m64n32<0>(sacc, a_hi, b_lo); wgmma_m64n32<0>(sacc, a_lo, b);
+                                }
+                                wg_commit();
+                                wg_wait_all();
+                            }
+                            release_stage(s);
+                        }
+                    if (tid == 0) mbar_arrive(&ct.q_empty);
+                    qcount++;
+                }
+                if (mine) {
+#pragma unroll
+                    for (int e = 0; e < 16; e++) {
+                        const int r = r0 + acc_row(t128, e);
+                        if (r < D) table[tix(r, acc_col(t128, e))] = sacc[e];
                     }
                 }
             }
-            tc_fence_before();
             named_bar(1, NT_WORK);
-            if (tid == 0) mbar_arrive(&ct.s_empty[j & 1]);
             if (tid == 0) TR(j, 5);
             PT(3);
 
@@ -477,7 +493,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                 }
             }
             if (a.corr_pos) { red_bv[warp * 32 + lane] = best_v; red_bk[warp * 32 + lane] = best_k; }
-            if (warp == 0 && j >= 1) wait_n(&ct.o_full[obuf(j - 1)], ouse(j - 1));   // GEMM2(j-1) has consumed the β panels
             named_bar(1, NT_WORK);
             PT(5);
             // ---------------- arg-max -> corr_pos (first maximum, like torch.argmax) ----------------
@@ -513,24 +528,16 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                 *reinterpret_cast<uint4 *>(bb + 4096 + off) = lo;
             }
             fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ct.beta_full);
             if (tid == 0) TR(j, 6);
             named_bar(1, NT_WORK);                          // the table is free: the epilogue transposes through it
             PT(7);
-            // ---------------- epilogue of the previous item (its GEMM2 ran during this item's softmax) ----------------
-            if (j >= 1) { tc_fence_after(); epilogue(j - 1); }
+            // ---------------- GEMM2 and epilogue ----------------
+            epilogue(j);
             if (tid == 0) TR(j, 7);
             PT(9);
 #ifdef EPI_PIPE_TIMERS
             if (pt_on) atomicAdd(&g_pipe_timers[8], 1ull);
 #endif
-        }
-        if (j >= 1) {                                   // drain
-            if (warp == 0) wait_n(&ct.o_full[obuf(j - 1)], ouse(j - 1));
-            named_bar(1, NT_WORK);
-            tc_fence_after();
-            epilogue(j - 1);
         }
     } else if (warp < W_GATHER) {
         // =====================================================================================================
@@ -770,7 +777,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
             if (st == 0) TR(j, 1);
             PT(11);
         }
-    } else if (warp < W_MMA) {
+    } else {
         // =====================================================================================================
         // GATHER WARPS (128 threads): query rows and feature stages, 16-byte cp.async into swizzled panels.
         // Thread t copies chunk j = t & 7 (8 channels) of rows (t >> 3) + 16·it; a row's 128-byte segment is read by 8
@@ -898,121 +905,16 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                 }
             }
             if (gt == 0) TR(j, 2);
-            if (j >= 1) {
-                if (desc_at(j - 1).D > 0) gemm2_stages(j - 1);
-                if (gt == 0) TR(j - 1, 8);
-                named_bar(3, NGATHER);                      // every gather thread has read item j-1's row list
-                if (gt == 0) mbar_arrive(&ct.desc_free[(j - 1) % NDESC]);
-            }
             if (last) break;
-        }
-    } else {
-        // =====================================================================================================
-        // MMA ISSUER
-        // =====================================================================================================
-        uint32_t qcount = 0, fcount = 0;
-        const uint32_t sq = smem_u32(smem + OFF_Q), sb = smem_u32(smem + OFF_BETA);
-        const bool pt_on = lane == 0; (void)pt_on;
-        PT_DECL;
-        auto gemm2 = [&](int jj) {
-            const Desc &d = desc_at(jj);
-            PT(20);
-            wait_n(&ct.beta_full, (uint32_t)jj);
-            PT(21);
-            if (jj >= (wide ? 1 : 2)) wait_n(&ct.o_empty[obuf(jj)], ouse(jj) - 1u);
-            PT(22);
-            tc_fence_after();
-            if (d.D > 0) {
-                const int D16 = (d.D + 15) & ~15, nblk = (D16 + 63) >> 6;
-                const uint32_t idesc64 = make_idesc_bf16(128, 2 * P, 1, 0), idesc32 = make_idesc_bf16(128, P, 1, 0);
-                for (int blk = 0; blk < nblk; blk++)
-                    for (int h = 0; h < NH; h++) {
-                        const uint32_t s = fcount % NSTAGE;
-                        PT(20);
-                        wait_n(&ct.f_full[s], fcount / NSTAGE);
-                        PT(23);
-                        fence_proxy_async_smem();           // cp.async (generic proxy) writes -> tcgen05.mma (async proxy) reads
-                        tc_fence_after();
-                        if (lane == 0) {
-                            const uint32_t sa = smem_u32(smem + OFF_STAGE + s * STAGE_BYTES);
-                            const uint32_t dst = tmem + ocol(jj, h);
-                            const int nk = min(4, (D16 - blk * 64) >> 4);
-                            for (int kk = 0; kk < nk; kk++) {
-                                const uint64_t a_hi = make_smem_desc(sa + kk * 2048, 8192, 1024), a_lo = make_smem_desc(sa + PLANE_BYTES + kk * 2048, 8192, 1024);
-                                const uint64_t b = make_smem_desc(sb + blk * PANEL_B2 + kk * 32, 16, 1024);
-                                mma_bf16(dst, a_hi, b, idesc64, (blk | kk) ? 1u : 0u);      // [Fᵀ_hi·β_hi | Fᵀ_hi·β_lo]
-                                mma_bf16(dst, a_lo, b, idesc32, 1u);                        //  += Fᵀ_lo·β_hi
-                            }
-                            mma_commit(&ct.f_empty[s]);
-                        }
-                        __syncwarp();
-                        fcount++;
-                    }
-            }
-            if (lane == 0) mma_commit(&ct.o_full[obuf(jj)]);
-            if (lane == 0) TR(jj, 9);
-            __syncwarp();
-        };
-        for (int j = 0;; j++) {
-            PT(20);
-            wait_n(&ct.desc_full[j % NDESC], (uint32_t)(j / NDESC));
-            PT(24);
-            const Desc &d = desc_at(j);
-            const bool last = d.tile < 0;
-            if (!last) {
-                if (j >= 2) wait_n(&ct.s_empty[j & 1], (uint32_t)((j >> 1) - 1));
-                PT(25);
-                tc_fence_after();
-                if (d.D > 0) {
-                    const int nch = (d.D + CHUNK - 1) / CHUNK;
-                    const uint32_t idesc64 = make_idesc_bf16(128, 2 * P, 0, 0), idesc32 = make_idesc_bf16(128, P, 0, 0);
-                    for (int qh = 0; qh < NQH; qh++) {
-                        const int npq = min(4, NP - qh * 4);
-                        PT(20);
-                        wait_n(&ct.q_full, qcount);
-                        PT(26);
-                        fence_proxy_async_smem();
-                        for (int c = 0; c < nch; c++)
-                            for (int kp = 0; kp < npq; kp++) {
-                                const uint32_t s = fcount % NSTAGE;
-                                PT(20);
-                                wait_n(&ct.f_full[s], fcount / NSTAGE);
-                                PT(27);
-                                fence_proxy_async_smem();
-                                tc_fence_after();
-                                if (lane == 0) {
-                                    const uint32_t sa = smem_u32(smem + OFF_STAGE + s * STAGE_BYTES);
-                                    const uint32_t dst = tmem + TMEM_S + (uint32_t)(j & 1) * 128u + (uint32_t)c * 64u;
-#pragma unroll
-                                    for (int ks = 0; ks < 4; ks++) {
-                                        const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = make_smem_desc(sa + PLANE_BYTES + ks * 32, 16, 1024);
-                                        const uint64_t b = make_smem_desc(sq + kp * PANEL_B2 + ks * 32, 16, 1024);
-                                        mma_bf16(dst, a_hi, b, idesc64, (qh | kp | ks) ? 1u : 0u);      // [F_hi·Q_hi | F_hi·Q_lo]
-                                        mma_bf16(dst, a_lo, b, idesc32, 1u);                           //  += F_lo·Q_hi
-                                    }
-                                    mma_commit(&ct.f_empty[s]);
-                                }
-                                __syncwarp();
-                                fcount++;
-                            }
-                        if (lane == 0) mma_commit(&ct.q_empty);
-                        __syncwarp();
-                        qcount++;
-                    }
-                }
-                if (lane == 0) mma_commit(&ct.s_full[j & 1]);
-                if (lane == 0) TR(j, 3);
-                __syncwarp();
-            }
-            if (j >= 1) gemm2(j - 1);
-            if (last) break;
+            if (d.D > 0) gemm2_stages(j);                   // the workers run GEMM2(j) before GEMM1(j+1)
+            if (gt == 0) TR(j, 8);
+            named_bar(3, NGATHER);                          // every gather thread has read item j's row list
+            if (gt == 0) mbar_arrive(&ct.desc_free[j % NDESC]);
         }
     }
 
     // ---------------- teardown ----------------
-    tc_fence_before();
     __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 #ifdef EPI_PIPE_TIMERS
     if (tid == 0 && blockIdx.x < 256) { unsigned long long g; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g)); g_pipe_cta[blockIdx.x * 4 + 2] = g; }
 #endif
@@ -1062,7 +964,7 @@ cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st) {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev);
-        if (sms_cached <= 0) sms_cached = 148;
+        if (sms_cached <= 0) sms_cached = 132;
     }
     const int grid = tiles < sms_cached ? tiles : sms_cached;      // one persistent CTA per SM
     cudaError_t le = launch_pdl(kern, dim3((unsigned)grid), dim3(NT_ALL), (size_t)SMEM_ALLOC, st, a);

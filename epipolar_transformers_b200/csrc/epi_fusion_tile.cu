@@ -1,4 +1,4 @@
-// epi_fusion_tile.cu — tensor-core fused kernel (tcgen05 + TMEM), one CTA per 4x8 tile of reference pixels.
+// epi_fusion_tile.cu — tensor-core fused kernel (warpgroup MMA), one CTA per 4x8 tile of reference pixels.
 //
 // Same arithmetic as the warp kernel (epi_fusion_warp.cu) but restructured around the linearity of
 // bilinear sampling:      sim_k = Σ_t w_kt · (q · f[p_t])        out = Σ_p β_p · f[p],  β_p = Σ_{k,t→p} a_k w_kt
@@ -6,7 +6,7 @@
 // lines touch (D rows, gathered once per GEMM into shared memory):
 //   GEMM1  S[d, i]  = Σ_c F[d, c] · Q[i, c]        (M = 128 source pixels / chunk, N = 32 ref pixels, K = C)
 //   GEMM2  O[c, i]  = Σ_d F[d, c] · β[i, d]        (M = 128 channels,             N = 32 ref pixels, K = D)
-// Operands are bf16 (hi, lo) pairs, three MMAs per product (hi·hi + hi·lo + lo·hi, fp32 accumulate in TMEM):
+// Operands are bf16 (hi, lo) pairs, three MMAs per product (hi·hi + hi·lo + lo·hi, fp32 accumulate in registers):
 // ~2^-16 relative, inside the 1e-4 parity bar, where a single bf16/TF32 pass is not.  The gathered chunk
 // F[d][c] sits in 128B-swizzled panels and is the K-major A operand of GEMM1 and — the same bytes read
 // transposed — the MN-major A operand of GEMM2.  Between the GEMMs the CUDA cores interpolate the scores
@@ -30,14 +30,12 @@ constexpr int CHUNK = 128;        // union rows per MMA (M of GEMM1, K of GEMM2)
 constexpr int DMAX = 480;         // max union size handled in one pass (table row length)
 constexpr int NT = 512;           // worker threads
 constexpr int NWARP = NT / 32;
-constexpr int NT_ALL = NT + 32;   // + one warp that only issues tcgen05.mma (keeps the ~75-cycle/MMA issue off the workers' critical path)
 constexpr int MAXWORDS = 512;     // bitmap words: H*W <= 16384
 constexpr int MAXKPL = 4;         // samples per lane: K <= 128
 constexpr float FIX = 1073741824.0f;   // 2^30 fixed point for the β scatter
 
 constexpr uint32_t STAGE_BYTES = 65536;        // [hi: 2 panels x 16 KB][lo: 2 panels x 16 KB]
 constexpr uint32_t PANEL_A = 16384;            // 128 rows x 128 B
-constexpr uint32_t PANEL_B = 4096;             // 32 rows x 128 B
 constexpr uint32_t OFF_STAGE = 0;
 constexpr uint32_t OFF_QB = 2 * STAGE_BYTES;                       // 32 KB: Q hi/lo panels | β chunk double buffer | attn tile
 constexpr uint32_t OFF_TABLE = OFF_QB + 32768;                     // [32][DMAX] fp32 / int32
@@ -49,17 +47,9 @@ constexpr uint32_t OFF_MISC = OFF_ENDS + TM * 16;
 constexpr uint32_t SMEM_BYTES = OFF_MISC + 512;
 constexpr uint32_t SMEM_ALLOC = SMEM_BYTES + 1024;                 // 1024-byte alignment slack
 
-// Each accumulator is 64 columns wide: [0,32) = A·B_hi (+ A_lo·B_hi), [32,64) = A_hi·B_lo — the B operand is the
-// (hi, lo) pair stacked along N, so hi·hi and hi·lo share one MMA (2 instead of 3 MMAs per K step).
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t TMEM_S = 0;       // 4 chunks x 64 columns
-constexpr uint32_t TMEM_O = 256;     // 2 channel halves x 64 columns
 constexpr uint32_t PANEL_B2 = 8192;  // stacked B panel: 64 rows x 128 B (rows 0-31 hi, 32-63 lo)
 
 struct Misc {
-    uint64_t bar_stage[2];
-    uint64_t bar_all;
-    uint32_t tmem_base;
     int stack[16];
     int sp;
     int total;
@@ -69,15 +59,6 @@ struct Misc {
     uint16_t tpy[TM], tpx[TM];      // sector tiles: (y, x) of the tile's pixels, 0xFFFF = no pixel
 };
 static_assert(sizeof(Misc) <= 512, "Misc too large");
-
-// CTA-wide rendezvous for the warp-specialised sections: worker warps and the MMA warp run different loops, so the
-// barrier lives in ONE non-inlined function — every thread of the CTA arrives at the same bar.sync instruction.
-__device__ __noinline__ void cta_sync_named() { __syncthreads(); }
-
-__device__ __forceinline__ void bounded_wait(uint64_t *bar, uint32_t parity) {
-    for (uint32_t it = 0; !mbar_try_wait(bar, parity); ++it)
-        if (it > (1u << 26)) __trap();      // a protocol bug must abort the launch, never hang the GPU
-}
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo_elem, hi_elem);     // .x = lo_elem (low 16 bits)
@@ -108,7 +89,7 @@ __device__ unsigned long long g_tile_timers[16];
 #endif
 
 template <int KPL, bool SECTOR>
-__global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const FusionArgs a) {
+__global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs a) {
     extern __shared__ uint8_t smem_raw[];
     // keep the shared address space visible to the compiler: offset arithmetic on the array, no integer casts
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -126,7 +107,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
     const int total_tiles = a.N * tiles_per_item;
     int n = 0, ty0 = 0, tx0 = 0;                    // current tile (persistent CTA, dynamic tile scheduler)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const bool worker = warp < NWARP;               // warp NWARP only issues MMAs (and joins the CTA barriers)
+    const int wg = warp >> 2, t128 = tid & 127;     // warpgroup (MMA issue unit), thread within it
     const int nwords = (HW + 31) >> 5;
     const int NH = (C + 127) >> 7;                  // channel halves of 128
     const GeomCfg gc = a.geom;
@@ -139,18 +120,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
     auto pix_x = [&](int i) { return SECTOR ? (int)ms.tpx[i] : tx0 + (i & 7); };
     auto pix_ok = [&](int i) { return SECTOR ? ms.tpy[i] != 0xFFFFu : (ty0 + (i >> 3) < H && tx0 + (i & 7) < W); };
 
-    // ---------------- one-time setup ----------------
-    if (warp == 0) tmem_alloc(&ms.tmem_base, TMEM_COLS);
-    if (tid == 32) {
-        mbar_init(&ms.bar_stage[0], 1); mbar_init(&ms.bar_stage[1], 1); mbar_init(&ms.bar_all, 1);
-        mbar_fence_init();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = ms.tmem_base;
-    uint32_t n_stage = 0;      // stages issued so far (buffer = n_stage & 1), CTA-uniform
-    uint32_t n_all = 0;        // completions requested on bar_all
     int cur_n = -1;
 #ifdef EPI_TILE_TIMERS
     long long t_prev = clock64();
@@ -215,7 +184,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
         // mark every in-bounds tap of every sample of the group's pixels.  lane <-> pixel, warp <-> sample
         // (k = warp, warp+16, ...): the 32 lanes of one atomic belong to 32 different epipolar lines, so they
         // spread over several bitmap words instead of piling onto the one word a single line crosses.
-        if (worker) {
+        {
             const int i = lane;
             if (i >= g0 && i < g0 + gn && pix_ok(i)) {
                 for (int k = warp; k < K; k += NWARP) {
@@ -240,7 +209,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
             int incl = v;
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-            if (lane == 31 && worker) ms.warp_tot[warp] = incl;
+            if (lane == 31) ms.warp_tot[warp] = incl;
             __syncthreads();
             int base = 0;
             for (int w = 0; w < warp; w++) base += ms.warp_tot[w];
@@ -271,8 +240,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
         if (SECTOR) {
             // the reference map was split to bf16 planes [HW][C] by the staging kernel: 16-byte chunk copies
             const int C8 = C >> 3, J = NH * 16, jsh = NH == 1 ? 4 : 5;      // J is 16 or 32
-            if (worker)
-                for (int e = tid; e < 2 * TM * J; e += NT) {
+            for (int e = tid; e < 2 * TM * J; e += NT) {
                     const int plane = e >> (jsh + 5), rem = e & ((TM << jsh) - 1), i = rem >> jsh, j = rem & (J - 1);
                     uint4 v = make_uint4(0u, 0u, 0u, 0u);
                     if (i >= g0 && i < g0 + gn && pix_ok(i) && j < C8)
@@ -286,7 +254,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
             const bool ok = i >= g0 && i < g0 + gn && pix_ok(i);
             const float *rb = a.feat_ref + (int64_t)n * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
             const int64_t sc = a.ref_stride[1];
-            if (worker) {
+            {
                 float f[2][8];
 #pragma unroll
                 for (int it = 0; it < 2; it++) {                   // groups of 8 channels: cg = warp, warp + 16
@@ -340,78 +308,59 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
                 *reinterpret_cast<uint4 *>(stage + off) = v[it];
             }
         };
+        // Stage st is double-buffered (buffer st & 1) and consumed synchronously: every warpgroup waits for its MMAs on stage st
+        // before the barrier of stage st + 1, so the buffer is free again when stage st + 2 is stored.
         const int n_st = nch * NH;
-        auto acquire_stage = [&]() -> uint8_t * {
-            const uint32_t buf = n_stage & 1;
-            if (n_stage >= 2) bounded_wait(&ms.bar_stage[buf], ((n_stage >> 1) + 1) & 1);   // MMAs that read this buffer are done
-            return smem + OFF_STAGE + buf * STAGE_BYTES;
-        };
 
-        // ---------------- phase A: S = F·Qᵀ ----------------
-        if (worker) {
+        // ---------------- phase A: S = F·Qᵀ -> table[i][d] ----------------
+        // Warpgroup wg accumulates union rows c * 128 + (wg & 1) * 64 .. +63 of the chunks c with c % 2 == wg >> 1.
+        {
+            float sacc[2][16];
+#pragma unroll
+            for (int e = 0; e < 16; e++) { sacc[0][e] = 0.f; sacc[1][e] = 0.f; }
             uint4 v[8];
             if (n_st > 0) gather_load(v, 0, 0);
             for (int st = 0; st < n_st; st++) {
-                uint8_t *stage = acquire_stage();
+                const int c = st / NH, h = st % NH;
+                uint8_t *stage = smem + OFF_STAGE + (st & 1) * STAGE_BYTES;
                 gather_store(stage, v);
                 if (st + 1 < n_st) gather_load(v, (st + 1) / NH, (st + 1) % NH);
                 fence_proxy_async_smem();
-                tc_fence_before();
-                cta_sync_named();
-                n_stage++;
-            }
-        } else {
-            for (int st = 0; st < n_st; st++) {
-                const int c = st / NH, h = st % NH;
-                cta_sync_named();                                   // stage st is in shared memory
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t idesc64 = make_idesc_bf16(128, 2 * TM, 0, 0), idesc32 = make_idesc_bf16(128, TM, 0, 0);
-                    const uint32_t sa = smem_u32(smem + OFF_STAGE + (n_stage & 1) * STAGE_BYTES), sq = smem_u32(qb);
-                    const uint32_t dst = tmem + TMEM_S + c * 2 * TM;
+                __syncthreads();                                    // stage st is in shared memory
+                if ((c & 1) == (wg >> 1) && c * CHUNK + (wg & 1) * 64 < D) {
+                    const uint32_t sa = smem_u32(stage) + (uint32_t)(wg & 1) * 8192u, sq = smem_u32(qb);
+                    wg_fence();
 #pragma unroll
                     for (int ks = 0; ks < 8; ks++) {
                         const uint32_t ao = (ks >> 2) * PANEL_A + (ks & 3) * 32, bo = (h * 2 + (ks >> 2)) * PANEL_B2 + (ks & 3) * 32;
-                        const uint64_t a_hi = make_smem_desc(sa + ao, 16, 1024), a_lo = make_smem_desc(sa + 32768 + ao, 16, 1024);
-                        const uint64_t b = make_smem_desc(sq + bo, 16, 1024);
-                        mma_bf16(dst, a_hi, b, idesc64, (h | ks) ? 1u : 0u);      // [F_hi·Q_hi | F_hi·Q_lo]
-                        mma_bf16(dst, a_lo, b, idesc32, 1u);                      //  += F_lo·Q_hi (first 32 rows of the stacked panel)
+                        const uint64_t a_hi = make_smem_desc(sa + ao, 16, 1024), a_lo = desc_add(a_hi, 32768);
+                        const uint64_t b = make_smem_desc(sq + bo, 16, 1024), b_lo = desc_add(b, 4096);
+                        if (c >> 1) { wgmma_m64n32<0>(sacc[1], a_hi, b); wgmma_m64n32<0>(sacc[1], a_hi, b_lo); wgmma_m64n32<0>(sacc[1], a_lo, b); }
+                        else        { wgmma_m64n32<0>(sacc[0], a_hi, b); wgmma_m64n32<0>(sacc[0], a_hi, b_lo); wgmma_m64n32<0>(sacc[0], a_lo, b); }
                     }
-                    mma_commit(&ms.bar_stage[n_stage & 1]);
+                    wg_commit();
+                    wg_wait_all();
                 }
-                __syncwarp();
-                n_stage++;
             }
-        }
-        if (nch > 0) {
-            if (tid == NT) mma_commit(&ms.bar_all);
-            bounded_wait(&ms.bar_all, n_all & 1); n_all++;
-        }
-        tc_fence_after();
-
-        TMARK(2);
-        // ---------------- phase B1: scores TMEM -> table[i][d] ----------------
-        {
-            const int c = warp >> 2;
-            if (c < nch) {
-                float v[32], v2[32];
-                tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + TMEM_S + c * 2 * TM, v);
-                tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + TMEM_S + c * 2 * TM + TM, v2);
-                tmem_ld_wait();
-                const int d = c * CHUNK + (warp & 3) * 32 + lane;
-                if (d < D) {
+            TMARK(2);
 #pragma unroll
-                    for (int i = 0; i < TM; i++) table[i * DMAX + d] = v[i] + v2[i];
+            for (int q = 0; q < 2; q++) {
+                const int c = 2 * q + (wg >> 1);
+                if (c < nch) {
+#pragma unroll
+                    for (int e = 0; e < 16; e++) {
+                        const int d = c * CHUNK + (wg & 1) * 64 + acc_row(t128, e);
+                        if (d < D) table[acc_col(t128, e) * DMAX + d] = sacc[q][e];
+                    }
                 }
             }
         }
-        tc_fence_before();
         __syncthreads();
 
         TMARK(3);
         // ---------------- phase B2: interpolate scores, softmax over K, outputs, β scatter ----------------
         float *attn_tile = reinterpret_cast<float *>(qb);         // [K][32]; Q panels are dead now
-        if (worker) {
+        {
             // Each warp owns up to two pixels (i0, i0+16) and runs them interleaved for instruction-level
             // parallelism; lane <-> sample.  Tap ranks and weights are kept in registers for the β scatter.
             constexpr int PW = TM / NWARP;                         // 2
@@ -520,7 +469,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
         TMARK(4);
         if (a.attn) {       // flush the attention tile: 8-pixel row segments
             float *ab = a.attn + (size_t)n * K * HW;
-            for (int e = tid; worker && e < K * TM; e += NT) {
+            for (int e = tid; e < K * TM; e += NT) {
                 const int i = e & 31, k = e >> 5;
                 if (i >= g0 && i < g0 + gn && pix_ok(i)) ab[(size_t)k * HW + pix_y(i) * W + pix_x(i)] = attn_tile[k * TM + i];
             }
@@ -529,13 +478,17 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
 
         TMARK(5);
         // ---------------- phase C: Oᵀ = Fᵀ·βᵀ ----------------
-        if (worker) {
+        // Warpgroup wg accumulates channels (wg >> 1) * 128 + (wg & 1) * 64 .. +63 over all chunks.
+        float oacc[16];
+#pragma unroll
+        for (int e = 0; e < 16; e++) oacc[e] = 0.f;
+        {
             uint4 v[8];
             if (n_st > 0) gather_load(v, 0, 0);
             for (int st = 0; st < n_st; st++) {
                 const int c = st / NH, h = st % NH;
                 uint8_t *bb = qb + (c & 1) * 16384;
-                uint8_t *stage = acquire_stage();      // also proves the MMAs that read β buffer c&1 two chunks ago are done
+                uint8_t *stage = smem + OFF_STAGE + (st & 1) * STAGE_BYTES;
                 gather_store(stage, v);
                 if (st + 1 < n_st) gather_load(v, (st + 1) / NH, (st + 1) % NH);
                 if (h == 0) {
@@ -555,60 +508,39 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
                     *reinterpret_cast<uint4 *>(bb + 4096 + off) = lo;
                 }
                 fence_proxy_async_smem();
-                tc_fence_before();
-                cta_sync_named();
-                n_stage++;
-            }
-        } else {
-            for (int st = 0; st < n_st; st++) {
-                const int c = st / NH, h = st % NH;
-                cta_sync_named();
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t idesc64 = make_idesc_bf16(128, 2 * TM, 1, 0), idesc32 = make_idesc_bf16(128, TM, 1, 0);
-                    const uint32_t sa = smem_u32(smem + OFF_STAGE + (n_stage & 1) * STAGE_BYTES), sb = smem_u32(qb + (c & 1) * 16384);
-                    const uint32_t dst = tmem + TMEM_O + h * 2 * TM;
+                __syncthreads();
+                if (h == (wg >> 1)) {
+                    const uint32_t sa = smem_u32(stage) + (uint32_t)(wg & 1) * PANEL_A, sb = smem_u32(bb);
+                    wg_fence();
 #pragma unroll
                     for (int ks = 0; ks < 8; ks++) {
                         const uint32_t ao = ks * 2048, bo = (ks >> 2) * PANEL_B2 + (ks & 3) * 32;
-                        const uint64_t a_hi = make_smem_desc(sa + ao, PANEL_A, 1024), a_lo = make_smem_desc(sa + 32768 + ao, PANEL_A, 1024);
-                        const uint64_t b = make_smem_desc(sb + bo, 16, 1024);
-                        mma_bf16(dst, a_hi, b, idesc64, (c | ks) ? 1u : 0u);      // [Fᵀ_hi·β_hi | Fᵀ_hi·β_lo]
-                        mma_bf16(dst, a_lo, b, idesc32, 1u);                      //  += Fᵀ_lo·β_hi
+                        const uint64_t a_hi = make_smem_desc(sa + ao, PANEL_A, 1024), a_lo = desc_add(a_hi, 32768);
+                        const uint64_t b = make_smem_desc(sb + bo, 16, 1024), b_lo = desc_add(b, 4096);
+                        wgmma_m64n32<1>(oacc, a_hi, b); wgmma_m64n32<1>(oacc, a_hi, b_lo); wgmma_m64n32<1>(oacc, a_lo, b);
                     }
-                    mma_commit(&ms.bar_stage[n_stage & 1]);
+                    wg_commit();
+                    wg_wait_all();
                 }
-                __syncwarp();
-                n_stage++;
             }
         }
-        if (nch > 0) {
-            if (tid == NT) mma_commit(&ms.bar_all);
-            bounded_wait(&ms.bar_all, n_all & 1); n_all++;
-        }
-        tc_fence_after();
+        __syncthreads();                                            // every warpgroup's MMAs are done with the stages
 
         TMARK(6);
-        // ---------------- phase D: fused feature TMEM -> shared (transposed) -> global ----------------
+        // ---------------- phase D: fused feature registers -> shared (transposed) -> global ----------------
         {
             // o_tile[i][ch] in the (now idle) stage buffers; row stride 260 floats keeps float4 alignment
             float *o_tile = reinterpret_cast<float *>(smem + OFF_STAGE);
             constexpr int OS = 260;
-            const int h = warp >> 2;
-            if (h < NH) {
-                float v[32], v2[32];
-                tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + TMEM_O + h * 2 * TM, v);
-                tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + TMEM_O + h * 2 * TM + TM, v2);
-                tmem_ld_wait();
-                const int ch = h * 128 + (warp & 3) * 32 + lane;
+            if ((wg >> 1) < NH) {
+                const int cb = (wg >> 1) * 128 + (wg & 1) * 64;
 #pragma unroll
-                for (int i = 0; i < TM; i++) o_tile[i * OS + ch] = nch ? v[i] + v2[i] : 0.f;   // nch==0: every sample masked, zero vectors
+                for (int e = 0; e < 16; e++) o_tile[acc_col(t128, e) * OS + cb + acc_row(t128, e)] = nch ? oacc[e] : 0.f;   // nch==0: every sample masked, zero vectors
             }
-            tc_fence_before();
             __syncthreads();
             if (a.out_hi) {
                 // bf16 (hi, lo) planes [N][HW][C]: the A operand of the z-projection GEMM; one 16-byte store per lane
-                for (int i = g0 + warp; worker && i < g0 + gn; i += NWARP) {
+                for (int i = g0 + warp; i < g0 + gn; i += NWARP) {
                     if (!pix_ok(i) || lane * 8 >= C) continue;
                     float f[8];
                     *reinterpret_cast<float4 *>(f) = *reinterpret_cast<const float4 *>(o_tile + i * OS + lane * 8);
@@ -625,7 +557,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
                 const bool ok = i >= g0 && i < g0 + gn && pix_ok(i);
                 float *ob = a.out + (int64_t)n * a.out_stride[0] + (int64_t)pix_y(i) * a.out_stride[2] + (int64_t)pix_x(i) * a.out_stride[3];
                 const float *rb = a.feat_ref + (int64_t)n * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
-                if (ok && worker)
+                if (ok)
                     for (int ch = warp; ch < C; ch += NWARP) {
                         float o = o_tile[i * OS + ch];
                         if (a.add_ref) o += __ldg(rb + ch * a.ref_stride[1]);
@@ -633,7 +565,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
                     }
             } else {
                 // channels-last: lane <-> channel
-                for (int i = g0 + warp; worker && i < g0 + gn; i += NWARP) {
+                for (int i = g0 + warp; i < g0 + gn; i += NWARP) {
                     if (!pix_ok(i)) continue;
                     float *ob = a.out + (int64_t)n * a.out_stride[0] + (int64_t)pix_y(i) * a.out_stride[2] + (int64_t)pix_x(i) * a.out_stride[3];
                     const float *rb = a.feat_ref + (int64_t)n * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
@@ -645,7 +577,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
                 }
             }
         }
-        tc_fence_before();
         TMARK(7);
 #ifdef EPI_TILE_TIMERS
         if (tid == 0) atomicAdd(&g_tile_timers[8], 1ull);
@@ -656,8 +587,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_tile_kernel(const Fusion
     tile = ms.next_tile;
     __syncthreads();
   }
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 bool fusion_tile_supported(const FusionArgs &a) {
@@ -682,11 +611,11 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
     else        kern = kpl <= 1 ? epi_fusion_tile_kernel<1, false> : (kpl <= 2 ? epi_fusion_tile_kernel<2, false> : epi_fusion_tile_kernel<4, false>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_ALLOC);
     if (e != cudaSuccess) return e;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = a.tile_counter ? (tiles < sms ? tiles : sms) : tiles;     // one persistent CTA per SM
-    kern<<<grid, NT_ALL, SMEM_ALLOC, st>>>(a);
+    kern<<<grid, NT, SMEM_ALLOC, st>>>(a);
     return cudaGetLastError();
 }
 

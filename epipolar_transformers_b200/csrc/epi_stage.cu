@@ -19,8 +19,7 @@ namespace stg {
 constexpr int NT = 256;
 constexpr int NBIN = 4096;
 constexpr int SMALL = 32;
-constexpr int TC = 64, TPX = 64, TPITCH = 65;       // layout-staging tile: 64 channels x 64 pixels (measured best: 16.4 us at cfg2 vs 19.4 us
-                                                    // for 64 x 128 and 22.4 us for 32 x 128 — profiles/stage_tile_sweep_r2.md)
+constexpr int TC = 64, TPX = 64, TPITCH = 65;       // layout-staging tile: 64 channels x 64 pixels
 
 // Monotone pseudo-angle of (u, v) in [-2, 2] (diamond angle): same ordering as atan2(v, u) at the price of one division.
 __device__ __forceinline__ float pseudo_angle(float u, float v) {
@@ -510,7 +509,7 @@ cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const fl
     if (!sms_cached) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms_cached <= 0) sms_cached = 148;
+        if (cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms_cached <= 0) sms_cached = 132;
     }
     s.persist = 0;
     if ((H * W) % stg::TPX == 0 && C % stg::TC == 0 && whole(ref, ref_stride) && whole(src, src_stride)) {

@@ -1,8 +1,8 @@
-// epi_umma.cuh — hand-written sm_100a plumbing for the tensor-core path: mbarrier, TMEM
-// allocation, tcgen05.mma / commit / ld, shared-memory matrix descriptors and the 128-byte
+// epi_umma.cuh — hand-written sm_90a plumbing for the tensor-core path: mbarrier, warpgroup
+// MMA (wgmma) with register accumulators, shared-memory matrix descriptors and the 128-byte
 // swizzle that the operand staging code must write.  Inline PTX only (no CUTLASS).
 //
-// Operand conventions used by the fusion kernel (bf16 operands, fp32 accumulate in TMEM):
+// Operand conventions used by the fusion kernel (bf16 operands, fp32 accumulate in registers):
 //   "panel"  = ROWS x 64 bf16 (one 128-byte row per matrix row), rows in 8-row / 1024-byte swizzle
 //              atoms (Swizzle<3,4,3>: 16-byte chunk index ^= row % 8).  A matrix with more than 64
 //              columns is a sequence of panels `panel_stride` bytes apart.
@@ -49,7 +49,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {}
 }
 
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma / TMA reads)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- 16-byte asynchronous copies global -> shared (LDGSTS), zero-fill when !valid ---------------------------
@@ -72,35 +72,41 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
                  : "memory");
 }
 
-// ---- TMEM ------------------------------------------------------------------------------------
-// Executed by ONE full warp; writes the allocated base address (lane<<16 | column) to *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols /* power of two >= 32 */) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---- warpgroup MMA (wgmma) -------------------------------------------------------------------------
+// All 128 threads of a warpgroup issue each call; the fp32 accumulator lives in their registers.  Fragment of
+// m64nNk16 (d[N/2] per thread): thread t of the warpgroup holds rows acc_row(t, e) and columns acc_col(t, e).
+__device__ __forceinline__ int acc_row(int t, int e) { return ((t >> 5) << 4) + ((t & 31) >> 2) + ((e >> 1) & 1) * 8; }
+__device__ __forceinline__ int acc_col(int t, int e) { return ((e >> 2) << 3) + ((t & 3) << 1) + (e & 1); }
 
-// 32 lanes x 32 consecutive fp32 columns: thread `lane` of warp w receives D[32*(w%4)+lane][col..col+31].
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float *v) {
-    uint32_t *r = reinterpret_cast<uint32_t *>(v);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D (+)= A·B, bf16 operands from shared memory, D always accumulates (callers zero it first).
+// TRANS_A = 0: A K-major; 1: A MN-major (the same panel bytes read transposed).  B is K-major.
+template <int TRANS_A>
+__device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %18, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "n"(TRANS_A)
         : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int TRANS_A>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %66, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "n"(TRANS_A)
+        : "memory");
+}
 
 // ---- descriptors -------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type 2), descriptor version 1 (sm_100).
+// Shared-memory matrix descriptor, 128-byte swizzle (layout type 1, bits 62-63).
 //   K-major : sbo = bytes between 8-row groups (1024 for dense panels), lbo ignored (1).
 //   MN-major: lbo = bytes between 64-element MN groups (panel stride), sbo = bytes between 8-row K groups.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -108,35 +114,11 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
     d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;          // version
-    d |= (uint64_t)2 << 61;          // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;          // SWIZZLE_128B
     return d;
 }
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32, dense.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4)                      // c_format  = F32
-           | (1u << 7)                    // a_format  = BF16
-           | (1u << 10)                   // b_format  = BF16
-           | ((uint32_t)a_mn_major << 15) // a_major
-           | ((uint32_t)b_mn_major << 16) // b_major
-           | ((uint32_t)(N >> 3) << 17)   // n_dim
-           | ((uint32_t)(M >> 4) << 24);  // m_dim
-}
-
-// D[tmem] (+)= A[smem] · B[smem]; issued by ONE thread.
-__device__ __forceinline__ void mma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// All previously issued MMAs of this thread arrive on the mbarrier when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+// descriptor of the panel `bytes` further on (16-byte units in the start-address field)
+__device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
 // ---- operand staging ----------------------------------------------------------------------------
 // Byte offset of element (row, col) inside a swizzled panel set (col over all panels).

@@ -1,8 +1,9 @@
-// epi_umma_selftest.cu — one-CTA GEMM that exercises exactly the tcgen05 operand forms the fusion
-// kernel uses, so descriptor / swizzle / TMEM-mapping mistakes show up as a plain matrix mismatch:
+// epi_umma_selftest.cu — one-CTA GEMM that exercises exactly the wgmma operand forms the fusion
+// kernels use, so descriptor / swizzle / fragment-mapping mistakes show up as a plain matrix mismatch:
 //   mode 0:  D[128 x N] = A[128 x K] · B[N x K]ᵀ          (A, B K-major panels)          -> S = F·Qᵀ
 //   mode 1:  D[128 x N] = Atᵀ[128 x Kd] · B[N x Kd]ᵀ      (A MN-major: At is [Kd x 128])  -> Oᵀ = Fᵀ·βᵀ
 // split=1 stages every operand as a bf16 (hi, lo) pair and issues hi·hi + hi·lo + lo·hi.
+// One warpgroup computes the product in m64n32 blocks (two 64-row halves, N/32 column blocks), like the fusion kernels.
 #include "../../include/epipolar_b200.h"
 #include "epi_umma.cuh"
 
@@ -12,18 +13,14 @@ using namespace umma;
 __global__ void __launch_bounds__(128) umma_selftest_kernel(int mode, const float *__restrict__ A, const float *__restrict__ B,
                                                             float *__restrict__ D, int N, int K, int split) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     // A region: (hi, lo) x panels.  mode 0: K/64 panels of 128 rows.  mode 1: 2 panels of K rows.
     const uint32_t a_rows = mode == 0 ? 128 : K, a_cols = mode == 0 ? K : 128;
     const uint32_t a_panel = a_rows * 128, a_bytes = a_panel * (a_cols / 64);
     const uint32_t b_panel = (uint32_t)N * 128, b_bytes = b_panel * (K / 64);
     uint8_t *a_hi = smem, *a_lo = smem + a_bytes, *b_hi = smem + 2 * a_bytes, *b_lo = b_hi + b_bytes;
 
-    if (warp == 0) tmem_alloc(&tmem_base_s, 256);
-    if (tid == 0) { mbar_init(&bar, 1); mbar_fence_init(); }
     for (uint32_t idx = tid; idx < a_rows * a_cols; idx += blockDim.x) {
         uint32_t r = idx / a_cols, c = idx % a_cols;
         __nv_bfloat16 hi, lo;
@@ -41,39 +38,31 @@ __global__ void __launch_bounds__(128) umma_selftest_kernel(int mode, const floa
         *reinterpret_cast<__nv_bfloat16 *>(b_lo + off) = lo;
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_s;
 
-    if (tid == 0) {
-        const uint32_t idesc = make_idesc_bf16(128, N, mode == 1, 0);
-        uint32_t acc = 0;
-        for (int ks = 0; ks < K / 16; ks++) {
-            for (int term = 0; term < (split ? 3 : 1); term++) {
-                const uint8_t *ap = term == 2 ? a_lo : a_hi;
-                const uint8_t *bp = term == 1 ? b_lo : b_hi;
-                uint64_t ad, bd;
-                if (mode == 0) ad = make_smem_desc(smem_u32(ap) + (ks / 4) * a_panel + (ks % 4) * 32, 16, 1024);
-                else           ad = make_smem_desc(smem_u32(ap) + ks * 2048, a_panel, 1024);
-                bd = make_smem_desc(smem_u32(bp) + (ks / 4) * b_panel + (ks % 4) * 32, 16, 1024);
-                mma_bf16(tmem, ad, bd, idesc, acc);
-                acc = 1;
+    for (int nb = 0; nb * 32 < N; nb++)
+        for (int mh = 0; mh < 2; mh++) {
+            float acc[16];
+#pragma unroll
+            for (int e = 0; e < 16; e++) acc[e] = 0.f;
+            wg_fence();
+            for (int ks = 0; ks < K / 16; ks++) {
+                for (int term = 0; term < (split ? 3 : 1); term++) {
+                    const uint8_t *ap = term == 2 ? a_lo : a_hi;
+                    const uint8_t *bp = term == 1 ? b_lo : b_hi;
+                    const uint64_t bd = make_smem_desc(smem_u32(bp) + (ks / 4) * b_panel + (ks % 4) * 32 + nb * 4096, 16, 1024);
+                    if (mode == 0) wgmma_m64n32<0>(acc, make_smem_desc(smem_u32(ap) + (ks / 4) * a_panel + (ks % 4) * 32 + mh * 8192, 16, 1024), bd);
+                    else           wgmma_m64n32<1>(acc, make_smem_desc(smem_u32(ap) + mh * a_panel + ks * 2048, a_panel, 1024), bd);
+                }
+            }
+            wg_commit();
+            wg_wait_all();
+#pragma unroll
+            for (int e = 0; e < 16; e++) {
+                const int col = nb * 32 + acc_col(tid, e);
+                if (col < N) D[(size_t)(mh * 64 + acc_row(tid, e)) * N + col] = acc[e];
             }
         }
-        mma_commit(&bar);
-    }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    for (int c0 = 0; c0 < N; c0 += 32) {
-        float v[32];
-        tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + c0, v);
-        tmem_ld_wait();
-        for (int j = 0; j < 32 && c0 + j < N; j++) D[(size_t)(warp * 32 + lane) * N + c0 + j] = v[j];
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
 }  // namespace epi
@@ -81,125 +70,9 @@ __global__ void __launch_bounds__(128) umma_selftest_kernel(int mode, const floa
 extern "C" int epi_umma_selftest(int mode, const float *A, const float *B, float *D, int N, int K, int split, void *stream) {
     if (!A || !B || !D || N < 16 || N > 256 || N % 16 || K < 64 || K > 256 || K % 64 || (mode != 0 && mode != 1)) return EPI_EINVAL;
     const size_t a_bytes = 128 * (size_t)K * 2, b_bytes = (size_t)N * K * 2;
-    const size_t smem = 2 * a_bytes + 2 * b_bytes + 1024;
+    const size_t smem = 2 * a_bytes + 2 * b_bytes + 1024 + 4096;      // + slack: an n32 block may read past N = 16 rows
     cudaError_t e = cudaFuncSetAttribute(epi::umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return EPI_ECUDA;
     epi::umma_selftest_kernel<<<1, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(mode, A, B, D, N, K, split);
     return cudaGetLastError() == cudaSuccess ? EPI_OK : EPI_ECUDA;
 }
-
-// The micro-benchmark and the M=64 probe below are developer tools: they are compiled into libepipolar_b200_timers.so only
-// (`python -m epipolar_transformers_b200.build --timers`), never into the product library.
-#ifdef EPI_PIPE_TIMERS
-// ---- micro-benchmark: cycles per tcgen05.mma for M=128, K=16 bf16, N in {32..256}, A K-major or MN-major ----
-namespace epi {
-using namespace umma;
-__global__ void __launch_bounds__(128) umma_bench_kernel(int M, int N, int reps, int mn_major, long long *out) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
-    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int tid = threadIdx.x, warp = tid >> 5;
-    for (int i = tid; i < (65536 + 32768) / 4; i += 128) reinterpret_cast<uint32_t *>(smem)[i] = 0x3f803f80u;
-    if (warp == 0) tmem_alloc(&tmem_base_s, 256);
-    if (tid == 0) { mbar_init(&bar, 1); mbar_fence_init(); }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_s;
-    if (tid == 0) {
-        const uint32_t idesc = make_idesc_bf16(M, N, mn_major, 0);
-        const uint32_t sa = smem_u32(smem), sb = sa + 65536;
-        long long t0 = clock64();
-        for (int r = 0; r < reps; r++) {
-            const int ks = r & 7;
-            const uint64_t ad = mn_major ? make_smem_desc(sa + ks * 2048, 16384, 1024) : make_smem_desc(sa + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024);
-            const uint64_t bd = make_smem_desc(sb + (ks & 3) * 32, 16, 1024);
-            mma_bf16(tmem, ad, bd, idesc, 1u);
-        }
-        long long t1 = clock64();
-        mma_commit(&bar);
-        out[1] = t1 - t0;
-        out[2] = t0;
-    }
-    mbar_wait(&bar, 0);
-    if (tid == 0) out[0] = clock64() - out[2];
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
-}
-}  // namespace epi
-
-extern "C" int epi_umma_bench(int M, int N, int reps, int mn_major, long long *out_dev, void *stream) {
-    const size_t smem = 65536 + 32768 + 1024;
-    cudaFuncSetAttribute(epi::umma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    epi::umma_bench_kernel<<<1, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(M, N, reps, mn_major, out_dev);
-    return cudaGetLastError() == cudaSuccess ? 0 : -3;
-}
-
-// ---- M=64 probe: D[64 x N] = At[K x 64]^T · B[N x K]^T (A MN-major, one 64-wide panel) or A K-major [64 x K];
-//      dumps all 128 TMEM lanes x N columns so the host can recover the lane mapping of M=64 accumulators. ----
-namespace epi {
-using namespace umma;
-__global__ void __launch_bounds__(128) umma_m64_probe_kernel(int mn_major, const float *__restrict__ A, const float *__restrict__ B,
-                                                             float *__restrict__ Dall, int N, int K) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
-    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // A: mn_major: rows = k (K of them), 64 columns (m)  -> one panel of K rows.   K-major: rows = m (64), K columns -> K/64 panels of 64 rows
-    const uint32_t a_rows = mn_major ? K : 64, a_cols = mn_major ? 64 : K;
-    const uint32_t a_panel = a_rows * 128;
-    const uint32_t b_panel = (uint32_t)N * 128;
-    uint8_t *a_s = smem, *b_s = smem + 32768;
-    for (uint32_t i = tid; i < 32768u / 4; i += 128) reinterpret_cast<uint32_t *>(smem)[i] = 0u;
-    __syncthreads();
-    if (warp == 0) tmem_alloc(&tmem_base_s, 256);
-    if (tid == 0) { mbar_init(&bar, 1); mbar_fence_init(); }
-    for (uint32_t idx = tid; idx < a_rows * a_cols; idx += 128) {
-        uint32_t r = idx / a_cols, c = idx % a_cols;
-        *reinterpret_cast<__nv_bfloat16 *>(a_s + panel_offset(r, c, a_panel)) = __float2bfloat16_rn(A[idx]);
-    }
-    for (uint32_t idx = tid; idx < (uint32_t)N * K; idx += 128) {
-        uint32_t r = idx / K, c = idx % K;
-        *reinterpret_cast<__nv_bfloat16 *>(b_s + panel_offset(r, c, b_panel)) = __float2bfloat16_rn(B[idx]);
-    }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_s;
-    // zero the accumulator region first so untouched lanes read as exact zeros
-    if (tid == 0) {
-        const uint32_t idesc = make_idesc_bf16(64, N, mn_major, 0);
-        for (int ks = 0; ks < K / 16; ks++) {
-            const uint64_t ad = mn_major ? make_smem_desc(smem_u32(a_s) + ks * 2048, 16, 1024)
-                                         : make_smem_desc(smem_u32(a_s) + (ks / 4) * a_panel + (ks % 4) * 32, 16, 1024);
-            const uint64_t bd = make_smem_desc(smem_u32(b_s) + (ks / 4) * b_panel + (ks % 4) * 32, 16, 1024);
-            mma_bf16(tmem, ad, bd, idesc, ks ? 1u : 0u);
-        }
-        mma_commit(&bar);
-    }
-    mbar_wait(&bar, 0);
-    tc_fence_after();
-    for (int c0 = 0; c0 < N; c0 += 32) {
-        float v[32];
-        tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + c0, v);
-        tmem_ld_wait();
-        for (int j = 0; j < 32 && c0 + j < N; j++) Dall[(size_t)(warp * 32 + lane) * N + c0 + j] = v[j];
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
-}
-}  // namespace epi
-
-extern "C" int epi_umma_m64_probe(int mn_major, const float *A, const float *B, float *Dall, int N, int K, void *stream) {
-    const size_t smem = 32768 + 32768 + 1024;
-    cudaFuncSetAttribute(epi::umma_m64_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    epi::umma_m64_probe_kernel<<<1, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(mn_major, A, B, Dall, N, K);
-    return cudaGetLastError() == cudaSuccess ? 0 : -3;
-}
-#endif  // EPI_PIPE_TIMERS

@@ -1,17 +1,17 @@
-// epi_zgemm.cu — z-projection epilogue on the tensor cores (tcgen05 + TMEM).
+// epi_zgemm.cu — z-projection epilogue on the tensor cores (TMA + warpgroup MMA).
 //
 //   y[n,o,p] = Σ_c Wf[o,c]·x[n,c,p] + bf[o]  (+ x[n,o,p] if ZRESIDUAL)  (+ feat_ref[n,o,p] for the caller's residual)
 // restates  finalout = bn(z(out)) [+ out]   /root/reference/modeling/layers/epipolar.py:249-253 (eval-mode BN folded
 // into Wf, bf by epi_fold_z_bn_f32) and  ret + feat   /root/reference/modeling/backbones/resnet.py:388.
 //
-// One CTA per 128 pixels and block of 128 output channels (blockIdx.y); small CTAs (69 KB, one K panel in flight) so that three
+// One CTA per 128 pixels and block of 128 output channels (blockIdx.y); small CTAs (69 KB, one K panel in flight) so that several
 // are resident per SM and their load / MMA / store phases overlap each other:
 // D[128 px, C out] = X[128 px, C]·Wfᵀ with X supplied by the fusion kernel as bf16
 // (hi, lo) planes [N·HW, C] (K-major rows) and Wf split to (hi, lo) while it is staged.  Three MMAs per
-// product (hi·hi + hi·lo + lo·hi), fp32 accumulation in TMEM (M=128, N=C<=256), K streamed in 64-channel
-// panels through a double-buffered shared-memory ring — the X panels arrive by TMA (cp.async.bulk.tensor.2d with the
-// 128-byte swizzle the UMMA descriptors expect, completion on an mbarrier); the epilogue adds bias/residuals and writes NCHW
-// (a warp's lanes are 32 consecutive pixels, so every store instruction is one 128-byte line per channel).
+// product (hi·hi + hi·lo + lo·hi), fp32 accumulation in registers (two warpgroups of M=64, N=128), K streamed in 64-channel
+// panels — the X and W panels arrive by TMA (cp.async.bulk.tensor.2d with the 128-byte swizzle the wgmma descriptors expect,
+// completion on an mbarrier); the epilogue adds bias/residuals and writes NCHW (a warp's lanes are 32 consecutive pixels, so
+// every store instruction is one 128-byte line per channel).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -32,7 +32,7 @@ constexpr uint32_t STAGE = 2 * A_PLANE + 2 * B_PLANE;   // 64 KB: one K panel of
 constexpr int OT = 132;                             // epilogue tile pitch (floats)
 constexpr uint32_t TILE_BYTES = NB * OT * 4;        // 67 584 B: the epilogue tile re-uses the stage
 constexpr uint32_t BUF_BYTES = TILE_BYTES > STAGE ? TILE_BYTES : STAGE;
-constexpr uint32_t SMEM_ALLOC = BUF_BYTES + 1024 + 128;     // ~69 KB: three CTAs per SM overlap each other's load / MMA / store phases
+constexpr uint32_t SMEM_ALLOC = BUF_BYTES + 1024 + 128;     // ~69 KB: up to three CTAs per SM by shared memory (two by registers)
 
 // 2-D tiled TMA load of a [128 rows x 64 bf16] box into a swizzled panel, completion counted on `bar`
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tmap, int c0, int c1, uint64_t *bar) {
@@ -50,8 +50,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
     using namespace zg;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + BUF_BYTES);       // [0] panel landed (TMA), [1] MMAs done with the panel, [2] all MMAs done
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + BUF_BYTES + 64);
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + BUF_BYTES);        // K panel landed (TMA)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int C = z.C, HW = z.HW, W = z.W;
     const int tiles = (HW + 127) / 128;
@@ -63,7 +62,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
     pdl_launch_dependents();
     // The bias and the caller's residual (inputs of the whole forward, not products of the previous launches) are fetched into
     // registers FIRST: their latency is paid under the previous kernel's tail and this kernel's main loop instead of once per
-    // output row of the epilogue (16 dependent round trips per warp — 30 % of the kernel's stall samples before the hoist).
+    // output row of the epilogue (16 dependent round trips per warp).
     const bool addr = z.ref && z.add_ref;
     const bool vec = (z.y_stride[3] == 1) && (z.y_stride[2] == W) && (HW % 4 == 0) && (z.y_stride[1] % 4 == 0) && (z.y_stride[0] % 4 == 0) &&
                      ((reinterpret_cast<uintptr_t>(z.y) & 15) == 0) &&
@@ -83,68 +82,61 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
                 res[k] = __ldcs(reinterpret_cast<const float4 *>(z.ref + (int64_t)n * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p));
         }
     }
-    if (warp == 0) tmem_alloc(tmem_slot, NB);
-    if (tid == 32) { for (int i = 0; i < 3; i++) mbar_init(&bars[i], 1); mbar_fence_init(); }
+    if (tid == 32) { mbar_init(bar, 1); mbar_fence_init(); }
     if (tid == 64) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_lo) : "memory");
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_wait();                                        // the fused kernel's feature planes
 
-    // One thread drives the main loop: TMA load of a K panel (A: 128 pixel rows x 64 channels of the (hi, lo) planes of x; B: NB output
-    // rows x 64 input channels of the (hi, lo) planes of Wf), three MMAs per 16-channel step, commit, next panel.
-    if (tid == 0) {
+    // Main loop: thread 0 issues the TMA loads of a K panel (A: 128 pixel rows x 64 channels of the (hi, lo) planes of x; B: NB output
+    // rows x 64 input channels of the (hi, lo) planes of Wf); warpgroup wg multiplies pixel rows 64 wg .. +63, three MMAs per
+    // 16-channel step, and waits for them before the panel is reloaded.  Output columns >= CO are computed and discarded.
+    const int wg = warp >> 2, t128 = tid & 127;
+    float acc[64];
+#pragma unroll
+    for (int e = 0; e < 64; e++) acc[e] = 0.f;
+    {
         const uint32_t wrows = (uint32_t)(C < NB ? C : NB);            // W box rows (the tensor map's box)
-        const uint32_t idesc = make_idesc_bf16(128, (uint32_t)((CO + 15) & ~15), 0, 0);
         for (int q = 0; q < nq; q++) {
-            if (q > 0) for (uint32_t it = 0; !mbar_try_wait(&bars[1], (q - 1) & 1); ++it) if (it > (1u << 24)) __trap();
-            mbar_arrive_expect_tx(&bars[0], 2 * A_PLANE + 2 * wrows * 128u);
-            tma_load_2d(smem, &tm_hi, q * 64, n * HW + p0, &bars[0]);
-            tma_load_2d(smem + A_PLANE, &tm_lo, q * 64, n * HW + p0, &bars[0]);
-            tma_load_2d(smem + 2 * A_PLANE, &tw_hi, q * 64, oc0, &bars[0]);
-            tma_load_2d(smem + 2 * A_PLANE + B_PLANE, &tw_lo, q * 64, oc0, &bars[0]);
-            for (uint32_t it = 0; !mbar_try_wait(&bars[0], q & 1); ++it) if (it > (1u << 24)) __trap();
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem), sb = sa + 2 * A_PLANE;
+            if (tid == 0) {
+                mbar_arrive_expect_tx(bar, 2 * A_PLANE + 2 * wrows * 128u);
+                tma_load_2d(smem, &tm_hi, q * 64, n * HW + p0, bar);
+                tma_load_2d(smem + A_PLANE, &tm_lo, q * 64, n * HW + p0, bar);
+                tma_load_2d(smem + 2 * A_PLANE, &tw_hi, q * 64, oc0, bar);
+                tma_load_2d(smem + 2 * A_PLANE + B_PLANE, &tw_lo, q * 64, oc0, bar);
+            }
+            for (uint32_t it = 0; !mbar_try_wait(bar, q & 1); ++it) if (it > (1u << 24)) __trap();
+            const uint32_t sa = smem_u32(smem) + (uint32_t)wg * 8192u, sb = smem_u32(smem) + 2 * A_PLANE;
+            wg_fence();
 #pragma unroll
             for (int ks = 0; ks < 4; ks++) {
-                const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = make_smem_desc(sa + A_PLANE + ks * 32, 16, 1024);
-                const uint64_t b_hi = make_smem_desc(sb + ks * 32, 16, 1024), b_lo = make_smem_desc(sb + B_PLANE + ks * 32, 16, 1024);
-                mma_bf16(tmem, a_hi, b_hi, idesc, (q | ks) ? 1u : 0u);
-                mma_bf16(tmem, a_hi, b_lo, idesc, 1u);
-                mma_bf16(tmem, a_lo, b_hi, idesc, 1u);
+                const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = desc_add(a_hi, A_PLANE);
+                const uint64_t b_hi = make_smem_desc(sb + ks * 32, 16, 1024), b_lo = desc_add(b_hi, B_PLANE);
+                wgmma_m64n128<0>(acc, a_hi, b_hi);
+                wgmma_m64n128<0>(acc, a_hi, b_lo);
+                wgmma_m64n128<0>(acc, a_lo, b_hi);
             }
-            mma_commit(&bars[1]);
+            wg_commit();
+            wg_wait_all();
+            __syncthreads();                           // both warpgroups are done with the panel
         }
-        mma_commit(&bars[2]);
     }
-    for (uint32_t it = 0; !mbar_try_wait(&bars[2], 0); ++it) if (it > (1u << 24)) __trap();
-    tc_fence_after();
 
     // ---- epilogue ------------------------------------------------------------------------------------------------
-    // phase 1 (thread <-> pixel = TMEM lane, 8 warps = 4 lane quadrants x 2 channel groups): accumulator -> shared tile
-    //   [channel][128 pixels] (the operand stages are free now).  The ZRESIDUAL needs no pass: the staged weight is Wf + I;
+    // phase 1 (accumulator fragments): registers -> shared tile [channel][128 pixels] (the operand stage is free now).
+    //   The ZRESIDUAL needs no pass: the staged weight is Wf + I;
     // phase 2 (warp <-> channel row, lane <-> 4 consecutive pixels): + bias + caller residual, 512-byte row segments of the NCHW output
     //   per warp instruction.  Falls back to per-element addressing for strides that are not pixel-contiguous.
     float *otile = reinterpret_cast<float *>(smem);            // [NB][132] fp32 over the (now idle) stage
-    {
-        const int r = (warp & 3) * 32 + lane;
-        for (int cb = (warp >> 2) * 32; cb < CO; cb += (NT / 128) * 32) {
-            float v[32];
-            tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + cb, v);
-            tmem_ld_wait();
 #pragma unroll
-            for (int jj = 0; jj < 32; jj++)
-                if (cb + jj < CO) otile[(cb + jj) * OT + r] = v[jj];
-        }
+    for (int e = 0; e < 64; e++) {
+        const int col = acc_col(t128, e);
+        if (col < CO) otile[col * OT + wg * 64 + acc_row(t128, e)] = acc[e];
     }
-    tc_fence_before();
     __syncthreads();
     {
         const int pp = lane * 4, p = p0 + pp;
@@ -169,234 +161,8 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, NB);
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Persistent variant (C <= 256, the shapes of the reference's configs): one CTA per SM keeps its block of the weight (128 output
-// channels x C, hi and lo: up to 128 KB) RESIDENT in shared memory and walks pixel tiles; the A panels stream through a 2-stage TMA
-// ring, the accumulator is double-buffered in TMEM, and the roles are separate warps (warp 0: TMA producer, warp 1: MMA issuer,
-// warps 2-9: epilogue), so the loads of tile k+1 and its MMAs run under the epilogue of tile k.  The one-tile-per-CTA kernel above
-// spent two thirds of its time in load -> MMA -> store latency chains that nothing overlapped.
-// ---------------------------------------------------------------------------------------------------------------------
-#ifdef EPI_PIPE_TIMERS
-__device__ long long g_zg_trace[64];
-__device__ unsigned long long g_zg_span[4];      // min start, max start, min end, max end (globaltimer ns)
-#define ZTR(i) do { if (blockIdx.x == 0) g_zg_trace[i] = clock64(); } while (0)
-__device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
-#else
-#define ZTR(i) do { } while (0)
-#endif
-namespace zp {
-constexpr int NT = 320;
-constexpr int NB = 128;
-constexpr int HB = 64;                              // output channels per epilogue pass (half tile)
-constexpr int OT = 132;
-constexpr uint32_t A_PLANE = 16384, A_STAGE = 2 * A_PLANE;
-constexpr uint32_t W_PLANE = 16384, W_PANEL = 2 * W_PLANE;      // [hi 128 rows x 128 B | lo]
-constexpr uint32_t OFF_W = 0;                       // 4 K panels
-constexpr uint32_t OFF_A = 4 * W_PANEL;             // 2 stages
-constexpr uint32_t OFF_T = OFF_A + 2 * A_STAGE;     // [HB][132] fp32
-constexpr uint32_t OFF_BAR = OFF_T + HB * OT * 4;
-constexpr uint32_t SMEM_ALLOC = OFF_BAR + 256 + 1024;
-static_assert(SMEM_ALLOC <= 232448, "fits the opt-in shared memory");
-__device__ __forceinline__ void wait_bar(uint64_t *bar, uint32_t parity) {
-    for (uint32_t it = 0; !mbar_try_wait(bar, parity); ++it) if (it > (1u << 24)) __trap();
-}
-}  // namespace zp
-
-__global__ void __launch_bounds__(zp::NT, 1) epi_zgemm_persist_kernel(const ZGemmArgs z, const __grid_constant__ CUtensorMap tm_hi,
-                                                                      const __grid_constant__ CUtensorMap tm_lo,
-                                                                      const __grid_constant__ CUtensorMap tw_hi,
-                                                                      const __grid_constant__ CUtensorMap tw_lo) {
-    using namespace zp;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + OFF_BAR);     // [0-3] W panel landed, [4,5] A stage full, [6,7] A stage free, [8,9] accumulator full, [10,11] accumulator free
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + OFF_BAR + 128);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int C = z.C, HW = z.HW, W = z.W;
-    const int tiles = (HW + 127) / 128, PT = z.N * tiles;
-    const int nq = (C + 63) / 64;
-    const int nblk = (C + NB - 1) / NB;
-    const int nb = (int)blockIdx.x % nblk, first = (int)blockIdx.x / nblk, step = (int)gridDim.x / nblk;   // gridDim.x % nblk == 0
-    const int oc0 = nb * NB, CO = min(NB, C - oc0);
-#ifdef EPI_PIPE_TIMERS
-    if (tid == 0) { const unsigned long long g = gtime(); atomicMin(&g_zg_span[0], g); atomicMax(&g_zg_span[1], g); }
-    if (tid == 0) ZTR(0);
-#endif
-
-    pdl_launch_dependents();
-    // per-thread constants of the epilogue: this warp's rows of both half tiles
-    const int ew = warp - 2;                          // epilogue warp 0..7
-    float bias[2][HB / 8];
-    if (ew >= 0) {
-#pragma unroll
-        for (int h = 0; h < 2; h++)
-#pragma unroll
-            for (int k = 0; k < HB / 8; k++) {
-                const int ol = h * HB + ew + 8 * k;
-                bias[h][k] = ol < CO ? __ldg(z.bf + oc0 + ol) : 0.f;    // folded bias: written before the staging launch was issued
-            }
-    }
-    if (warp == 2) tmem_alloc(tmem_slot, 256);
-    if (tid == 0) {
-        for (int i = 0; i < 12; i++) mbar_init(&bars[i], 1);
-        mbar_fence_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_lo) : "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    if (tid == 0) ZTR(1);
-    pdl_wait();                                        // the fused kernel's feature planes (and, transitively, the staged weight)
-    if (tid == 0) ZTR(2);
-
-    if (warp == 0) {
-        // ---------------- TMA producer ----------------
-        if (lane == 0 && first < PT) {
-            const uint32_t wrows = (uint32_t)(C < NB ? C : NB);
-            uint32_t ac = 0;
-            bool first_unit = true;
-            for (int pt = first; pt < PT; pt += step) {
-                const int n = pt / tiles, p0 = (pt % tiles) * 128;
-                for (int q = 0; q < nq; q++, ac++) {
-                    if (first_unit) {                         // weight panel q right before the first A panel that multiplies with it: one
-                        mbar_arrive_expect_tx(&bars[q], 2u * wrows * 128u);     // barrier per panel, so the MMAs start after 1/nq of the weight
-                        zg::tma_load_2d(smem + OFF_W + q * W_PANEL, &tw_hi, q * 64, oc0, &bars[q]);
-                        zg::tma_load_2d(smem + OFF_W + q * W_PANEL + W_PLANE, &tw_lo, q * 64, oc0, &bars[q]);
-                    }
-                    const uint32_t s = ac & 1u;
-                    if (ac >= 2) wait_bar(&bars[6 + s], ((ac >> 1) - 1u) & 1u);
-                    mbar_arrive_expect_tx(&bars[4 + s], 2 * A_PLANE);
-                    zg::tma_load_2d(smem + OFF_A + s * A_STAGE, &tm_hi, q * 64, n * HW + p0, &bars[4 + s]);
-                    zg::tma_load_2d(smem + OFF_A + s * A_STAGE + A_PLANE, &tm_lo, q * 64, n * HW + p0, &bars[4 + s]);
-                }
-                first_unit = false;
-            }
-        }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        if (lane == 0 && first < PT) {
-            const uint32_t idesc = make_idesc_bf16(128, (uint32_t)((CO + 15) & ~15), 0, 0);
-            ZTR(3);
-            uint32_t ac = 0;
-            int k = 0;
-            for (int pt = first; pt < PT; pt += step, k++) {
-                const uint32_t buf = (uint32_t)k & 1u;
-                if (k >= 2) wait_bar(&bars[10 + buf], (uint32_t)((k >> 1) - 1) & 1u);
-                tc_fence_after();
-                for (int q = 0; q < nq; q++, ac++) {
-                    const uint32_t s = ac & 1u;
-                    if (k == 0) wait_bar(&bars[q], 0);            // weight panel q (resident afterwards)
-                    wait_bar(&bars[4 + s], (ac >> 1) & 1u);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + OFF_A + s * A_STAGE), sb = smem_u32(smem + OFF_W + q * W_PANEL);
-#pragma unroll
-                    for (int ks = 0; ks < 4; ks++) {
-                        const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = make_smem_desc(sa + A_PLANE + ks * 32, 16, 1024);
-                        const uint64_t b_hi = make_smem_desc(sb + ks * 32, 16, 1024), b_lo = make_smem_desc(sb + W_PLANE + ks * 32, 16, 1024);
-                        mma_bf16(tmem + buf * NB, a_hi, b_hi, idesc, (q | ks) ? 1u : 0u);
-                        mma_bf16(tmem + buf * NB, a_hi, b_lo, idesc, 1u);
-                        mma_bf16(tmem + buf * NB, a_lo, b_hi, idesc, 1u);
-                    }
-                    mma_commit(&bars[6 + s]);
-                }
-                mma_commit(&bars[8 + buf]);
-                if (k < 8) ZTR(8 + k);
-            }
-        }
-    } else {
-        // ---------------- epilogue (8 warps): TMEM -> [64 channels][128 pixels] tile -> + bias (+ residual) -> NCHW ----------------
-        float *otile = reinterpret_cast<float *>(smem + OFF_T);
-        const bool addr = z.ref && z.add_ref;
-        const bool vec = (z.y_stride[3] == 1) && (z.y_stride[2] == W) && (HW % 4 == 0) && (z.y_stride[1] % 4 == 0) && (z.y_stride[0] % 4 == 0) &&
-                         ((reinterpret_cast<uintptr_t>(z.y) & 15) == 0) &&
-                         (!addr || ((z.ref_stride[3] == 1) && (z.ref_stride[2] == W) && (z.ref_stride[1] % 4 == 0) && (z.ref_stride[0] % 4 == 0) &&
-                                    ((reinterpret_cast<uintptr_t>(z.ref) & 15) == 0)));
-        const int et = tid - 64;
-        int k = 0;
-        for (int pt = first; pt < PT; pt += step, k++) {
-            const int n = pt / tiles, p0 = (pt % tiles) * 128;
-            const uint32_t buf = (uint32_t)k & 1u;
-            if (ew == 0) wait_bar(&bars[8 + buf], (uint32_t)(k >> 1) & 1u);
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            if (et == 0 && k < 8) ZTR(16 + k);
-            tc_fence_after();
-            const int pp = lane * 4, p = p0 + pp;
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                if (h * HB < CO) {
-                    // residual rows of this half: issued first, consumed after the transposition
-                    float4 res[HB / 8];
-#pragma unroll
-                    for (int kk = 0; kk < HB / 8; kk++) {
-                        const int ol = h * HB + ew + 8 * kk;
-                        res[kk] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (addr && vec && p + 3 < HW && ol < CO)
-                            res[kk] = __ldcs(reinterpret_cast<const float4 *>(z.ref + (int64_t)n * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p));
-                    }
-                    {
-                        // a warp reads the TMEM lane quadrant (warp index % 4); warps 2-5 take the first 32 columns of the half, 6-9 the rest
-                        const int r = (warp & 3) * 32 + lane, cb = (ew >> 2) * 32;
-                        float v[32];
-                        tmem_ld_32x32(tmem + ((uint32_t)((warp & 3) * 32) << 16) + buf * NB + h * HB + cb, v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int jj = 0; jj < 32; jj++) otile[(cb + jj) * OT + r] = v[jj];
-                    }
-                    if (h == 1 || HB >= CO) tc_fence_before();
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if ((h == 1 || HB >= CO) && et == 0) mbar_arrive(&bars[10 + buf]);       // accumulator buffer drained
-#pragma unroll
-                    for (int kk = 0; kk < HB / 8; kk++) {
-                        const int hl = ew + 8 * kk, ol = h * HB + hl;
-                        if (ol < CO) {
-                            const int o = oc0 + ol;
-                            const float4 t = *reinterpret_cast<const float4 *>(otile + hl * OT + pp);
-                            const float b = bias[h][kk];
-                            float y[4] = {t.x + b, t.y + b, t.z + b, t.w + b};
-                            if (vec && p + 3 < HW) {
-                                __stcs(reinterpret_cast<float4 *>(z.y + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + p),   // streaming: written
-                                       make_float4(y[0] + res[kk].x, y[1] + res[kk].y, y[2] + res[kk].z, y[3] + res[kk].w));           // once, not re-read here
-                            } else {
-                                for (int e = 0; e < 4 && p + e < HW; e++) {
-                                    const int py = (p + e) / W, px = (p + e) % W;
-                                    float val = y[e];
-                                    if (addr) val += __ldg(z.ref + (int64_t)n * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3]);
-                                    z.y[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = val;
-                                }
-                            }
-                        }
-                    }
-                    asm volatile("bar.sync 1, 256;" ::: "memory");                          // the tile is rewritten by the next pass
-                }
-            }
-            if (et == 0 && k < 8) ZTR(24 + k);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem, 256);
-#ifdef EPI_PIPE_TIMERS
-    if (tid == 0) { ZTR(4); const unsigned long long g = gtime(); atomicMin(&g_zg_span[2], g); atomicMax(&g_zg_span[3], g); }
-#endif
-}
-
-#ifdef EPI_PIPE_TIMERS
-extern "C" void epi_zgemm_trace_read(long long *out64, unsigned long long *span4, int reset) {
-    cudaMemcpyFromSymbol(out64, g_zg_trace, sizeof(long long) * 64);
-    cudaMemcpyFromSymbol(span4, g_zg_span, sizeof(unsigned long long) * 4);
-    if (reset) { unsigned long long z4[4] = {~0ull, 0ull, ~0ull, 0ull}; cudaMemcpyToSymbol(g_zg_span, z4, sizeof(z4)); }
-}
-#endif
 
 bool zgemm_supported(int C) { return C % 64 == 0 && C >= 64 && C <= 512; }   // whole 64-channel TMA panels
 
@@ -413,7 +179,7 @@ EncodeTiledFn encode_fn() {
     }();
     return fn;
 }
-// [rows, cols = C] bf16 plane, box = 64 columns x box_rows rows, 128-byte swizzle (what the UMMA K-major descriptor reads)
+// [rows, cols = C] bf16 plane, box = 64 columns x box_rows rows, 128-byte swizzle (what the wgmma K-major descriptor reads)
 bool make_plane_map(CUtensorMap *m, const __nv_bfloat16 *base, int rows, int C, int box_rows) {
     EncodeTiledFn fn = encode_fn();
     if (!fn || C % 8 != 0) return false;
@@ -429,13 +195,11 @@ bool make_plane_map(CUtensorMap *m, const __nv_bfloat16 *base, int rows, int C, 
 
 cudaError_t launch_zgemm(const ZGemmArgs &z, cudaStream_t st) {
     const int tiles = (z.HW + 127) / 128;
-    const bool persist = z.C <= 256;
-    static thread_local bool attr_set[2] = {false, false};
-    if (!attr_set[persist ? 1 : 0]) {
-        cudaError_t e = persist ? cudaFuncSetAttribute(epi_zgemm_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zp::SMEM_ALLOC)
-                                : cudaFuncSetAttribute(epi_zgemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
+    static thread_local bool attr_set = false;
+    if (!attr_set) {
+        cudaError_t e = cudaFuncSetAttribute(epi_zgemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
         if (e != cudaSuccess) return e;
-        attr_set[persist ? 1 : 0] = true;
+        attr_set = true;
     }
     // tensor maps are a pure function of (pointers, shape): keep the last set per host thread
     struct MapCache { const void *xh, *wh; int rows, C; CUtensorMap m[4]; };
@@ -446,19 +210,6 @@ cudaError_t launch_zgemm(const ZGemmArgs &z, cudaStream_t st) {
             !make_plane_map(&mc.m[2], z.w_hi, z.C, z.C, wrows) || !make_plane_map(&mc.m[3], z.w_lo, z.C, z.C, wrows))
             return cudaErrorInvalidValue;
         mc.xh = z.x_hi; mc.wh = z.w_hi; mc.rows = z.N * z.HW; mc.C = z.C;
-    }
-    if (persist) {
-        static thread_local int sms_cached = 0;
-        if (!sms_cached) {
-            int dev = 0;
-            cudaGetDevice(&dev);
-            if (cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms_cached <= 0) sms_cached = 148;
-        }
-        const int nblk = (z.C + zp::NB - 1) / zp::NB, PT = z.N * tiles;
-        int per = sms_cached / nblk;                       // CTAs per block of output channels
-        if (per > PT) per = PT;
-        if (per < 1) per = 1;
-        return launch_pdl(epi_zgemm_persist_kernel, dim3((unsigned)(per * nblk)), dim3(zp::NT), (size_t)zp::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3]);
     }
     return launch_pdl(epi_zgemm_kernel, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::NB - 1) / zg::NB)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3]);
 }

@@ -1,4 +1,4 @@
-"""Host side of the B200 epipolar fusion path: `Epipolar(nn.Module)` with the reference's
+"""Host side of the CUDA epipolar fusion path: `Epipolar(nn.Module)` with the reference's
 constructor / forward contract, calling the C ABI (include/epipolar_b200.h) through ctypes.
 
 Mirrors /root/reference/modeling/layers/epipolar.py:
@@ -41,7 +41,7 @@ def _check_feat(name, t):
     if not isinstance(t, torch.Tensor) or t.dim() != 4:
         raise ValueError("%s must be a 4-D tensor [N,C,H,W]" % name)
     if not t.is_cuda:
-        raise RuntimeError("%s is on %s: the B200 epipolar path has no CPU implementation" % (name, t.device))
+        raise RuntimeError("%s is on %s: the CUDA epipolar path has no CPU implementation" % (name, t.device))
     if t.dtype != torch.float32:
         raise TypeError("%s must be float32 (got %s)" % (name, t.dtype))
 

@@ -1,8 +1,8 @@
 """Host-buffer front end of the fusion layer: pinned host tensors in, pinned host tensors out.
 
 The reference's test loop moves every batch host->device before the model call and the predictions back
-afterwards (/root/reference/engine/tester.py:131-134, modeling/model.py:282-300).  On a B200 the fused layer
-takes ~0.3 ms while the PCIe copies of its operands take ~1 ms, so this class overlaps consecutive steps on two
+afterwards (engine/tester.py:131-134, modeling/model.py:282-300 of the original project).  The PCIe copies of the fused
+layer's operands take longer than its kernels, so this class overlaps consecutive steps on two
 CUDA streams — host->device copies of step i+1 run while step i's kernels and device->host copies run — with
 `depth` rotating device input buffers.  With `d2h_stream=True` the results return on a THIRD stream (the step's output
 tensors are handed to it with `record_stream`), so step i+1's kernels do not queue behind step i's device->host copies;

@@ -22,7 +22,7 @@ def find_tensor_peak_batch(heatmap: torch.Tensor, radius, downsample, threshold:
     if not isinstance(heatmap, torch.Tensor) or heatmap.dim() not in (3, 4):
         raise ValueError("The dimension of the heatmap is wrong : %s" % (tuple(heatmap.shape),))
     if not heatmap.is_cuda:
-        raise RuntimeError("heatmap is on %s: the B200 peak finder has no CPU implementation" % heatmap.device)
+        raise RuntimeError("heatmap is on %s: the CUDA peak finder has no CPU implementation" % heatmap.device)
     if not (radius > 0):
         raise ValueError("The radius is not ok : %r" % (radius,))
     batched = heatmap.dim() == 4

@@ -1,4 +1,4 @@
-/* epipolar_b200.h — C ABI of the B200-native epipolar-transformer fusion path.
+/* epipolar_b200.h — C ABI of the H100-native (sm_90a) epipolar-transformer fusion path (the names predate the H100 port).
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference has no FFI: its "operator" is the
  * Python call  Epipolar.forward(feat1, feat2, P1, P2, ...)  at
@@ -152,7 +152,7 @@ int epi_fold_z_bn_f32(const float *z_weight, const float *z_bias, const float *b
                       const float *bn_bias, const float *bn_mean, const float *bn_var, float bn_eps,
                       int32_t C, float *w_folded, float *b_folded, void *stream);
 
-/* Diagnostic: one-CTA tcgen05 GEMM in the exact operand forms the fusion kernel uses
+/* Diagnostic: one-CTA wgmma GEMM in the exact operand forms the fusion kernels use
  * (mode 0: D[128,N] = A[128,K]·B[N,K]^T, both K-major;  mode 1: D[128,N] = At[K,128]^T·B[N,K]^T, A MN-major;
  * split=1: bf16 (hi,lo) three-term products).  All pointers device fp32, row-major. */
 int epi_umma_selftest(int mode, const float *A, const float *B, float *D, int N, int K, int split, void *stream);

@@ -90,7 +90,7 @@ class TorchGeometry:
 
 def forward(cfg, feat_ref, feat_src, P_ref, P_src, params=None, locs=None, threads=None, geometry=None):
     """feat_*: torch float32 [N,C,H,W] (CPU for the baseline; a CUDA tensor runs the same ATen op sequence on the
-    GPU, which is the "reference PyTorch forward on the same B200" of BASELINE.md B2); P_*: numpy [N,3,4].
+    GPU, which is the "reference PyTorch forward on the same GPU" of BASELINE.md B2); P_*: numpy [N,3,4].
     Returns (finalout, corr_pos, attn)."""
     if threads:
         torch.set_num_threads(int(threads))

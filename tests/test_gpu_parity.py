@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI, against
 (a) golden vectors frozen from the reference and (b) the CPU oracle on the same seeded inputs.
 
 Protocol (SURVEY.md section 8c; fp32, tolerance 1e-4 relative to max|ref| as north_star states):

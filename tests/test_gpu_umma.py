@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 building blocks (descriptors, 128B swizzle, TMEM mapping, bf16 hi/lo split) checked as
+"""GPU: the wgmma building blocks (descriptors, 128B swizzle, accumulator fragment mapping, bf16 hi/lo split) checked as
 plain GEMMs against torch fp32/fp64 matmul before the fusion kernel relies on them."""
 import ctypes
 
