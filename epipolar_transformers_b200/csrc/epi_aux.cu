@@ -111,7 +111,9 @@ cudaError_t launch_split_planes(const float *src, const int64_t stride[4], __nv_
 // ------------------------------------------------------------------------------------------
 // Pixel-major fp32 plane [N,H*W,C] (what the fused kernel writes with full 128-byte lines) -> the caller's
 // [N,C,H,W] tensor (any strides), optionally adding the caller's residual feat_ref (resnet.py:388).  64 x 64
-// tiles through shared memory: float4 reads along channels, float4 writes along pixels.
+// tiles through shared memory: reads along channels (float4 when C % 4 == 0, so that every pixel row starts on a
+// 16-byte boundary; scalar otherwise, as for the source gradient of a backward with C % 4 != 0), float4 writes
+// along pixels.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ pm, const float *__restrict__ ref, int64_t rn,
                                                       int64_t rc, int64_t rh, int64_t rw, float *__restrict__ out, int64_t on,
@@ -125,7 +127,12 @@ __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ 
         for (int i = 0; i < 4; i++) {
             const int p = p0 + pl + i * 16, c = c0 + q * 4;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p < HW && c < C) v = __ldg(reinterpret_cast<const float4 *>(pm + ((size_t)n * HW + p) * C + c));   // C % 4 == 0
+            if (p < HW && c < C) {
+                const float *row = pm + ((size_t)n * HW + p) * C + c;
+                if (C % 4 == 0) v = __ldg(reinterpret_cast<const float4 *>(row));
+                else v = make_float4(__ldg(row), c + 1 < C ? __ldg(row + 1) : 0.f, c + 2 < C ? __ldg(row + 2) : 0.f,
+                                     c + 3 < C ? __ldg(row + 3) : 0.f);
+            }
             tile[q * 4 + 0][pl + i * 16] = v.x; tile[q * 4 + 1][pl + i * 16] = v.y;
             tile[q * 4 + 2][pl + i * 16] = v.z; tile[q * 4 + 3][pl + i * 16] = v.w;
         }

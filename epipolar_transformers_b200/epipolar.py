@@ -192,14 +192,20 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
 
 
 class _FusionFn(torch.autograd.Function):
-    """The fused attention under autograd (no z epilogue: conv/BN stay in PyTorch when gradients are needed)."""
+    """The fused attention under autograd (no z epilogue: conv/BN stay in PyTorch when gradients are needed).
+    The backward samples at the locations the forward emitted rather than re-deriving them from the cameras: the forward
+    kernels round the line geometry differently, and with ill-conditioned cameras a recomputation moves samples by
+    thousandths of a feature pixel, enough to put the gradients ~1e-3 (relative) off the function the forward computed."""
 
     @staticmethod
     def forward(ctx, feat_ref, feat_src, P_ref, P_src, opts):
         with torch.no_grad():
-            out, corr, attn, locs = epipolar_fusion(feat_ref, feat_src, P_ref, P_src, want_attn=True, **opts["fwd"])
-        ctx.save_for_backward(feat_ref, feat_src, P_ref, P_src, attn)
+            out, corr, attn, locs = epipolar_fusion(feat_ref, feat_src, P_ref, P_src, want_attn=True,
+                                                    **dict(opts["fwd"], want_locs=True))
+        ctx.save_for_backward(feat_ref, feat_src, P_ref, P_src, attn, locs)
         ctx.opts = opts
+        if not opts["fwd"].get("want_locs", False):
+            locs = None
         nd = [t for t in (corr, locs) if t is not None]
         if nd:
             ctx.mark_non_differentiable(*nd)
@@ -207,7 +213,7 @@ class _FusionFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_out, g_corr, g_attn, g_locs):
-        feat_ref, feat_src, P_ref, P_src, attn = ctx.saved_tensors
+        feat_ref, feat_src, P_ref, P_src, attn, locs = ctx.saved_tensors
         o = ctx.opts
         if g_out is None:
             g_out = torch.zeros_like(feat_ref)
@@ -216,7 +222,8 @@ class _FusionFn(torch.autograd.Function):
         g_ref, g_src = epipolar_fusion_backward(
             feat_ref, feat_src, P_ref, P_src, attn, g_out, K=f["K"], downsample=f["downsample"], img_scale=f["img_scale"],
             softmax_scale=f["softmax_scale"], correct_normalize=f["correct_normalize"], align_corners=f["align_corners"],
-            grad_attn=g_attn, grad_keys=o["grad_keys"], grad_vals=o["grad_vals"], need_ref=need_ref, need_src=need_src)
+            grad_attn=g_attn, sample_locs_in=locs, grad_keys=o["grad_keys"], grad_vals=o["grad_vals"], need_ref=need_ref,
+            need_src=need_src)
         if ctx.needs_input_grad[1] and g_src is None:
             g_src = torch.zeros_like(feat_src)
         return g_ref, g_src, None, None, None

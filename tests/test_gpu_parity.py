@@ -260,6 +260,29 @@ def test_z_epilogue_tensor_core_channel_counts(C):
     assert rel_max(out.cpu().numpy(), want) < TOL
 
 
+@pytest.mark.parametrize("zres", [True, False])
+@pytest.mark.parametrize("C", [24, 130, 264, 1024])
+def test_z_epilogue_fp32_channel_counts(C, zres):
+    """z conv + BN(eval) (+ ZRESIDUAL) + the caller residual on the fp32 CUDA-core epilogue, which takes every channel count
+    the tensor-core GEMM does not, behind whichever kernel automatic selection picks: C = 24 the pipelined kernel, C = 264 its
+    two-pass epilogue into the NCHW pre-z buffer, C = 130 and 1024 the CUDA-core kernel."""
+    from epipolar_transformers_b200 import synthetic as syn
+    N, H, W, K = 2, 24, 24, 16
+    cfg = epi.make_cfg(KEYPOINT=dict(HEATMAP_SIZE=(H, W), NFEATS=C),
+                       EPIPOLAR=dict(SAMPLESIZE=K, USE_CORRECT_NORMALIZE=True, PARAMETERIZED=("z",), ZRESIDUAL=zres))
+    P1, P2 = syn.pairs_from_ring(N, 4 * H)
+    P1, P2 = P1.astype(np.float32), P2.astype(np.float32)
+    f1, f2 = syn.features(N, C, H, W, "randn", 21), syn.features(N, C, H, W, "randn", 22)
+    params = syn.z_bn_params(C, 5)
+    out, corr, attn, locs = epi.epipolar_fusion(dev(f1), dev(f2), dev(P1), dev(P2), K=K, correct_normalize=True, want_locs=True,
+                                                z_folded=fold_params(params, zres), z_residual=zres, add_ref_residual=True,
+                                                variant="auto")
+    torch.cuda.synchronize()
+    o = c_oracle.forward(cfg, f1, f2, P1, P2, locs=locs.cpu().numpy())
+    want = eo.z_epilogue(o["out"], params, zres) + f1
+    assert rel_max(out.cpu().numpy(), want) < TOL
+
+
 def test_fused_caller_residual_module():
     """Epipolar(fuse_ref_residual=True) + fused_other_feat == the reference caller's `ret + feat`
     (modeling/backbones/resnet.py:377-388), with and without the z epilogue; other_features=None passes feat through."""
@@ -382,6 +405,10 @@ SWEEP = [  # (N, C, H, W, K)   BASELINE config 5 corners + map sizes on both sid
     (1, 16, 144, 144, 16), (2, 24, 100, 400, 64), (1, 8, 300, 100, 16),                          # H*W > 16384: row-windowed union; H > 256 -> warp kernel
     (2, 40, 24, 40, 48),                                                                         # C % 32 != 0, partial tiles
     (1, 64, 256, 256, 16),                                                                       # literal 256x256 feature-map reading
+    # the CUDA-core kernel's own envelope (C % 8 != 0, C > 512, K > 128): one shape per instantiation <VEC,NV>
+    (2, 3, 20, 24, 16), (1, 70, 24, 24, 64), (1, 130, 16, 16, 129),                              # <1,1>, <1,4>, <1,16> (K = 129)
+    (1, 260, 16, 24, 65), (1, 1024, 12, 16, 32), (1, 516, 16, 16, 256),                          # <4,4> (C % 8 != 0), <4,8> (C > 512, K = 256)
+    (2, 64, 32, 32, 200), (1, 256, 24, 24, 256),                                                 # <4,1> and <4,2> at K > 128
 ]
 
 
