@@ -11,7 +11,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libepipolar_b200.so")
 
-EPI_ABI_VERSION = 2
+EPI_ABI_VERSION = 3
+EPI_DTYPE_F32, EPI_DTYPE_BF16, EPI_DTYPE_F16 = 0, 1, 2
 EPI_VARIANT_AUTO, EPI_VARIANT_WARP, EPI_VARIANT_TILE, EPI_VARIANT_SECTOR, EPI_VARIANT_PIPE = 0, 1, 2, 3, 4
 VARIANTS = {"auto": EPI_VARIANT_AUTO, "warp": EPI_VARIANT_WARP, "tile": EPI_VARIANT_TILE, "sector": EPI_VARIANT_SECTOR,
             "pipe": EPI_VARIANT_PIPE}
@@ -37,7 +38,8 @@ class EpiFusionParams(ctypes.Structure):
         ("N", ctypes.c_int32), ("C", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("K", ctypes.c_int32),
         ("downsample", ctypes.c_float), ("img_scale", ctypes.c_float), ("eps", ctypes.c_float), ("softmax_scale", ctypes.c_float),
         ("align_corners", ctypes.c_int32), ("correct_normalize", ctypes.c_int32), ("z_residual", ctypes.c_int32),
-        ("add_ref_residual", ctypes.c_int32), ("variant", ctypes.c_int32), ("reserved", ctypes.c_int32 * 3),
+        ("add_ref_residual", ctypes.c_int32), ("variant", ctypes.c_int32), ("feat_dtype", ctypes.c_int32),
+        ("reserved", ctypes.c_int32 * 2),
         ("cache", ctypes.c_void_p), ("cache_bytes", ctypes.c_size_t),
     ]
 
@@ -57,7 +59,8 @@ class EpiFusionBwdParams(ctypes.Structure):
         ("N", ctypes.c_int32), ("C", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32), ("K", ctypes.c_int32),
         ("downsample", ctypes.c_float), ("img_scale", ctypes.c_float), ("eps", ctypes.c_float), ("softmax_scale", ctypes.c_float),
         ("align_corners", ctypes.c_int32), ("correct_normalize", ctypes.c_int32),
-        ("grad_keys", ctypes.c_int32), ("grad_vals", ctypes.c_int32), ("reserved", ctypes.c_int32 * 4),
+        ("grad_keys", ctypes.c_int32), ("grad_vals", ctypes.c_int32), ("feat_dtype", ctypes.c_int32),
+        ("reserved", ctypes.c_int32 * 3),
     ]
 
 

@@ -28,8 +28,9 @@ bool src_is_channels_last(const EpiFusionParams *p) {
 }
 
 struct Plan {
-    size_t off_src = 0, off_prez = 0, off_counter = 0, off_ref = 0, off_order = 0, off_wplanes = 0, off_geom = 0, total = 0;
+    size_t off_src = 0, off_prez = 0, off_counter = 0, off_ref = 0, off_order = 0, off_wplanes = 0, off_geom = 0, off_ref32 = 0, total = 0;
     bool stage_src = false, has_z = false, tile = false, sector = false, pipe = false, unstage = false;
+    bool ref32 = false;     // fp32 channels-last copy of a low-precision feat_ref for the kernels that read feat_ref as fp32
 };
 
 bool want_pipe(const EpiFusionParams *p) {
@@ -51,17 +52,21 @@ bool want_tile(const EpiFusionParams *p) {
 Plan make_plan(const EpiFusionParams *p) {
     Plan pl;
     const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
+    const bool lowp = p->feat_dtype != EPI_DTYPE_F32;
     pl.pipe = want_pipe(p);
     if (pl.pipe) {
-        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes (bytes of two fp32 maps), pre-z planes, pixel order, pair constants
+        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes (bytes of two fp32 maps; bf16 maps: [ref_hi | src_hi], one fp32 map),
+        // pre-z planes, pixel order, pair constants
         pl.has_z = p->z_weight_folded != nullptr;
         size_t off = 0;
-        pl.off_ref = off; off += align_up(2 * map);
+        pl.off_ref = off; off += align_up(p->feat_dtype == EPI_DTYPE_BF16 ? map : 2 * map);
         // pre-z planes (z path) or the pixel-major fp32 plane the fused kernel writes when the caller's tensor is NCHW
         pl.unstage = !pl.has_z && !(p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0);
         if (pl.has_z || pl.unstage) { pl.off_prez = off; off += align_up(map); }
         pl.off_counter = off; off += 256;
         if (pl.has_z && epi::zgemm_supported(p->C)) { pl.off_wplanes = off; off += align_up((size_t)p->C * p->C * 4); }
+        pl.ref32 = lowp && pl.has_z && !epi::zgemm_supported(p->C) && p->add_ref_residual;      // the fp32 z epilogue's residual
+        if (pl.ref32) { pl.off_ref32 = off; off += align_up(map); }
         if (!p->cache) {               // no persistent cache: pixel order and pair constants are rebuilt in the workspace every call
             pl.off_order = off; off += align_up((size_t)p->N * p->H * p->W * sizeof(uint16_t));
             pl.off_geom = off; off += align_up((size_t)p->N * sizeof(epi::PairGeom));
@@ -73,9 +78,12 @@ Plan make_plan(const EpiFusionParams *p) {
     // sector tiles (pixels grouped by epipolar angle) need the fused geometry; injected locations and an explicit
     // EPI_VARIANT_TILE request use the 4x8 block tiles
     pl.sector = pl.tile && p->variant != EPI_VARIANT_TILE && p->sample_locs_in == nullptr;
-    pl.stage_src = pl.tile || !src_is_channels_last(p);      // tile kernel: bf16 (hi, lo) planes, same bytes as one fp32 map
+    // tile kernel: bf16 (hi, lo) planes, same bytes as one fp32 map; the warp kernel reads a channels-last fp32 source in place
+    pl.stage_src = pl.tile || !src_is_channels_last(p) || lowp;
     pl.has_z = p->z_weight_folded != nullptr;
+    pl.ref32 = lowp;                                         // these kernels read the query (and the residual) as fp32
     size_t off = 0;
+    if (pl.ref32) { pl.off_ref32 = off; off += align_up(map); }
     if (pl.stage_src) { pl.off_src = off; off += align_up(map); }
     if (pl.has_z) { pl.off_prez = off; off += align_up(map); }
     if (pl.tile) { pl.off_counter = off; off += 256; }
@@ -97,6 +105,7 @@ int validate(const EpiFusionParams *p) {
     if (!(p->downsample > 0.f) || !(p->img_scale > 0.f)) return fail(EPI_EINVAL, "downsample and img_scale must be positive");
     if (p->z_weight_folded && !p->z_bias_folded) return fail(EPI_EINVAL, "z_bias_folded required with z_weight_folded");
     if (p->variant < EPI_VARIANT_AUTO || p->variant > EPI_VARIANT_PIPE) return fail(EPI_EINVAL, "unknown variant");
+    if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
     if (p->z_weight_folded && (reinterpret_cast<uintptr_t>(p->z_weight_folded) % 16 != 0 || reinterpret_cast<uintptr_t>(p->z_bias_folded) % 4 != 0))
         return fail(EPI_EINVAL, "z_weight_folded must be 16-byte aligned (contiguous [C,C]) and z_bias_folded 4-byte aligned");
     return EPI_OK;
@@ -175,14 +184,18 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         cudaEventRecord(g_evA, st);
     }
 
+    const int dt = p->feat_dtype;
     epi::FusionArgs a;
     memset(&a, 0, sizeof(a));
-    a.feat_ref = p->feat_ref;
+    a.feat_ref = static_cast<const float *>(p->feat_ref); a.ref_dtype = dt;
     a.P_ref = p->P_ref; a.P_src = p->P_src; a.locs_in = p->sample_locs_in;
     a.attn = p->attn; a.corr_pos = p->corr_pos; a.locs_out = p->sample_locs_out;
     a.N = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale;
     for (int i = 0; i < 4; i++) a.ref_stride[i] = p->ref_stride[i];
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
+    // fp32 kernels that read feat_ref get a channels-last fp32 copy of a low-precision map
+    float *ref32 = pl.ref32 ? reinterpret_cast<float *>(ws + pl.off_ref32) : nullptr;
+    const int64_t ref32_stride[4] = {(int64_t)p->C * p->H * p->W, 1, (int64_t)p->W * p->C, p->C};
 
     if (p->variant == EPI_VARIANT_PIPE && !pl.pipe) return fail(EPI_EINVAL, "pipe variant does not support this shape");
     if (pl.pipe) {
@@ -212,28 +225,36 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         if (!have_P) { order = nullptr; okey = nullptr; }
         const bool z_planes = pl.has_z && epi::zgemm_supported(p->C);
         __nv_bfloat16 *wpl = z_planes ? reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_wplanes) : nullptr;
-        e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, planes, p->P_ref, p->P_src, pg, order, okey,
+        e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, planes, p->P_ref, p->P_src, pg, order, okey,
                               z_planes ? p->z_weight_folded : nullptr, wpl, p->z_residual ? 1 : 0, words, p->N, p->C, p->H, p->W, a.geom, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
         launches += (order && (size_t)p->H * p->W * 2 + 16384 > 64 * 1024) ? 2 : 1;      // large maps order their pixels in a launch of their own
         w_hi = wpl; w_lo = wpl ? wpl + (size_t)p->C * p->C : nullptr;
-        a.ref_hi = planes; a.ref_lo = planes + elems; a.src_hi = planes + 2 * elems; a.src_lo = planes + 3 * elems;
+        if (dt == EPI_DTYPE_BF16) { a.ref_hi = planes; a.src_hi = planes + elems; }       // no lo planes: the pipe kernel's LO = false form
+        else { a.ref_hi = planes; a.ref_lo = planes + elems; a.src_hi = planes + 2 * elems; a.src_lo = planes + 3 * elems; }
         a.order = order; a.pair_geom = pg; a.tile_counter = words; a.err_flag = words + 1;
     } else
     if (p->variant == EPI_VARIANT_TILE && !pl.tile) return fail(EPI_EINVAL, "tile variant does not support this shape");
     if (p->variant == EPI_VARIANT_SECTOR && !pl.sector) return fail(EPI_EINVAL, "sector variant does not support this shape / injected locations");
+    if (!pl.pipe && ref32) {
+        e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
+        if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
+        launches++;
+        a.feat_ref = ref32; a.ref_dtype = EPI_DTYPE_F32;
+        for (int i = 0; i < 4; i++) a.ref_stride[i] = ref32_stride[i];
+    }
     if (pl.tile) {
         __nv_bfloat16 *hi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_src);
         __nv_bfloat16 *lo = hi + (size_t)p->N * p->C * p->H * p->W;
         a.tile_counter = reinterpret_cast<int *>(ws + pl.off_counter);
-        e = epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, p->N, p->C, p->H, p->W, a.tile_counter, st);
+        e = epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, p->N, p->C, p->H, p->W, a.tile_counter, dt, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
         launches++;
         a.src_hi = hi; a.src_lo = lo;
         if (pl.sector) {
             __nv_bfloat16 *rhi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_ref);
             __nv_bfloat16 *rlo = rhi + (size_t)p->N * p->C * p->H * p->W;
-            e = epi::launch_split_planes(p->feat_ref, p->ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, st);
+            e = epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st);
             if (e != cudaSuccess) return fail(EPI_ECUDA, "reference staging launch failed: %s", cudaGetErrorString(e));
             uint16_t *order = reinterpret_cast<uint16_t *>(ws + pl.off_order);
             e = epi::launch_sector_order(p->P_ref, p->P_src, order, p->N, a.geom, st);
@@ -243,12 +264,12 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         }
     } else if (pl.stage_src) {
         float *nhwc = reinterpret_cast<float *>(ws + pl.off_src);
-        e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, st);
+        e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "layout staging launch failed: %s", cudaGetErrorString(e));
         launches++;
         a.src_nhwc = nhwc;
     } else {
-        a.src_nhwc = p->feat_src;
+        a.src_nhwc = static_cast<const float *>(p->feat_src);
     }
 
     const bool z_tc = pl.has_z && pl.pipe && epi::zgemm_supported(p->C);      // tensor-core z GEMM (operand planes come from the staging launch)
@@ -282,7 +303,8 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     launches++;
 
     if (pl.pipe && pl.unstage) {
-        e = epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, p->ref_stride, p->out, p->out_stride, p->N, p->C, p->H, p->W, st);
+        e = epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out, EPI_DTYPE_F32, p->out_stride,
+                                p->N, p->C, p->H, p->W, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "output transposition launch failed: %s", cudaGetErrorString(e));
         launches++;
     }
@@ -290,7 +312,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         epi::ZGemmArgs z;
         memset(&z, 0, sizeof(z));
         z.x_hi = a.out_hi; z.x_lo = a.out_lo; z.w_hi = w_hi; z.w_lo = w_lo; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
-        z.ref = p->feat_ref; z.y = p->out;
+        z.ref = p->feat_ref; z.ref_dtype = dt; z.y = p->out;
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
         z.N = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
@@ -298,11 +320,16 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         if (e != cudaSuccess) return fail(EPI_ECUDA, "z GEMM launch failed: %s", cudaGetErrorString(e));
         launches++;
     } else if (pl.has_z) {
+        if (pl.pipe && ref32) {            // (the other kernels' plans made the copy before the fused kernel)
+            e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
+            if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
+            launches++;
+        }
         epi::ZArgs z;
         memset(&z, 0, sizeof(z));
         z.x = a.out;
-        for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
-        z.ref = p->feat_ref; z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
+        for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? ref32_stride[i] : p->ref_stride[i]; }
+        z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.N = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         e = epi::launch_z_epilogue(z, st);
@@ -317,7 +344,9 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p) {
     if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0) return 0;
     const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
-    return 2 * align_up(map);          // pixel-major copy of feat_src + pixel-major accumulator of its gradient
+    // pixel-major copy of feat_src + pixel-major accumulator of its gradient; low-precision maps: + a channels-last fp32 copy of
+    // feat_ref and a pixel-major fp32 buffer of its gradient (rounded once to the maps' type by the transposition pass)
+    return (p->feat_dtype != EPI_DTYPE_F32 ? 4 : 2) * align_up(map);
 }
 
 int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
@@ -326,34 +355,54 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
     if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2 || p->K < 2 || p->K > 256) return fail(EPI_EINVAL, "bad shape");
     if (p->C > 512 || (p->C > 128 && p->C % 4 != 0)) return fail(EPI_EINVAL, "backward supports C <= 128, or C <= 512 with C % 4 == 0");
+    if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
     if (!p->grad_ref && !p->grad_src) return EPI_OK;
     const size_t need = epi_fusion_backward_workspace_bytes(p);
     if (!p->workspace || p->workspace_bytes < need) return fail(EPI_EWORKSPACE, "workspace too small");
     if (reinterpret_cast<uintptr_t>(p->workspace) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
+    const int dt = p->feat_dtype;
+    const bool lowp = dt != EPI_DTYPE_F32;
     float *nhwc = reinterpret_cast<float *>(p->workspace);
     float *dsrc = reinterpret_cast<float *>(static_cast<char *>(p->workspace) + align_up(map));
-    cudaError_t e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, st);
+    float *ref32 = lowp ? reinterpret_cast<float *>(static_cast<char *>(p->workspace) + 2 * align_up(map)) : nullptr;
+    float *gref32 = lowp ? reinterpret_cast<float *>(static_cast<char *>(p->workspace) + 3 * align_up(map)) : nullptr;
+    const int64_t pm_stride[4] = {(int64_t)p->C * p->H * p->W, 1, (int64_t)p->W * p->C, p->C};      // pixel-major / channels-last
+    cudaError_t e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st);
     if (e != cudaSuccess) return fail(EPI_ECUDA, "layout staging launch failed: %s", cudaGetErrorString(e));
     int launches = 1;
+    if (lowp) {
+        e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
+        if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
+        launches++;
+    }
     if (p->grad_src) {
         e = cudaMemsetAsync(dsrc, 0, map, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "memset failed: %s", cudaGetErrorString(e));
     }
     epi::BwdArgs a;
     memset(&a, 0, sizeof(a));
-    a.feat_ref = p->feat_ref; a.src_nhwc = nhwc; a.P_ref = p->P_ref; a.P_src = p->P_src; a.locs_in = p->sample_locs_in;
-    a.attn = p->attn; a.grad_out = p->grad_out; a.grad_attn = p->grad_attn; a.grad_ref = p->grad_ref;
+    a.feat_ref = lowp ? ref32 : static_cast<const float *>(p->feat_ref); a.src_nhwc = nhwc; a.P_ref = p->P_ref; a.P_src = p->P_src;
+    a.locs_in = p->sample_locs_in; a.attn = p->attn; a.grad_out = p->grad_out; a.grad_attn = p->grad_attn;
+    a.grad_ref = !p->grad_ref ? nullptr : (lowp ? gref32 : static_cast<float *>(p->grad_ref));
     a.dsrc_nhwc = p->grad_src ? dsrc : nullptr;
-    for (int i = 0; i < 4; i++) { a.ref_stride[i] = p->ref_stride[i]; a.gout_stride[i] = p->gout_stride[i]; a.gref_stride[i] = p->gref_stride[i]; }
+    for (int i = 0; i < 4; i++) {
+        a.ref_stride[i] = lowp ? pm_stride[i] : p->ref_stride[i]; a.gout_stride[i] = p->gout_stride[i];
+        a.gref_stride[i] = lowp ? pm_stride[i] : p->gref_stride[i];
+    }
     a.N = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale; a.grad_keys = p->grad_keys; a.grad_vals = p->grad_vals;
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
     e = epi::launch_fusion_bwd(a, st);
     if (e != cudaSuccess) return fail(EPI_ECUDA, "backward kernel launch failed: %s", cudaGetErrorString(e));
     launches++;
     if (p->grad_src) {
-        e = epi::launch_unstage(dsrc, nullptr, p->gsrc_stride, p->grad_src, p->gsrc_stride, p->N, p->C, p->H, p->W, st);
+        e = epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride, p->N, p->C, p->H, p->W, st);
+        if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
+        launches++;
+    }
+    if (p->grad_ref && lowp) {         // fp32 gradient of a low-precision reference map, rounded once to its type
+        e = epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride, p->N, p->C, p->H, p->W, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
         launches++;
     }

@@ -4,21 +4,22 @@
 namespace epi {
 
 // ------------------------------------------------------------------------------------------
-// [N,C,H,W] (any strides) -> [N,H,W,C] contiguous.  32x32 shared-memory transpose per item:
-// reads are coalesced along the pixel axis when stride[3]==1 (NCHW), writes along channels.
+// [N,C,H,W] (any strides, element type T) -> [N,H,W,C] contiguous fp32.  32x32 shared-memory transpose per
+// item: reads are coalesced along the pixel axis when stride[3]==1 (NCHW), writes along channels.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) nchw_to_nhwc_kernel(const float *__restrict__ src, int64_t sn, int64_t sc,
+template <typename T>
+__global__ void __launch_bounds__(256) nchw_to_nhwc_kernel(const T *__restrict__ src, int64_t sn, int64_t sc,
                                                            int64_t sh, int64_t sw, float *__restrict__ dst,
                                                            int C, int H, int W) {
     __shared__ float tile[32][33];
     const int HW = H * W;
     const int n = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;          // 32 x 8
-    const float *s = src + (int64_t)n * sn;
+    const T *s = src + (int64_t)n * sn;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         int c = c0 + ty + i * 8, p = p0 + tx;
-        tile[ty + i * 8][tx] = (c < C && p < HW) ? __ldg(s + c * sc + (p / W) * sh + (p % W) * sw) : 0.f;
+        tile[ty + i * 8][tx] = (c < C && p < HW) ? to_f32(__ldg(s + c * sc + (p / W) * sh + (p % W) * sw)) : 0.f;
     }
     __syncthreads();
     float *d = dst + (size_t)n * HW * C;
@@ -29,18 +30,24 @@ __global__ void __launch_bounds__(256) nchw_to_nhwc_kernel(const float *__restri
     }
 }
 
-cudaError_t launch_nchw_to_nhwc(const float *src, const int64_t stride[4], float *dst, int N, int C, int H, int W,
+cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
                                 cudaStream_t st) {
     dim3 grid((H * W + 31) / 32, (C + 31) / 32, N);
-    nchw_to_nhwc_kernel<<<grid, 256, 0, st>>>(src, stride[0], stride[1], stride[2], stride[3], dst, C, H, W);
+    if (dtype == kBF16)
+        nchw_to_nhwc_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16 *>(src), stride[0], stride[1], stride[2], stride[3], dst, C, H, W);
+    else if (dtype == kF16)
+        nchw_to_nhwc_kernel<<<grid, 256, 0, st>>>(static_cast<const __half *>(src), stride[0], stride[1], stride[2], stride[3], dst, C, H, W);
+    else
+        nchw_to_nhwc_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(src), stride[0], stride[1], stride[2], stride[3], dst, C, H, W);
     return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------
-// [N,C,H,W] fp32 (any strides) -> two bf16 planes [N,H,W,C] with src ≈ hi + lo (operands of the
-// tensor-core kernel; |src - hi - lo| <~ 2^-17 |src|).  Same 32x32 transpose tile as above.
+// [N,C,H,W] (any strides, element type T) -> two bf16 planes [N,H,W,C] with src ≈ hi + lo (operands of the
+// tensor-core kernel; |src - hi - lo| <~ 2^-17 |src|, exact for bf16 and fp16 inputs).
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) split_planes_kernel(const float *__restrict__ src, int64_t sn, int64_t sc, int64_t sh,
+template <typename T>
+__global__ void __launch_bounds__(256) split_planes_kernel(const T *__restrict__ src, int64_t sn, int64_t sc, int64_t sh,
                                                            int64_t sw, __nv_bfloat16 *__restrict__ hi,
                                                            __nv_bfloat16 *__restrict__ lo, int C, int H, int W, int *zero_me) {
     // tile: 64 channels x 64 pixels.  NCHW sources are read as float4 (a warp covers two 256-byte runs, which also
@@ -51,8 +58,8 @@ __global__ void __launch_bounds__(256) split_planes_kernel(const float *__restri
     const int HW = H * W;
     const int n = blockIdx.z, c0 = blockIdx.y * 64, p0 = blockIdx.x * 64;
     const int t = threadIdx.x;
-    const float *s = src + (int64_t)n * sn;
-    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(s) & 15) == 0);
+    const T *s = src + (int64_t)n * sn;
+    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(s) & (4 * sizeof(T) - 1)) == 0);
     if (sc != 1) {
         const int q = t & 15, cy = t >> 4;                      // 16 float4 per channel row, 16 channels per pass
 #pragma unroll
@@ -60,10 +67,10 @@ __global__ void __launch_bounds__(256) split_planes_kernel(const float *__restri
             const int c = c0 + cy + i * 16, p = p0 + q * 4;
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
             if (c < C) {
-                if (vec && p + 3 < HW) v = __ldg(reinterpret_cast<const float4 *>(s + c * sc + p));
+                if (vec && p + 3 < HW) v = ld4_nc(s + c * sc + p);
                 else {
                     float e[4] = {0.f, 0.f, 0.f, 0.f};
-                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = __ldg(s + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw);
+                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = to_f32(__ldg(s + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw));
                     v = make_float4(e[0], e[1], e[2], e[3]);
                 }
             }
@@ -75,7 +82,7 @@ __global__ void __launch_bounds__(256) split_planes_kernel(const float *__restri
 #pragma unroll
         for (int i = 0; i < 16; i++) {
             const int p = p0 + py + i * 4, c = c0 + cx;
-            tile[cx][py + i * 4] = (c < C && p < HW) ? __ldg(s + c + (p / W) * sh + (p % W) * sw) : 0.f;
+            tile[cx][py + i * 4] = (c < C && p < HW) ? to_f32(__ldg(s + c + (p / W) * sh + (p % W) * sw)) : 0.f;
         }
     }
     __syncthreads();
@@ -101,22 +108,29 @@ __global__ void __launch_bounds__(256) split_planes_kernel(const float *__restri
     }
 }
 
-cudaError_t launch_split_planes(const float *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
-                                int H, int W, int *zero_me, cudaStream_t st) {
+cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
+                                int H, int W, int *zero_me, int dtype, cudaStream_t st) {
     dim3 grid((H * W + 63) / 64, (C + 63) / 64, N);
-    split_planes_kernel<<<grid, 256, 0, st>>>(src, stride[0], stride[1], stride[2], stride[3], hi, lo, C, H, W, zero_me);
+    if (dtype == kBF16)
+        split_planes_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16 *>(src), stride[0], stride[1], stride[2], stride[3], hi, lo, C, H, W, zero_me);
+    else if (dtype == kF16)
+        split_planes_kernel<<<grid, 256, 0, st>>>(static_cast<const __half *>(src), stride[0], stride[1], stride[2], stride[3], hi, lo, C, H, W, zero_me);
+    else
+        split_planes_kernel<<<grid, 256, 0, st>>>(static_cast<const float *>(src), stride[0], stride[1], stride[2], stride[3], hi, lo, C, H, W, zero_me);
     return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------
 // Pixel-major fp32 plane [N,H*W,C] (what the fused kernel writes with full 128-byte lines) -> the caller's
-// [N,C,H,W] tensor (any strides), optionally adding the caller's residual feat_ref (resnet.py:388).  64 x 64
+// [N,C,H,W] tensor of element type TO (any strides; fp32 sums rounded once), optionally adding the caller's residual
+// feat_ref of element type TR (resnet.py:388).  64 x 64
 // tiles through shared memory: reads along channels (float4 when C % 4 == 0, so that every pixel row starts on a
 // 16-byte boundary; scalar otherwise, as for the source gradient of a backward with C % 4 != 0), float4 writes
 // along pixels.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ pm, const float *__restrict__ ref, int64_t rn,
-                                                      int64_t rc, int64_t rh, int64_t rw, float *__restrict__ out, int64_t on,
+template <typename TO, typename TR>
+__global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ pm, const TR *__restrict__ ref, int64_t rn,
+                                                      int64_t rc, int64_t rh, int64_t rw, TO *__restrict__ out, int64_t on,
                                                       int64_t oc, int64_t oh, int64_t ow, int C, int H, int W) {
     __shared__ float tile[64][65];                              // [channel][pixel]
     const int HW = H * W, t = threadIdx.x;
@@ -138,8 +152,8 @@ __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ 
         }
     }
     __syncthreads();
-    const bool vec_o = (ow == 1) && (oh == W) && (HW % 4 == 0) && (oc % 4 == 0) && (on % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
-    const bool vec_r = !ref || ((rw == 1) && (rh == W) && (rc % 4 == 0) && (rn % 4 == 0) && ((reinterpret_cast<uintptr_t>(ref) & 15) == 0));
+    const bool vec_o = (ow == 1) && (oh == W) && (HW % 4 == 0) && (oc % 4 == 0) && (on % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & (4 * sizeof(TO) - 1)) == 0);
+    const bool vec_r = !ref || ((rw == 1) && (rh == W) && (rc % 4 == 0) && (rn % 4 == 0) && ((reinterpret_cast<uintptr_t>(ref) & (4 * sizeof(TR) - 1)) == 0));
     const int q = t & 15, cy = t >> 4;                          // 16 float4 per channel row, 16 channels per pass
 #pragma unroll
     for (int i = 0; i < 4; i++) {
@@ -148,26 +162,38 @@ __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ 
         float v[4] = {tile[cy + i * 16][q * 4], tile[cy + i * 16][q * 4 + 1], tile[cy + i * 16][q * 4 + 2], tile[cy + i * 16][q * 4 + 3]};
         if (vec_o && vec_r && p + 3 < HW) {
             if (ref) {
-                const float4 r4 = __ldg(reinterpret_cast<const float4 *>(ref + (int64_t)n * rn + (int64_t)c * rc + p));
+                const float4 r4 = ld4_nc(ref + (int64_t)n * rn + (int64_t)c * rc + p);
                 v[0] += r4.x; v[1] += r4.y; v[2] += r4.z; v[3] += r4.w;
             }
-            *reinterpret_cast<float4 *>(out + (int64_t)n * on + (int64_t)c * oc + p) = make_float4(v[0], v[1], v[2], v[3]);
+            st4(out + (int64_t)n * on + (int64_t)c * oc + p, make_float4(v[0], v[1], v[2], v[3]));
         } else {
             for (int j = 0; j < 4 && p + j < HW; j++) {
                 const int y = (p + j) / W, x = (p + j) % W;
                 float o = v[j];
-                if (ref) o += __ldg(ref + (int64_t)n * rn + (int64_t)c * rc + (int64_t)y * rh + (int64_t)x * rw);
-                out[(int64_t)n * on + (int64_t)c * oc + (int64_t)y * oh + (int64_t)x * ow] = o;
+                if (ref) o += to_f32(__ldg(ref + (int64_t)n * rn + (int64_t)c * rc + (int64_t)y * rh + (int64_t)x * rw));
+                out[(int64_t)n * on + (int64_t)c * oc + (int64_t)y * oh + (int64_t)x * ow] = from_f32<TO>(o);
             }
         }
     }
 }
 
-cudaError_t launch_unstage(const float *pm, const float *ref, const int64_t ref_stride[4], float *out, const int64_t out_stride[4],
-                           int N, int C, int H, int W, cudaStream_t st) {
+template <typename TO, typename TR>
+static void unstage_t(dim3 grid, cudaStream_t st, const float *pm, const void *ref, const int64_t ref_stride[4], void *out,
+                      const int64_t out_stride[4], int C, int H, int W) {
+    unstage_kernel<TO, TR><<<grid, 256, 0, st>>>(pm, static_cast<const TR *>(ref), ref ? ref_stride[0] : 0, ref ? ref_stride[1] : 0,
+                                                 ref ? ref_stride[2] : 0, ref ? ref_stride[3] : 0, static_cast<TO *>(out), out_stride[0],
+                                                 out_stride[1], out_stride[2], out_stride[3], C, H, W);
+}
+
+cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
+                           const int64_t out_stride[4], int N, int C, int H, int W, cudaStream_t st) {
     dim3 grid((H * W + 63) / 64, (C + 63) / 64, N);
-    unstage_kernel<<<grid, 256, 0, st>>>(pm, ref, ref ? ref_stride[0] : 0, ref ? ref_stride[1] : 0, ref ? ref_stride[2] : 0,
-                                         ref ? ref_stride[3] : 0, out, out_stride[0], out_stride[1], out_stride[2], out_stride[3], C, H, W);
+    if (out_dtype != kF32 && ref) return cudaErrorInvalidValue;           // a low-precision output is a gradient: no residual
+    if (out_dtype == kBF16) unstage_t<__nv_bfloat16, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, C, H, W);
+    else if (out_dtype == kF16) unstage_t<__half, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, C, H, W);
+    else if (ref_dtype == kBF16) unstage_t<float, __nv_bfloat16>(grid, st, pm, ref, ref_stride, out, out_stride, C, H, W);
+    else if (ref_dtype == kF16) unstage_t<float, __half>(grid, st, pm, ref, ref_stride, out, out_stride, C, H, W);
+    else unstage_t<float, float>(grid, st, pm, ref, ref_stride, out, out_stride, C, H, W);
     return cudaGetLastError();
 }
 

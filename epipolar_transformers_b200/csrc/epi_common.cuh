@@ -5,6 +5,8 @@
 // :39-57 de_normalize, :154-163 pix2coord/coord2pix) per pixel, with the better-conditioned
 // infinite-homography point x2' = (A2 A1^-1) p on the same epipolar line (SURVEY.md app. B).
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -12,6 +14,60 @@ namespace epi {
 
 constexpr float kFar = 10000.0f;      // epipolar.py:51-53
 constexpr float kMasked = -1e10f;     // epipolar.py:298
+
+// Element types of the feature maps (EPI_DTYPE_* of the C ABI).  bf16 and fp16 values are exact in fp32, so every kernel
+// computes on the fp32 value of the input; only the loads (and the backward's gradient stores) see the storage type.
+enum FeatDtype { kF32 = 0, kBF16 = 1, kF16 = 2 };
+
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+
+// four consecutive elements as fp32; p is aligned to 4 elements.  Streaming (read-once) load.
+__device__ __forceinline__ float4 ld4_cs(const float *p) { return __ldcs(reinterpret_cast<const float4 *>(p)); }
+__device__ __forceinline__ float4 ld4_cs(const __nv_bfloat16 *p) {
+    const uint2 r = __ldcs(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.x)), b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 ld4_cs(const __half *p) {
+    const uint2 r = __ldcs(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&r.x)), b = __half22float2(*reinterpret_cast<const __half2 *>(&r.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+// the same through the read-only cache
+__device__ __forceinline__ float4 ld4_nc(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
+__device__ __forceinline__ float4 ld4_nc(const __nv_bfloat16 *p) {
+    const uint2 r = __ldg(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.x)), b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ float4 ld4_nc(const __half *p) {
+    const uint2 r = __ldg(reinterpret_cast<const uint2 *>(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&r.x)), b = __half22float2(*reinterpret_cast<const __half2 *>(&r.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+// four consecutive elements from fp32, rounded once to T; p is aligned to 4 elements
+__device__ __forceinline__ void st4(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
+__device__ __forceinline__ void st4(__nv_bfloat16 *p, float4 v) {
+    const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    *reinterpret_cast<uint2 *>(p) = make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b));
+}
+__device__ __forceinline__ void st4(__half *p, float4 v) {
+    const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+    *reinterpret_cast<uint2 *>(p) = make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b));
+}
+// element i of a feature map whose type is only known at run time (residual reads off the hot loops)
+__device__ __forceinline__ float ld_feat(const void *p, int64_t i, int dtype) {
+    if (dtype == kBF16) return __bfloat162float(__ldg(static_cast<const __nv_bfloat16 *>(p) + i));
+    if (dtype == kF16) return __half2float(__ldg(static_cast<const __half *>(p) + i));
+    return __ldg(static_cast<const float *>(p) + i);
+}
+__host__ __device__ __forceinline__ int feat_esize(int dtype) { return dtype == kF32 ? 4 : 2; }
 
 // Per-(ref,src)-pair constants: M = A2·A1^-1 (row-major 3x3) and the epipole e2/e2.z.
 struct PairGeom {

@@ -141,7 +141,10 @@ __device__ unsigned long long g_pipe_cta[256 * 4];     // per CTA: globaltimer a
 #define PT(slot) do { } while (0)
 #endif
 
-template <int KPL>
+// LO: the operands have a lo part (fp32 / fp16 maps).  bf16 maps are their own hi part: no lo planes are gathered, GEMM1 is
+// the single product hi·hi and GEMM2 (whose β is fp32-derived) hi·β_hi + hi·β_lo.  The products that remain are issued in the
+// same order as with LO, and the ones left out are exact zeros, so both forms accumulate the same sums.
+template <int KPL, bool LO>
 __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const FusionArgs a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -240,8 +243,8 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                             for (int kk = 0; kk < nk; kk++) {
                                 const uint64_t a_hi = make_smem_desc(sa + kk * 2048, 8192, 1024), a_lo = desc_add(a_hi, PLANE_BYTES);
                                 const uint64_t b = make_smem_desc(sb + blk * PANEL_B2 + kk * 32, 16, 1024), b_lo = desc_add(b, 4096);
-                                if (h >> 1) { wgmma_m64n32<1>(o1, a_hi, b); wgmma_m64n32<1>(o1, a_hi, b_lo); wgmma_m64n32<1>(o1, a_lo, b); }
-                                else        { wgmma_m64n32<1>(o0, a_hi, b); wgmma_m64n32<1>(o0, a_hi, b_lo); wgmma_m64n32<1>(o0, a_lo, b); }
+                                if (h >> 1) { wgmma_m64n32<1>(o1, a_hi, b); wgmma_m64n32<1>(o1, a_hi, b_lo); if (LO) wgmma_m64n32<1>(o1, a_lo, b); }
+                                else        { wgmma_m64n32<1>(o0, a_hi, b); wgmma_m64n32<1>(o0, a_hi, b_lo); if (LO) wgmma_m64n32<1>(o0, a_lo, b); }
                             }
                             wg_commit();
                             wg_wait_all();
@@ -282,11 +285,11 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                         } else {
                             const float ov[4] = {o.x, o.y, o.z, o.w};
                             float *ob = a.out + (int64_t)d.n * a.out_stride[0] + (int64_t)y * a.out_stride[2] + (int64_t)x * a.out_stride[3];
-                            const float *rb = a.feat_ref + (int64_t)d.n * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
+                            const int64_t rb = (int64_t)d.n * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
 #pragma unroll
                             for (int e = 0; e < 4; e++) {
                                 float val = ov[e];
-                                if (a.add_ref) val += __ldg(rb + (int64_t)(c0 + e) * a.ref_stride[1]);
+                                if (a.add_ref) val += ld_feat(a.feat_ref, rb + (int64_t)(c0 + e) * a.ref_stride[1], a.ref_dtype);
                                 ob[(int64_t)(c0 + e) * a.out_stride[1]] = val;
                             }
                         }
@@ -337,7 +340,8 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                                 for (int ks = 0; ks < 4; ks++) {
                                     const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = desc_add(a_hi, PLANE_BYTES);
                                     const uint64_t b = make_smem_desc(sq + kp * PANEL_B2 + ks * 32, 16, 1024), b_lo = desc_add(b, 4096);
-                                    wgmma_m64n32<0>(sacc, a_hi, b); wgmma_m64n32<0>(sacc, a_hi, b_lo); wgmma_m64n32<0>(sacc, a_lo, b);
+                                    wgmma_m64n32<0>(sacc, a_hi, b);
+                                    if (LO) { wgmma_m64n32<0>(sacc, a_hi, b_lo); wgmma_m64n32<0>(sacc, a_lo, b); }
                                 }
                                 wg_commit();
                                 wg_wait_all();
@@ -784,7 +788,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         // consecutive lanes.  Completion: cp.async.mbarrier.arrive.noinc on the stage's mbarrier (count = 128 threads).
         // =====================================================================================================
         const int gt = tid - W_GATHER * 32, gj = gt & 7, gr = gt >> 3;
-        const __nv_bfloat16 *planes = a.ref_hi;          // [ref_hi | ref_lo | src_hi | src_lo], each [N*HW][C]
+        // [ref_hi | ref_lo | src_hi | src_lo] (LO) or [ref_hi | src_hi], each [N*HW][C]; a lo plane follows its hi plane
         const size_t plane_elems = (size_t)NHW * C;
         uint32_t qcount = 0, fcount = 0;
         const bool pt_on = gt == 0; (void)pt_on;
@@ -811,7 +815,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         auto gemm2_stages = [&](int jj) {
             const Desc &d = desc_at(jj);
             const int D16 = (d.D + 15) & ~15, nblk = (D16 + 63) >> 6;
-            const __nv_bfloat16 *src = planes + 2 * plane_elems + (size_t)d.n * HW * C;
+            const __nv_bfloat16 *src = a.src_hi + (size_t)d.n * HW * C;
             for (int blk = 0; blk < nblk; blk++) {               // (block of 64 union rows) outer, channel half inner: row addresses are
                 const int rows = min(64, D16 - blk * 64);        // computed once per block
                 uint32_t roff[4];
@@ -829,7 +833,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                                 const int ch = (h * 2 + pn) * 64 + gj * 8;
                                 if (ch < C) {
                                     cp16(stg + pn * 8192 + so, row + ch, true);
-                                    cp16(stg + PLANE_BYTES + pn * 8192 + so, row + plane_elems + ch, true);
+                                    if (LO) cp16(stg + PLANE_BYTES + pn * 8192 + so, row + plane_elems + ch, true);
                                 }
                             }
                         }
@@ -850,7 +854,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                 // ---- per half of the query panels (one half unless C > 256): the item's query rows as stacked panels
                 //      [hi 32 rows | lo 32 rows], then the GEMM1 stages (chunk, 64-channel panel) that multiply with them ----
                 const int D16 = (d.D + 15) & ~15, nch = (d.D + CHUNK - 1) / CHUNK;
-                const __nv_bfloat16 *src = planes + 2 * plane_elems + (size_t)d.n * HW * C;
+                const __nv_bfloat16 *src = a.src_hi + (size_t)d.n * HW * C;
                 for (int qh = 0; qh < NQH; qh++) {
                     const int npq = min(4, NP - qh * 4);
                     if (qcount >= 1) {
@@ -859,7 +863,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                     }
                     PT(16);
                     {
-                        const __nv_bfloat16 *ref = planes + (size_t)d.n * HW * C;
+                        const __nv_bfloat16 *ref = a.ref_hi + (size_t)d.n * HW * C;
 #pragma unroll
                         for (int it = 0; it < 2; it++) {
                             const int r = gr + 16 * it;
@@ -872,7 +876,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                                 if (kp < npq) {                 // channels beyond C are zero-filled: they are part of the MMA K range
                                     const bool ok = ch < C;
                                     cp16(so + kp * PANEL_B2, ok ? row + ch : row, ok);
-                                    cp16(so + kp * PANEL_B2 + 4096, ok ? row + plane_elems + ch : row, ok);
+                                    if (LO) cp16(so + kp * PANEL_B2 + 4096, ok ? row + plane_elems + ch : row, ok);
                                 }
                             }
                         }
@@ -895,7 +899,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                                     const __nv_bfloat16 *row = colp + roff[it];
                                     const uint32_t so = stg + so0 + (uint32_t)it * 2048u;
                                     cp16(so, row, ok);
-                                    cp16(so + PLANE_BYTES, row + plane_elems, ok);
+                                    if (LO) cp16(so + PLANE_BYTES, row + plane_elems, ok);
                                 }
                             }
                             arrive_async(&ct.f_full[fcount % NSTAGE]);
@@ -951,10 +955,12 @@ cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st) {
     const int HW = a.geom.H * a.geom.W;
     const int tiles = a.N * ((HW + P - 1) / P);
     const int kpl = (a.geom.K + 31) / 32;
-    void (*kern)(const FusionArgs) = kpl <= 1 ? epi_fusion_pipe_kernel<1> : (kpl <= 2 ? epi_fusion_pipe_kernel<2> : epi_fusion_pipe_kernel<4>);
+    const bool lo = a.src_lo != nullptr;
+    void (*kern)(const FusionArgs) = lo ? (kpl <= 1 ? epi_fusion_pipe_kernel<1, true> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, true> : epi_fusion_pipe_kernel<4, true>))
+                                        : (kpl <= 1 ? epi_fusion_pipe_kernel<1, false> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, false> : epi_fusion_pipe_kernel<4, false>));
     static thread_local int sms_cached = 0;
-    static thread_local bool attr_set[3] = {false, false, false};
-    const int ki = kpl <= 1 ? 0 : (kpl <= 2 ? 1 : 2);
+    static thread_local bool attr_set[6] = {false, false, false, false, false, false};
+    const int ki = (kpl <= 1 ? 0 : (kpl <= 2 ? 1 : 2)) + (lo ? 0 : 3);
     if (!attr_set[ki]) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_ALLOC);
         if (e != cudaSuccess) return e;

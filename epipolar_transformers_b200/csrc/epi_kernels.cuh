@@ -8,10 +8,12 @@ namespace epi {
 
 // Device-side view of one fused forward (built from EpiFusionParams by the ABI layer).
 struct FusionArgs {
-    const float *feat_ref;  int64_t ref_stride[4];
+    const float *feat_ref;  int64_t ref_stride[4];   // fp32 (the caller's map, or a fp32 copy of a low-precision one) ...
+    int ref_dtype;                            // ... except for the pipe kernel, which reads the caller's map in its own type (kF32/kBF16/kF16)
     const float *src_nhwc;                    // [N,H,W,C] contiguous, 16-byte aligned (zero-copy or staged) — warp kernel
     const __nv_bfloat16 *src_hi, *src_lo;     // [N,H,W,C] bf16 planes, src ≈ hi + lo — tile kernel
-    const __nv_bfloat16 *ref_hi, *ref_lo;     // same for feat_ref — sector tiles only
+    const __nv_bfloat16 *ref_hi, *ref_lo;     // same for feat_ref — sector tiles and pipe kernel
+                                              // (pipe kernel: lo planes are null for bf16 inputs, whose lo part is zero)
     const uint16_t *order;                    // [N,H*W] pixels sorted by epipolar angle — sector tiles only (else null)
     const float *P_ref, *P_src;
     const float *locs_in;
@@ -62,7 +64,8 @@ struct ZGemmArgs {
     const __nv_bfloat16 *x_hi, *x_lo;
     const __nv_bfloat16 *w_hi, *w_lo;         // Wf (+ I when ZRESIDUAL) [C out][C in] as bf16 (hi, lo) planes (written by the staging kernel)
     const float *Wf, *bf;
-    const float *ref;       int64_t ref_stride[4];
+    const void *ref;        int64_t ref_stride[4];   // element type ref_dtype
+    int ref_dtype;
     float *y;               int64_t y_stride[4];
     int N, C, HW, W, Npad;
     int z_residual, add_ref;
@@ -79,18 +82,22 @@ int fusion_pipe_plan_records(int N, int H, int W);
 bool fusion_tile_supported(const FusionArgs &a);
 bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, const GeomCfg &gc, cudaStream_t st);
-cudaError_t launch_split_planes(const float *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
-                                int H, int W, int *zero_me, cudaStream_t st);
+// `dtype` (kF32 / kBF16 / kF16): element type of the source map(s)
+cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
+                                int H, int W, int *zero_me, int dtype, cudaStream_t st);
 
-cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const float *src, const int64_t src_stride[4],
+// planes: [ref_hi | ref_lo | src_hi | src_lo] for fp32 / fp16 maps, [ref_hi | src_hi] for bf16 maps (their lo part is zero)
+cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int C,
                          int H, int W, const GeomCfg &gc, cudaStream_t st);
 
-cudaError_t launch_nchw_to_nhwc(const float *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, cudaStream_t st);
+cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
+                                cudaStream_t st);
 cudaError_t launch_z_epilogue(const ZArgs &z, cudaStream_t st);
-cudaError_t launch_unstage(const float *pm, const float *ref, const int64_t ref_stride[4], float *out, const int64_t out_stride[4],
-                           int N, int C, int H, int W, cudaStream_t st);
+// out_dtype != kF32 (a gradient rounded once) takes no residual
+cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
+                           const int64_t out_stride[4], int N, int C, int H, int W, cudaStream_t st);
 cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, const float *b, const float *mean,
                              const float *var, float eps, int C, float *wf, float *bf, cudaStream_t st);
 cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, int J, int H, int W, float radius, float downsample,

@@ -5,11 +5,15 @@
 //                      reference pixels sorted by epipolar angle (counting sort on a 12-bit angle key, ties by pixel index
 //                      => deterministic).  Pixels on one epipolar line of the reference view share one epipolar line in
 //                      the source view, so 32 consecutive list entries have nearly identical sets of bilinear taps.
-//   remaining blocks   [N,C,H,W] fp32 (any strides) -> pixel-major bf16 (hi, lo) planes [N,H*W,C] with x ≈ hi + lo, for
-//                      BOTH feature maps (reference -> planes 0,1; source -> planes 2,3 of one buffer), 64 x 64 tiles through
-//                      shared memory: coalesced float4 reads along pixels, 16-byte writes along channels.
+//   remaining blocks   [N,C,H,W] (any strides; fp32, bf16 or fp16 elements) -> pixel-major bf16 (hi, lo) planes [N,H*W,C] with
+//                      x ≈ hi + lo, for BOTH feature maps (reference -> planes 0,1; source -> planes 2,3 of one buffer), 64 x 64
+//                      tiles through shared memory: coalesced 4-pixel vector reads along pixels, 16-byte writes along channels.
+//                      fp16 values are split exactly like fp32 ones (hi + lo holds them exactly); a bf16 value is its own hi
+//                      part, so bf16 maps write hi planes only (reference -> plane 0, source -> plane 1).
 // Also zeroes the fused kernel's tile counter and error word.
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "epi_kernels.cuh"
 
@@ -50,10 +54,11 @@ extern "C" void epi_stage_timers_read(unsigned long long *out16) { cudaMemcpyFro
 #define ST(slot) do { } while (0)
 #endif
 
+template <typename T>
 struct StageArgs {
-    const float *ref, *src;
+    const T *ref, *src;
     int64_t ref_stride[4], src_stride[4];
-    __nv_bfloat16 *planes;            // [4][N*HW][C]: ref_hi, ref_lo, src_hi, src_lo
+    __nv_bfloat16 *planes;            // [4][N*HW][C]: ref_hi, ref_lo, src_hi, src_lo  (bf16 maps: [2][N*HW][C]: ref_hi, src_hi)
     const float *P_ref, *P_src;       // may be null (injected locations): no order, no pair constants
     PairGeom *pair_geom;              // [N]
     uint16_t *order;                  // [N][HW]
@@ -69,8 +74,11 @@ struct StageArgs {
 };
 
 // (min 5 blocks per SM: the layout-staging blocks need few registers; the rare order blocks may spill a little)
-__global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s) {
+template <typename T>
+__global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T> s) {
     using namespace stg;
+    constexpr bool LO = !std::is_same<T, __nv_bfloat16>::value;   // a bf16 value's lo part is zero: no lo planes
+    constexpr int NPL = LO ? 2 : 1;                               // planes per map
     extern __shared__ __align__(16) uint8_t dyn[];        // transposition tile [64 ch][65] fp32 | order blocks: histogram + pixel list
     float (*tile)[TPITCH] = reinterpret_cast<float (*)[TPITCH]>(dyn);
     const int t = threadIdx.x;
@@ -315,9 +323,9 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
     // cover its whole 128-byte row; the reader undoes the k ^ b order with four selects.
     uint32_t *whi = reinterpret_cast<uint32_t *>(dyn), *wlo = whi + TPX * 32;
     const int fq = t & 15, hsel = (t >> 4) & 1, fw = t >> 5;
-    auto fast_load = [&](const float *spn, int64_t scn, int c0n, int p0n, float4 *v) {
+    auto fast_load = [&](const T *spn, int64_t scn, int c0n, int p0n, float4 *v) {
 #pragma unroll
-        for (int i = 0; i < RPASS; i++) v[i] = __ldcs(reinterpret_cast<const float4 *>(spn + (int64_t)(c0n + 2 * fw + hsel + i * RPP) * scn + p0n + fq * 4));   // read once: streaming, keeps L2 for the planes
+        for (int i = 0; i < RPASS; i++) v[i] = ld4_cs(spn + (int64_t)(c0n + 2 * fw + hsel + i * RPP) * scn + p0n + fq * 4);   // read once: streaming, keeps L2 for the planes
     };
     auto fast_split = [&](const float4 *v) {            // registers -> (hi, lo) words in shared memory
 #pragma unroll
@@ -337,7 +345,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
                 const int px = 4 * fq + 2 * hsel + u, sw5 = (px >> 1) & 31;
                 const int pos = px * 32 + (((g ^ (sw5 >> 2)) << 2) | (k ^ (sw5 & 3)));
                 whi[pos] = *reinterpret_cast<const uint32_t *>(&hv);
-                wlo[pos] = *reinterpret_cast<const uint32_t *>(&lv);
+                if (LO) wlo[pos] = *reinterpret_cast<const uint32_t *>(&lv);
             }
         }
     };
@@ -352,7 +360,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
             if (sw5 & 2) { uint32_t x_; x_ = h4.x; h4.x = h4.z; h4.z = x_; x_ = h4.y; h4.y = h4.w; h4.w = x_; x_ = l4.x; l4.x = l4.z; l4.z = x_; x_ = l4.y; l4.y = l4.w; l4.w = x_; }
             const size_t o = ((size_t)nn * HW + p0n + px) * C + c0n + g * 8;
             *reinterpret_cast<uint4 *>(hin + o) = h4;
-            *reinterpret_cast<uint4 *>(lon + o) = l4;
+            if (LO) *reinterpret_cast<uint4 *>(lon + o) = l4;
         }
     };
     const size_t plane_elems_all = (size_t)s.N * HW * C;
@@ -383,7 +391,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
                 decode(nxt, mp2, nn2, c02, p02);
                 fast_load((mp2 ? s.src : s.ref) + (int64_t)nn2 * (mp2 ? s.src_stride[0] : s.ref_stride[0]), mp2 ? s.src_stride[1] : s.ref_stride[1], c02, p02, v);
             }
-            __nv_bfloat16 *hin = s.planes + (size_t)(2 * mp) * plane_elems_all;
+            __nv_bfloat16 *hin = s.planes + (size_t)(NPL * mp) * plane_elems_all;
             fast_store(hin, hin + plane_elems_all, nn, c0n, p0n);
             if (nxt >= nt) return;
             __syncthreads();
@@ -397,13 +405,13 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
     else map = s.do_src ? 1 : 0;
     const int n = lin / (tiles_p * tiles_c), rem = lin % (tiles_p * tiles_c);
     const int c0 = (rem / tiles_p) * TC, p0 = (rem % tiles_p) * TPX;
-    const float *base = map ? s.src : s.ref;
+    const T *base = map ? s.src : s.ref;
     const int64_t *strd = map ? s.src_stride : s.ref_stride;
     const int64_t sn = strd[0], sc = strd[1], sh = strd[2], sw = strd[3];
-    const float *sp = base + (int64_t)n * sn;
+    const T *sp = base + (int64_t)n * sn;
     const size_t plane_elems = (size_t)s.N * HW * C;
-    __nv_bfloat16 *hi = s.planes + (size_t)(2 * map) * plane_elems, *lo = hi + plane_elems;
-    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(sp) & 15) == 0);
+    __nv_bfloat16 *hi = s.planes + (size_t)(NPL * map) * plane_elems, *lo = hi + plane_elems;
+    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(sp) & (4 * sizeof(T) - 1)) == 0);
     if (vec && sc != 1 && p0 + TPX <= HW && c0 + TC <= C) {
         float4 v[RPASS];
         fast_load(sp, sc, c0, p0, v);
@@ -420,10 +428,10 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
             const int c = c0 + cy + i * RPP, p = p0 + q * 4;
             v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (c < C) {
-                if (vec && p + 3 < HW) v[i] = __ldg(reinterpret_cast<const float4 *>(sp + c * sc + p));
+                if (vec && p + 3 < HW) v[i] = ld4_nc(sp + c * sc + p);
                 else {
                     float e[4] = {0.f, 0.f, 0.f, 0.f};
-                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = __ldg(sp + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw);
+                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = to_f32(__ldg(sp + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw));
                     v[i] = make_float4(e[0], e[1], e[2], e[3]);
                 }
             }
@@ -439,7 +447,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
 #pragma unroll
         for (int i = 0; i < TPX / PPP; i++) {
             const int p = p0 + py + i * PPP, c = c0 + cx;
-            tile[cx][py + i * PPP] = (c < C && p < HW) ? __ldg(sp + c + (p / W) * sh + (p % W) * sw) : 0.f;
+            tile[cx][py + i * PPP] = (c < C && p < HW) ? to_f32(__ldg(sp + c + (p / W) * sh + (p % W) * sw)) : 0.f;
         }
     }
     __syncthreads();
@@ -461,16 +469,17 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs s
             }
             const size_t o = ((size_t)n * HW + p) * C + c;
             *reinterpret_cast<uint4 *>(hi + o) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4 *>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
+            if (LO) *reinterpret_cast<uint4 *>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
         }
     }
 }
 
-cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const float *src, const int64_t src_stride[4],
-                         __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
-                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int C,
-                         int H, int W, const GeomCfg &gc, cudaStream_t st) {
-    StageArgs s;
+template <typename T>
+static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], const T *src, const int64_t src_stride[4],
+                                  __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
+                                  float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
+                                  int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
+    StageArgs<T> s;
     s.ref = ref; s.src = src;
     for (int i = 0; i < 4; i++) { s.ref_stride[i] = ref_stride[i]; s.src_stride[i] = src_stride[i]; }
     s.planes = planes; s.P_ref = P_ref; s.P_src = P_src; s.pair_geom = pair_geom; s.order = order; s.order_key = order_key; s.Wf = Wf; s.w_planes = w_planes; s.w_add_identity = w_add_identity;
@@ -484,7 +493,7 @@ cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const fl
     static thread_local size_t smem_set = 0;
     auto ensure = [&](size_t smem) -> cudaError_t {
         if (smem + 1024 > 48 * 1024 && smem > smem_set) {        // (+ the kernel's small static arrays)
-            cudaError_t e = cudaFuncSetAttribute(epi_stage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            cudaError_t e = cudaFuncSetAttribute(epi_stage_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
             smem_set = smem;
         }
@@ -493,17 +502,17 @@ cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const fl
     // Shared memory is a per-launch size: above 64 KB the order blocks' pixel list would cut the residency of every transposition
     // block of the same launch, so maps that large order their pixels in a launch of their own (a no-op on a cached camera pair).
     if (s.do_order && smem_order > 64 * 1024) {
-        StageArgs o = s;
+        StageArgs<T> o = s;
         o.do_ref = 0; o.do_src = 0; o.Wf = nullptr; o.w_planes = nullptr; o.persist = 0;
         cudaError_t e = ensure(smem_order);
         if (e != cudaSuccess) return e;
-        e = launch_pdl(epi_stage_kernel, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o);
+        e = launch_pdl(epi_stage_kernel<T>, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o);
         if (e != cudaSuccess) return e;
         s.do_order = 0; s.zero_words = nullptr;                  // the order launch has zeroed the counters
     }
     // streaming blocks when every tile of both maps is a whole, 16-byte-vectorisable NCHW tile
-    auto whole = [&](const float *b, const int64_t *sd) {
-        return sd[3] == 1 && sd[2] == W && sd[1] % 4 == 0 && sd[0] % 4 == 0 && sd[1] != 1 && (reinterpret_cast<uintptr_t>(b) & 15) == 0;
+    auto whole = [&](const T *b, const int64_t *sd) {
+        return sd[3] == 1 && sd[2] == W && sd[1] % 4 == 0 && sd[0] % 4 == 0 && sd[1] != 1 && (reinterpret_cast<uintptr_t>(b) & (4 * sizeof(T) - 1)) == 0;
     };
     static thread_local int sms_cached = 0;
     if (!sms_cached) {
@@ -520,7 +529,21 @@ cudaError_t launch_stage(const float *ref, const int64_t ref_stride[4], const fl
     const size_t smem = (s.do_order && smem_order > smem_tile) ? smem_order : smem_tile;
     cudaError_t e = ensure(smem);
     if (e != cudaSuccess) return e;
-    return launch_pdl(epi_stage_kernel, dim3((unsigned)grid), dim3(stg::NT), smem, st, s);
+    return launch_pdl(epi_stage_kernel<T>, dim3((unsigned)grid), dim3(stg::NT), smem, st, s);
+}
+
+cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
+                         __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
+                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int C,
+                         int H, int W, const GeomCfg &gc, cudaStream_t st) {
+    if (dtype == kBF16)
+        return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
+    if (dtype == kF16)
+        return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
+    return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
+                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
 }
 
 }  // namespace epi

@@ -37,13 +37,25 @@ def _strides4(t: torch.Tensor):
     return (ctypes.c_int64 * 4)(*t.stride())
 
 
-def _check_feat(name, t):
-    if not isinstance(t, torch.Tensor) or t.dim() != 4:
-        raise ValueError("%s must be a 4-D tensor [N,C,H,W]" % name)
-    if not t.is_cuda:
-        raise RuntimeError("%s is on %s: the CUDA epipolar path has no CPU implementation" % (name, t.device))
-    if t.dtype != torch.float32:
-        raise TypeError("%s must be float32 (got %s)" % (name, t.dtype))
+# element types the kernels read natively (EPI_DTYPE_*); bf16 / fp16 maps give the fp32 result of their exact values
+FEAT_DTYPES = {torch.float32: _lib.EPI_DTYPE_F32, torch.bfloat16: _lib.EPI_DTYPE_BF16, torch.float16: _lib.EPI_DTYPE_F16}
+
+
+def _check_feat_pair(feat_ref, feat_src, out=None):
+    """Both maps: 4-D, one supported dtype, on the GPU (a caller-supplied `out` must be float32).  -> EPI_DTYPE_* code."""
+    for name, t in (("feat_ref", feat_ref), ("feat_src", feat_src)):
+        if not isinstance(t, torch.Tensor) or t.dim() != 4:
+            raise ValueError("%s must be a 4-D tensor [N,C,H,W]" % name)
+        if t.dtype not in FEAT_DTYPES:
+            raise TypeError("%s must be float32, bfloat16 or float16 (got %s)" % (name, t.dtype))
+    if feat_ref.dtype != feat_src.dtype:
+        raise TypeError("feat_ref and feat_src must have the same dtype (got %s and %s)" % (feat_ref.dtype, feat_src.dtype))
+    if out is not None and out.dtype != torch.float32:
+        raise TypeError("out must be float32 (got %s): the fused feature is computed and stored in float32" % out.dtype)
+    for name, t in (("feat_ref", feat_ref), ("feat_src", feat_src)):
+        if not t.is_cuda:
+            raise RuntimeError("%s is on %s: the CUDA epipolar path has no CPU implementation" % (name, t.device))
+    return FEAT_DTYPES[feat_ref.dtype]
 
 
 class FusionState:
@@ -68,15 +80,16 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
                     variant="auto", out=None, state: Optional[FusionState] = None):
     """Functional form of the fused forward.  Returns (out, corr_pos|None, attn|None, sample_locs|None).
 
-    feat_ref/feat_src: CUDA float32 [N,C,H,W] (NCHW or channels_last strides).
+    feat_ref/feat_src: CUDA [N,C,H,W] (NCHW or channels_last strides), both float32, both bfloat16 or both float16 (what a
+      backbone under torch.autocast produces).  The result is the float32 computation on the exact input values, and every
+      output (including a caller-supplied `out`) is float32.
     P_ref/P_src: [N,3,4] (cast to float32 like modeling/model.py:183-195).
     z_folded: optional (Wf [C,C], bf [C]) from `fold_z_bn` (eval-mode epilogue, epipolar.py:249-253).
     sample_locs_in: optional [K,N,H,W,2] normalised locations replacing the fused geometry.
     state: optional FusionState (persistent workspace + camera-keyed cache); without it scratch is allocated per call.
     """
     lib = _lib.load()
-    _check_feat("feat_ref", feat_ref)
-    _check_feat("feat_src", feat_src)
+    dcode = _check_feat_pair(feat_ref, feat_src, out)
     if feat_ref.shape != feat_src.shape or feat_ref.device != feat_src.device:
         raise ValueError("feat_ref and feat_src must have the same shape and device")
     N, C, H, W = feat_ref.shape
@@ -93,13 +106,13 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
         if tuple(sample_locs_in.shape) != (K, N, H, W, 2):
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
     if out is None:
-        out = torch.empty_like(feat_ref)           # preserves NCHW / channels_last
+        out = torch.empty_like(feat_ref, dtype=torch.float32)           # preserves NCHW / channels_last
     attn = torch.empty((N, K, H, W), device=dev, dtype=torch.float32) if want_attn else None
     corr = torch.empty((N, H, W, 2), device=dev, dtype=torch.float32) if want_corr else None
     locs = torch.empty((K, N, H, W, 2), device=dev, dtype=torch.float32) if want_locs else None
 
     vcode = _lib.VARIANTS[variant] if isinstance(variant, str) else int(variant)
-    key = (dev, N, C, H, W, int(K), feat_ref.stride(), feat_src.stride(), out.stride(), z_folded is not None, vcode,
+    key = (dev, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
     if state is not None and state.key == key:
@@ -113,6 +126,7 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
         p.align_corners = int(bool(align_corners)); p.correct_normalize = int(bool(correct_normalize))
         p.z_residual = int(bool(z_residual)); p.add_ref_residual = int(bool(add_ref_residual))
         p.variant = vcode
+        p.feat_dtype = dcode
     p.feat_ref = feat_ref.data_ptr(); p.feat_src = feat_src.data_ptr()
     p.P_ref = P_ref.data_ptr() if sample_locs_in is None else None
     p.P_src = P_src.data_ptr() if sample_locs_in is None else None
@@ -150,8 +164,10 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
                              sample_locs_in=None, grad_keys=True, grad_vals=True, need_ref=True, need_src=True):
     """Backward of `epipolar_fusion` without the z epilogue: returns (dL/dfeat_ref | None, dL/dfeat_src | None).
     Restates autograd through epipolar.py:188-247 (grid_sample x2, mul/sum, ==0 mask, softmax, weighted sum);
-    grad_keys / grad_vals = 'other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD (:141-153)."""
+    grad_keys / grad_vals = 'other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD (:141-153).
+    The gradients have the maps' dtype (computed in float32, rounded once); grad_out is float32 like the forward's `out`."""
     lib = _lib.load()
+    dcode = _check_feat_pair(feat_ref, feat_src)
     N, C, H, W = feat_ref.shape
     dev = feat_ref.device
     grad_out = grad_out if grad_out.dtype == torch.float32 else grad_out.float()
@@ -182,6 +198,7 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
     p.downsample = float(downsample); p.img_scale = float(img_scale); p.eps = _EPSILON; p.softmax_scale = float(softmax_scale)
     p.align_corners = int(bool(align_corners)); p.correct_normalize = int(bool(correct_normalize))
     p.grad_keys = int(bool(grad_keys)); p.grad_vals = int(bool(grad_vals))
+    p.feat_dtype = dcode
     nbytes = lib.epi_fusion_backward_workspace_bytes(ctypes.byref(p))
     ws = torch.empty(max(nbytes, 1), device=dev, dtype=torch.uint8)
     p.workspace = ws.data_ptr(); p.workspace_bytes = nbytes
@@ -193,6 +210,7 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
 
 class _FusionFn(torch.autograd.Function):
     """The fused attention under autograd (no z epilogue: conv/BN stay in PyTorch when gradients are needed).
+    The gradients of bfloat16 / float16 maps come back in their dtype.
     The backward samples at the locations the forward emitted rather than re-deriving them from the cameras: the forward
     kernels round the line geometry differently, and with ill-conditioned cameras a recomputation moves samples by
     thousandths of a feature pixel, enough to put the gradients ~1e-3 (relative) off the function the forward computed."""
@@ -216,7 +234,7 @@ class _FusionFn(torch.autograd.Function):
         feat_ref, feat_src, P_ref, P_src, attn, locs = ctx.saved_tensors
         o = ctx.opts
         if g_out is None:
-            g_out = torch.zeros_like(feat_ref)
+            g_out = torch.zeros_like(feat_ref, dtype=torch.float32)
         need_ref, need_src = ctx.needs_input_grad[0], ctx.needs_input_grad[1] and (o["grad_keys"] or o["grad_vals"])
         f = o["fwd"]
         g_ref, g_src = epipolar_fusion_backward(

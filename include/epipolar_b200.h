@@ -13,7 +13,9 @@
  * here (epipolar_transformers_b200/epipolar.py) does exactly that.
  *
  * Conventions: plain pointers + sizes, no torch types.  All tensor pointers are DEVICE
- * pointers to float32 unless a name ends in _host.  The library never allocates persistent
+ * pointers to float32 unless a name ends in _host, except the feature maps feat_ref / feat_src and the backward's
+ * grad_ref / grad_src, whose element type is the params' feat_dtype (EPI_DTYPE_*: float32, bfloat16 or float16; both maps
+ * share it).  Every other output stays float32.  The library never allocates persistent
  * device memory; the caller passes a workspace.  Every entry point is re-entrant, takes the
  * CUDA stream explicitly, never synchronises the device, and returns 0 on success or a
  * negative EPI_E* code (epi_last_error() gives a thread-local message).
@@ -28,12 +30,18 @@
 extern "C" {
 #endif
 
-#define EPI_ABI_VERSION 2
+#define EPI_ABI_VERSION 3
 
 #define EPI_OK 0
 #define EPI_EINVAL (-1)       /* bad argument / unsupported shape */
 #define EPI_EWORKSPACE (-2)   /* workspace too small */
 #define EPI_ECUDA (-3)        /* CUDA runtime error at launch (message has the cudaError string) */
+
+/* element type of the feature maps (EpiFusionParams.feat_dtype, EpiFusionBwdParams.feat_dtype).  The result is the float32
+ * computation applied to the exact input values: bfloat16 and float16 values are exact (hi, lo) bf16 pairs of the operand split. */
+#define EPI_DTYPE_F32 0
+#define EPI_DTYPE_BF16 1
+#define EPI_DTYPE_F16 2
 
 /* kernel variants (EpiFusionParams.variant) */
 #define EPI_VARIANT_AUTO 0    /* pipelined kernel when the shape allows, else sector / block tiles, else warp */
@@ -44,9 +52,9 @@ extern "C" {
 
 typedef struct EpiFusionParams {
     /* ---- inputs ---------------------------------------------------------------------- */
-    const float *feat_ref;        /* [N,C,H,W] logical; element strides below (NCHW or channels-last) */
+    const void *feat_ref;         /* [N,C,H,W] logical, element type feat_dtype; element strides below (NCHW or channels-last) */
     int64_t ref_stride[4];
-    const float *feat_src;        /* [N,C,H,W] logical */
+    const void *feat_src;         /* [N,C,H,W] logical, element type feat_dtype */
     int64_t src_stride[4];
     const float *P_ref;           /* [N,3,4] contiguous: KRT of the reference view  (forward arg P1) */
     const float *P_src;           /* [N,3,4] contiguous: KRT of the source view     (forward arg P2) */
@@ -75,7 +83,8 @@ typedef struct EpiFusionParams {
     int32_t z_residual;           /* cfg.EPIPOLAR.ZRESIDUAL (only with z_weight_folded) */
     int32_t add_ref_residual;     /* 1: also add feat_ref (the caller's `ret + feat`, resnet.py:388) */
     int32_t variant;              /* EPI_VARIANT_* */
-    int32_t reserved[3];
+    int32_t feat_dtype;           /* EPI_DTYPE_* of feat_ref and feat_src (ABI v3; 0 = float32) */
+    int32_t reserved[2];
     /* ---- optional persistent state (ABI v2) -------------------------------------------- */
     void *cache;                  /* device memory the caller keeps alive ACROSS calls and zero-fills once, or NULL.  Holds the
                                      per-pair constants and the epipolar pixel order keyed by (P_ref, P_src, H, W, downsample,
@@ -107,9 +116,9 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream);
  * grad_keys / grad_vals select the OTHER_GRAD members 'other1' / 'other2' (:141-153).  The z conv + BN of training mode
  * stay in PyTorch, so `grad_out` is the gradient w.r.t. the PRE-z fused feature. */
 typedef struct EpiFusionBwdParams {
-    const float *feat_ref;        /* [N,C,H,W] logical, strides below */
+    const void *feat_ref;         /* [N,C,H,W] logical, element type feat_dtype, strides below */
     int64_t ref_stride[4];
-    const float *feat_src;
+    const void *feat_src;         /* element type feat_dtype */
     int64_t src_stride[4];
     const float *P_ref, *P_src;   /* [N,3,4] */
     const float *sample_locs_in;  /* optional, as in the forward */
@@ -117,9 +126,9 @@ typedef struct EpiFusionBwdParams {
     const float *grad_out;        /* [N,C,H,W] logical: dL/d(fused feature) */
     int64_t gout_stride[4];
     const float *grad_attn;       /* optional [N,K,H,W] contiguous: dL/d(attention output) */
-    float *grad_ref;              /* optional out [N,C,H,W] logical: dL/dfeat_ref */
+    void *grad_ref;               /* optional out [N,C,H,W] logical, element type feat_dtype: dL/dfeat_ref (fp32, rounded once) */
     int64_t gref_stride[4];
-    float *grad_src;              /* optional out [N,C,H,W] logical: dL/dfeat_src (overwritten, not accumulated) */
+    void *grad_src;               /* optional out [N,C,H,W] logical, element type feat_dtype: dL/dfeat_src (overwritten, not accumulated) */
     int64_t gsrc_stride[4];
     void *workspace;
     size_t workspace_bytes;       /* >= epi_fusion_backward_workspace_bytes(p) */
@@ -127,7 +136,8 @@ typedef struct EpiFusionBwdParams {
     float downsample, img_scale, eps, softmax_scale;
     int32_t align_corners, correct_normalize;
     int32_t grad_keys, grad_vals; /* 'other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD */
-    int32_t reserved[4];
+    int32_t feat_dtype;           /* EPI_DTYPE_* of feat_ref, feat_src, grad_ref and grad_src (ABI v3; 0 = float32) */
+    int32_t reserved[3];
 } EpiFusionBwdParams;
 
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p);
