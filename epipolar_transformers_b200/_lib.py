@@ -18,7 +18,7 @@ VARIANTS = {"auto": EPI_VARIANT_AUTO, "warp": EPI_VARIANT_WARP, "tile": EPI_VARI
             "pipe": EPI_VARIANT_PIPE}
 
 EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_fusion_cache_bytes", "epi_fusion_forward_f32",
-           "epi_fusion_backward_workspace_bytes", "epi_fusion_backward_f32", "epi_find_peaks_f32",
+           "epi_fusion_backward_workspace_bytes", "epi_fusion_backward_f32", "epi_find_peaks_f32", "epi_find_peaks_best_f32",
            "epi_sample_locs_f32", "epi_fold_z_bn_f32", "epi_last_launch_count", "epi_umma_selftest",
            "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3")
 
@@ -39,7 +39,7 @@ class EpiFusionParams(ctypes.Structure):
         ("downsample", ctypes.c_float), ("img_scale", ctypes.c_float), ("eps", ctypes.c_float), ("softmax_scale", ctypes.c_float),
         ("align_corners", ctypes.c_int32), ("correct_normalize", ctypes.c_int32), ("z_residual", ctypes.c_int32),
         ("add_ref_residual", ctypes.c_int32), ("variant", ctypes.c_int32), ("feat_dtype", ctypes.c_int32),
-        ("reserved", ctypes.c_int32 * 2),
+        ("n_src", ctypes.c_int32), ("reserved", ctypes.c_int32 * 1),
         ("cache", ctypes.c_void_p), ("cache_bytes", ctypes.c_size_t),
     ]
 
@@ -96,6 +96,9 @@ def load():
     lib.epi_find_peaks_f32.restype = ctypes.c_int
     lib.epi_find_peaks_f32.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                        ctypes.c_int32, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int32, ctypes.c_void_p]
+    lib.epi_find_peaks_best_f32.restype = ctypes.c_int
+    lib.epi_find_peaks_best_f32.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int32] * 5 + \
+        [ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_int32, ctypes.c_void_p]
     lib.epi_sample_locs_f32.restype = ctypes.c_int
     lib.epi_sample_locs_f32.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                         ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_float, ctypes.c_float,

@@ -20,10 +20,15 @@ int fail(int code, const char *fmt, const char *detail = "") {
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
+// source views per reference item (EpiFusionParams.n_src: 0 and 1 both mean one)
+inline int n_sources(const EpiFusionParams *p) { return p->n_src > 1 ? p->n_src : 1; }
+// (reference, source) pairs = items of feat_src, out, attn, corr_pos and the sample locations
+inline int n_pairs(const EpiFusionParams *p) { return n_sources(p) * p->N; }
+
 bool src_is_channels_last(const EpiFusionParams *p) {
     const int64_t *s = p->src_stride;
     const int64_t C = p->C, H = p->H, W = p->W;
-    return s[1] == 1 && s[3] == C && s[2] == W * C && (p->N == 1 || s[0] == H * W * C) &&
+    return s[1] == 1 && s[3] == C && s[2] == W * C && (n_pairs(p) == 1 || s[0] == H * W * C) &&
            (reinterpret_cast<uintptr_t>(p->feat_src) % 16 == 0);
 }
 
@@ -49,27 +54,31 @@ bool want_tile(const EpiFusionParams *p) {
     return epi::fusion_tile_shape_ok(p->C, p->H, p->W, p->K, p->sample_locs_in != nullptr);
 }
 
+// Sizes: `ref_map` is one fp32 copy of the N reference items, `map` one fp32 map of the S·N pairs (source items, fused features).
+// The reference planes are staged once however many sources they are fused with.
 Plan make_plan(const EpiFusionParams *p) {
     Plan pl;
-    const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
+    const size_t ref_map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
+    const size_t map = (size_t)n_pairs(p) * p->C * p->H * p->W * sizeof(float);
+    const size_t NP = (size_t)n_pairs(p);
     const bool lowp = p->feat_dtype != EPI_DTYPE_F32;
     pl.pipe = want_pipe(p);
     if (pl.pipe) {
-        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes (bytes of two fp32 maps; bf16 maps: [ref_hi | src_hi], one fp32 map),
-        // pre-z planes, pixel order, pair constants
+        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes (bytes of one fp32 reference map + one fp32 source map; bf16 maps:
+        // [ref_hi | src_hi], half of that), pre-z planes, pixel order, pair constants
         pl.has_z = p->z_weight_folded != nullptr;
         size_t off = 0;
-        pl.off_ref = off; off += align_up(p->feat_dtype == EPI_DTYPE_BF16 ? map : 2 * map);
+        pl.off_ref = off; off += align_up(p->feat_dtype == EPI_DTYPE_BF16 ? (ref_map + map) / 2 : ref_map + map);
         // pre-z planes (z path) or the pixel-major fp32 plane the fused kernel writes when the caller's tensor is NCHW
         pl.unstage = !pl.has_z && !(p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0);
         if (pl.has_z || pl.unstage) { pl.off_prez = off; off += align_up(map); }
         pl.off_counter = off; off += 256;
         if (pl.has_z && epi::zgemm_supported(p->C)) { pl.off_wplanes = off; off += align_up((size_t)p->C * p->C * 4); }
         pl.ref32 = lowp && pl.has_z && !epi::zgemm_supported(p->C) && p->add_ref_residual;      // the fp32 z epilogue's residual
-        if (pl.ref32) { pl.off_ref32 = off; off += align_up(map); }
+        if (pl.ref32) { pl.off_ref32 = off; off += align_up(ref_map); }
         if (!p->cache) {               // no persistent cache: pixel order and pair constants are rebuilt in the workspace every call
-            pl.off_order = off; off += align_up((size_t)p->N * p->H * p->W * sizeof(uint16_t));
-            pl.off_geom = off; off += align_up((size_t)p->N * sizeof(epi::PairGeom));
+            pl.off_order = off; off += align_up(NP * p->H * p->W * sizeof(uint16_t));
+            pl.off_geom = off; off += align_up(NP * sizeof(epi::PairGeom));
         }
         pl.total = off;
         return pl;
@@ -83,13 +92,13 @@ Plan make_plan(const EpiFusionParams *p) {
     pl.has_z = p->z_weight_folded != nullptr;
     pl.ref32 = lowp;                                         // these kernels read the query (and the residual) as fp32
     size_t off = 0;
-    if (pl.ref32) { pl.off_ref32 = off; off += align_up(map); }
+    if (pl.ref32) { pl.off_ref32 = off; off += align_up(ref_map); }
     if (pl.stage_src) { pl.off_src = off; off += align_up(map); }
     if (pl.has_z) { pl.off_prez = off; off += align_up(map); }
     if (pl.tile) { pl.off_counter = off; off += 256; }
     if (pl.sector) {
-        pl.off_ref = off; off += align_up(map);
-        pl.off_order = off; off += align_up((size_t)p->N * p->H * p->W * sizeof(uint16_t));
+        pl.off_ref = off; off += align_up(ref_map);
+        pl.off_order = off; off += align_up(NP * p->H * p->W * sizeof(uint16_t));
     }
     pl.total = off;
     return pl;
@@ -106,6 +115,15 @@ int validate(const EpiFusionParams *p) {
     if (p->z_weight_folded && !p->z_bias_folded) return fail(EPI_EINVAL, "z_bias_folded required with z_weight_folded");
     if (p->variant < EPI_VARIANT_AUTO || p->variant > EPI_VARIANT_PIPE) return fail(EPI_EINVAL, "unknown variant");
     if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    if (p->n_src < 0) return fail(EPI_EINVAL, "n_src must be >= 0 (0 or 1: one source view per reference item)");
+    if (p->n_src > 1) {
+        // the layout, transposition and z epilogue kernels put the item in the grid's z dimension; the pipelined kernel numbers
+        // its per-pair work records, and the staging kernel its tiles, in 32-bit ints
+        const int64_t np = (int64_t)p->n_src * p->N, hw = (int64_t)p->H * p->W;
+        if (np > 65535) return fail(EPI_EINVAL, "n_src * N must be <= 65535 (grid z dimension of the per-item kernels)");
+        if (np * ((hw + 31) / 32 + 1) + p->n_src * 256 > INT32_MAX || 2 * np * ((hw + 63) / 64) * ((p->C + 63) / 64) > INT32_MAX || np * hw > INT32_MAX)
+            return fail(EPI_EINVAL, "n_src * N * H * W too large: per-pair work records and staging tiles are counted in int32");
+    }
     if (p->z_weight_folded && (reinterpret_cast<uintptr_t>(p->z_weight_folded) % 16 != 0 || reinterpret_cast<uintptr_t>(p->z_bias_folded) % 4 != 0))
         return fail(EPI_EINVAL, "z_weight_folded must be 16-byte aligned (contiguous [C,C]) and z_bias_folded 4-byte aligned");
     return EPI_OK;
@@ -155,15 +173,17 @@ float epi_kernel_timing_last_ms(void) {
     return ms;
 }
 
+// per pair: key (32 words), constants, pixel order, work records of the pipelined kernel
 size_t epi_fusion_cache_bytes(const EpiFusionParams *p) {
-    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0 || !want_pipe(p)) return 0;
-    return align_up((size_t)p->N * 32 * sizeof(float)) + align_up((size_t)p->N * sizeof(epi::PairGeom)) +
-           align_up((size_t)p->N * p->H * p->W * sizeof(uint16_t)) +
-           align_up((size_t)epi::fusion_pipe_plan_records(p->N, p->H, p->W) * epi::fusion_pipe_plan_record_bytes());
+    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0 || p->n_src < 0 || !want_pipe(p)) return 0;
+    const size_t NP = (size_t)n_pairs(p);
+    return align_up(NP * 32 * sizeof(float)) + align_up(NP * sizeof(epi::PairGeom)) +
+           align_up(NP * p->H * p->W * sizeof(uint16_t)) +
+           align_up((size_t)epi::fusion_pipe_plan_records((int)NP, p->N, p->H, p->W) * epi::fusion_pipe_plan_record_bytes());
 }
 
 size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) {
-    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0) return 0;
+    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0 || p->n_src < 0) return 0;
     return make_plan(p).total;
 }
 
@@ -185,12 +205,13 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     }
 
     const int dt = p->feat_dtype;
+    const int NP = n_pairs(p);          // pairs: items of feat_src and of every output; feat_ref has p->N items
     epi::FusionArgs a;
     memset(&a, 0, sizeof(a));
     a.feat_ref = static_cast<const float *>(p->feat_ref); a.ref_dtype = dt;
     a.P_ref = p->P_ref; a.P_src = p->P_src; a.locs_in = p->sample_locs_in;
     a.attn = p->attn; a.corr_pos = p->corr_pos; a.locs_out = p->sample_locs_out;
-    a.N = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale;
+    a.N = NP; a.n_ref = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale;
     for (int i = 0; i < 4; i++) a.ref_stride[i] = p->ref_stride[i];
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
     // fp32 kernels that read feat_ref get a channels-last fp32 copy of a low-precision map
@@ -199,7 +220,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
 
     if (p->variant == EPI_VARIANT_PIPE && !pl.pipe) return fail(EPI_EINVAL, "pipe variant does not support this shape");
     if (pl.pipe) {
-        const size_t elems = (size_t)p->N * p->C * p->H * p->W;
+        const size_t ref_elems = (size_t)p->N * p->C * p->H * p->W, elems = (size_t)NP * p->C * p->H * p->W;
         __nv_bfloat16 *planes = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_ref);
         int *words = reinterpret_cast<int *>(ws + pl.off_counter);
         const bool have_P = p->P_ref && p->P_src;
@@ -211,11 +232,11 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
             if (reinterpret_cast<uintptr_t>(p->cache) % 256 != 0) return fail(EPI_EINVAL, "cache must be 256-byte aligned");
             char *cb = static_cast<char *>(p->cache);
             okey = reinterpret_cast<float *>(cb);
-            pg = reinterpret_cast<epi::PairGeom *>(cb + align_up((size_t)p->N * 32 * sizeof(float)));
-            order = reinterpret_cast<uint16_t *>(cb + align_up((size_t)p->N * 32 * sizeof(float)) + align_up((size_t)p->N * sizeof(epi::PairGeom)));
+            pg = reinterpret_cast<epi::PairGeom *>(cb + align_up((size_t)NP * 32 * sizeof(float)));
+            order = reinterpret_cast<uint16_t *>(cb + align_up((size_t)NP * 32 * sizeof(float)) + align_up((size_t)NP * sizeof(epi::PairGeom)));
             if (have_P) {                      // cached work items of the fused kernel, valid per pair for the epoch stored in key slot 31
-                a.plan_cache = reinterpret_cast<uint8_t *>(order) + align_up((size_t)p->N * p->H * p->W * sizeof(uint16_t));
-                a.plan_records = epi::fusion_pipe_plan_records(p->N, p->H, p->W);
+                a.plan_cache = reinterpret_cast<uint8_t *>(order) + align_up((size_t)NP * p->H * p->W * sizeof(uint16_t));
+                a.plan_records = epi::fusion_pipe_plan_records(NP, p->N, p->H, p->W);
                 a.pair_epoch = reinterpret_cast<const uint32_t *>(okey) + 31;
             }
         } else {
@@ -226,12 +247,12 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         const bool z_planes = pl.has_z && epi::zgemm_supported(p->C);
         __nv_bfloat16 *wpl = z_planes ? reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_wplanes) : nullptr;
         e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, planes, p->P_ref, p->P_src, pg, order, okey,
-                              z_planes ? p->z_weight_folded : nullptr, wpl, p->z_residual ? 1 : 0, words, p->N, p->C, p->H, p->W, a.geom, st);
+                              z_planes ? p->z_weight_folded : nullptr, wpl, p->z_residual ? 1 : 0, words, NP, p->N, p->C, p->H, p->W, a.geom, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
         launches += (order && (size_t)p->H * p->W * 2 + 16384 > 64 * 1024) ? 2 : 1;      // large maps order their pixels in a launch of their own
         w_hi = wpl; w_lo = wpl ? wpl + (size_t)p->C * p->C : nullptr;
-        if (dt == EPI_DTYPE_BF16) { a.ref_hi = planes; a.src_hi = planes + elems; }       // no lo planes: the pipe kernel's LO = false form
-        else { a.ref_hi = planes; a.ref_lo = planes + elems; a.src_hi = planes + 2 * elems; a.src_lo = planes + 3 * elems; }
+        if (dt == EPI_DTYPE_BF16) { a.ref_hi = planes; a.src_hi = planes + ref_elems; }       // no lo planes: the pipe kernel's LO = false form
+        else { a.ref_hi = planes; a.ref_lo = planes + ref_elems; a.src_hi = planes + 2 * ref_elems; a.src_lo = planes + 2 * ref_elems + elems; }
         a.order = order; a.pair_geom = pg; a.tile_counter = words; a.err_flag = words + 1;
     } else
     if (p->variant == EPI_VARIANT_TILE && !pl.tile) return fail(EPI_EINVAL, "tile variant does not support this shape");
@@ -245,9 +266,9 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     }
     if (pl.tile) {
         __nv_bfloat16 *hi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_src);
-        __nv_bfloat16 *lo = hi + (size_t)p->N * p->C * p->H * p->W;
+        __nv_bfloat16 *lo = hi + (size_t)NP * p->C * p->H * p->W;
         a.tile_counter = reinterpret_cast<int *>(ws + pl.off_counter);
-        e = epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, p->N, p->C, p->H, p->W, a.tile_counter, dt, st);
+        e = epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, NP, p->C, p->H, p->W, a.tile_counter, dt, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
         launches++;
         a.src_hi = hi; a.src_lo = lo;
@@ -257,14 +278,14 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
             e = epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st);
             if (e != cudaSuccess) return fail(EPI_ECUDA, "reference staging launch failed: %s", cudaGetErrorString(e));
             uint16_t *order = reinterpret_cast<uint16_t *>(ws + pl.off_order);
-            e = epi::launch_sector_order(p->P_ref, p->P_src, order, p->N, a.geom, st);
+            e = epi::launch_sector_order(p->P_ref, p->P_src, order, NP, p->N, a.geom, st);
             if (e != cudaSuccess) return fail(EPI_ECUDA, "sector ordering launch failed: %s", cudaGetErrorString(e));
             launches += 2;
             a.ref_hi = rhi; a.ref_lo = rlo; a.order = order;
         }
     } else if (pl.stage_src) {
         float *nhwc = reinterpret_cast<float *>(ws + pl.off_src);
-        e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st);
+        e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, NP, p->C, p->H, p->W, dt, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "layout staging launch failed: %s", cudaGetErrorString(e));
         launches++;
         a.src_nhwc = nhwc;
@@ -276,7 +297,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     if (z_tc) {         // fused feature leaves the tile kernel as bf16 (hi, lo) planes: the A operand of the z GEMM
         a.out = nullptr;
         a.out_hi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_prez);
-        a.out_lo = a.out_hi + (size_t)p->N * p->C * p->H * p->W;
+        a.out_lo = a.out_hi + (size_t)NP * p->C * p->H * p->W;
         a.add_ref = 0;
     } else if (pl.pipe && pl.unstage) {   // fused feature leaves the kernel pixel-major (full 128-byte lines); a transposition pass writes `out`
         a.out = reinterpret_cast<float *>(ws + pl.off_prez);
@@ -304,7 +325,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
 
     if (pl.pipe && pl.unstage) {
         e = epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out, EPI_DTYPE_F32, p->out_stride,
-                                p->N, p->C, p->H, p->W, st);
+                                NP, p->N, p->C, p->H, p->W, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "output transposition launch failed: %s", cudaGetErrorString(e));
         launches++;
     }
@@ -314,7 +335,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         z.x_hi = a.out_hi; z.x_lo = a.out_lo; z.w_hi = w_hi; z.w_lo = w_lo; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.ref = p->feat_ref; z.ref_dtype = dt; z.y = p->out;
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
-        z.N = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
+        z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         e = epi::launch_zgemm(z, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "z GEMM launch failed: %s", cudaGetErrorString(e));
@@ -330,7 +351,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         z.x = a.out;
         for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? ref32_stride[i] : p->ref_stride[i]; }
         z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
-        z.N = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
+        z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         e = epi::launch_z_epilogue(z, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "z epilogue launch failed: %s", cudaGetErrorString(e));
@@ -397,12 +418,12 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     if (e != cudaSuccess) return fail(EPI_ECUDA, "backward kernel launch failed: %s", cudaGetErrorString(e));
     launches++;
     if (p->grad_src) {
-        e = epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride, p->N, p->C, p->H, p->W, st);
+        e = epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride, p->N, p->N, p->C, p->H, p->W, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
         launches++;
     }
     if (p->grad_ref && lowp) {         // fp32 gradient of a low-precision reference map, rounded once to its type
-        e = epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride, p->N, p->C, p->H, p->W, st);
+        e = epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride, p->N, p->N, p->C, p->H, p->W, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
         launches++;
     }
@@ -428,6 +449,18 @@ int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_
     if ((int)(radius + 0.5f) < 1) return fail(EPI_EINVAL, "radius must round to at least 1");
     cudaError_t e = epi::launch_peaks(heatmaps, locs, scores, B, J, H, W, radius, downsample, threshold, int_div,
                                       reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(EPI_ECUDA, "peak kernel launch failed: %s", cudaGetErrorString(e));
+    return EPI_OK;
+}
+
+int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32_t *src_index, int32_t S, int32_t B, int32_t J,
+                            int32_t H, int32_t W, float radius, float downsample, float threshold, int32_t int_div, void *stream) {
+    if (!heat || !locs || !scores) return fail(EPI_EINVAL, "null pointer");
+    if (S <= 0 || B <= 0 || J <= 0 || H < 2 || W < 2 || !(radius > 0.f)) return fail(EPI_EINVAL, "bad shape or radius");
+    if ((int)(radius + 0.5f) < 1) return fail(EPI_EINVAL, "radius must round to at least 1");
+    if ((int64_t)B * J > INT32_MAX / 32) return fail(EPI_EINVAL, "B * J too large (one warp per joint, counted in int32)");
+    cudaError_t e = epi::launch_peaks_best(heat, locs, scores, src_index, S, B, J, H, W, radius, downsample, threshold, int_div,
+                                           reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(EPI_ECUDA, "peak kernel launch failed: %s", cudaGetErrorString(e));
     return EPI_OK;
 }

@@ -155,9 +155,13 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
     const int C = a.C, K = a.geom.K, H = a.geom.H, W = a.geom.W, HW = H * W;
     const int tiles_per_item = (HW + P - 1) / P;
     const int total_tiles = a.N * tiles_per_item;
-    // tail balancing: the tiles of the last, partial round over the grid are handed out as half items (16 pixels)
-    const int tail_tiles = a.tile_counter ? total_tiles % (int)gridDim.x : 0;
-    const int r_half = min(tiles_per_item, (tail_tiles + a.N - 1) / a.N);          // per pair
+    // tail balancing: the tiles of the last, partial round over the grid are handed out as half items (16 pixels).  How a tile
+    // is split changes the union rows its pixels share, hence the order of the GEMM sums, so with several sources per reference
+    // item (n_ref < N) the split is the one a call with the n_ref pairs of a single source makes on its own grid: every source
+    // gets, bit for bit, what a separate call gives it.
+    const int grid1 = min(a.n_ref * tiles_per_item, (int)gridDim.x);
+    const int tail_tiles = a.tile_counter ? (a.n_ref * tiles_per_item) % grid1 : 0;
+    const int r_half = min(tiles_per_item, (tail_tiles + a.n_ref - 1) / a.n_ref);  // per pair
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nwords = (HW + 31) >> 5;
     const bool big = nwords > MAXWORDS;             // row-windowed union bitmap (see WinView)
@@ -168,7 +172,6 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
     const bool wide = C > 256;
     const int NQH = wide ? 2 : 1;
     const GeomCfg gc = a.geom;
-    const int NHW = a.N * HW;                       // plane stride (rows) of the operand buffer [ref_hi|ref_lo|src_hi|src_lo]
     constexpr int KW = 2 * KPL;                     // samples per worker warp (k = warp + 16 jj)
 
     // ---------------- one-time setup (overlaps the staging launch's tail: programmatic dependent launch) ----------------
@@ -285,7 +288,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                         } else {
                             const float ov[4] = {o.x, o.y, o.z, o.w};
                             float *ob = a.out + (int64_t)d.n * a.out_stride[0] + (int64_t)y * a.out_stride[2] + (int64_t)x * a.out_stride[3];
-                            const int64_t rb = (int64_t)d.n * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
+                            const int64_t rb = (int64_t)(d.n % a.n_ref) * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
 #pragma unroll
                             for (int e = 0; e < 4; e++) {
                                 float val = ov[e];
@@ -788,8 +791,9 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         // consecutive lanes.  Completion: cp.async.mbarrier.arrive.noinc on the stage's mbarrier (count = 128 threads).
         // =====================================================================================================
         const int gt = tid - W_GATHER * 32, gj = gt & 7, gr = gt >> 3;
-        // [ref_hi | ref_lo | src_hi | src_lo] (LO) or [ref_hi | src_hi], each [N*HW][C]; a lo plane follows its hi plane
-        const size_t plane_elems = (size_t)NHW * C;
+        // [ref_hi | ref_lo | src_hi | src_lo] (LO) or [ref_hi | src_hi]; a lo plane follows its hi plane.  Reference planes are
+        // [n_ref*HW][C], source planes [N*HW][C] (pair n queries reference item n % n_ref)
+        const size_t plane_elems = (size_t)a.N * HW * C, ref_plane_elems = (size_t)a.n_ref * HW * C;
         uint32_t qcount = 0, fcount = 0;
         const bool pt_on = gt == 0; (void)pt_on;
         PT_DECL;
@@ -863,7 +867,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                     }
                     PT(16);
                     {
-                        const __nv_bfloat16 *ref = a.ref_hi + (size_t)d.n * HW * C;
+                        const __nv_bfloat16 *ref = a.ref_hi + (size_t)(d.n % a.n_ref) * HW * C;
 #pragma unroll
                         for (int it = 0; it < 2; it++) {
                             const int r = gr + 16 * it;
@@ -876,7 +880,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                                 if (kp < npq) {                 // channels beyond C are zero-filled: they are part of the MMA K range
                                     const bool ok = ch < C;
                                     cp16(so + kp * PANEL_B2, ok ? row + ch : row, ok);
-                                    if (LO) cp16(so + kp * PANEL_B2 + 4096, ok ? row + plane_elems + ch : row, ok);
+                                    if (LO) cp16(so + kp * PANEL_B2 + 4096, ok ? row + ref_plane_elems + ch : row, ok);
                                 }
                             }
                         }
@@ -935,8 +939,9 @@ extern "C" void epi_pipe_timers_read(unsigned long long *out32, int reset) {
 #endif
 
 size_t fusion_pipe_plan_record_bytes() { return DESC_BYTES; }
-// claims = whole tiles + the half items of the last partial round over the grid (< number of SMs, rounded up per pair)
-int fusion_pipe_plan_records(int N, int H, int W) { return N * ((H * W + P - 1) / P) + 256 + N; }
+// claims = whole tiles + the half items of the last partial round over the grid of n_ref pairs (< number of SMs, rounded up per
+// pair), for each of the N / n_ref sources
+int fusion_pipe_plan_records(int N, int n_ref, int H, int W) { return N * ((H * W + P - 1) / P) + (N / n_ref) * (256 + n_ref); }
 
 bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in) {
     if (C % 8 != 0 || C > 512 || C < 8) return false;

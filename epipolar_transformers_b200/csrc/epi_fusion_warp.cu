@@ -47,11 +47,12 @@ epi_fusion_warp_kernel(const FusionArgs a) {
     float *a_tile = smem + (size_t)C * 33;                   // [K][33]  attention weights
     __shared__ PairGeom s_geom;
 
-    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * n, a.P_src + 12 * n, s_geom);
+    const int nr = n % a.n_ref;                              // the pair's reference item
+    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * nr, a.P_src + 12 * n, s_geom);
 
     // ---- stage the query tile: coalesced along whichever of (pixel, channel) is contiguous ----
     {
-        const float *base = a.feat_ref + (int64_t)n * a.ref_stride[0];
+        const float *base = a.feat_ref + (int64_t)nr * a.ref_stride[0];
         const int64_t sc = a.ref_stride[1], sh = a.ref_stride[2], sw = a.ref_stride[3];
         if (sc != 1) {
             for (int idx = tid; idx < C * kWarpTilePix; idx += blockDim.x) {
@@ -209,7 +210,7 @@ epi_fusion_warp_kernel(const FusionArgs a) {
     {
         float *obase = a.out + (int64_t)n * a.out_stride[0];
         const int64_t sc = a.out_stride[1], sh = a.out_stride[2], sw = a.out_stride[3];
-        const float *rbase = a.feat_ref + (int64_t)n * a.ref_stride[0];
+        const float *rbase = a.feat_ref + (int64_t)nr * a.ref_stride[0];
         if (sc != 1) {
             for (int idx = tid; idx < C * kWarpTilePix; idx += blockDim.x) {
                 int pp = idx & 31, c = idx >> 5, p = p0 + pp;

@@ -20,7 +20,8 @@ struct FusionArgs {
     float *out;             int64_t out_stride[4];
     __nv_bfloat16 *out_hi, *out_lo;           // optional: fused feature as bf16 (hi, lo) planes [N,H,W,C] (feeds the z GEMM)
     float *attn, *corr_pos, *locs_out;
-    int N, C;
+    int N, C;                                 // N: pairs (S·N of the ABI)
+    int n_ref;                                // reference items: pair n reads reference item n % n_ref (feat_ref, ref_hi/lo, P_ref)
     float softmax_scale;
     int add_ref;
     int *tile_counter;                        // zeroed by the staging kernel; dynamic tile scheduler of the tile kernel
@@ -52,10 +53,10 @@ cudaError_t launch_fusion_bwd(const BwdArgs &a, cudaStream_t st);
 // z-projection epilogue:  y[n,o,p] = sum_c Wf[o,c]·x[n,c,p] + bf[o] (+x[n,o,p]) (+ref[n,o,p])
 struct ZArgs {
     const float *x;         int64_t x_stride[4];     // pre-z fused feature
-    const float *ref;       int64_t ref_stride[4];   // may be null
+    const float *ref;       int64_t ref_stride[4];   // may be null; item n reads ref item n % n_ref
     float *y;               int64_t y_stride[4];
     const float *Wf, *bf;
-    int N, C, HW, W;
+    int N, C, HW, W, n_ref;
     int z_residual, add_ref;
 };
 
@@ -67,7 +68,7 @@ struct ZGemmArgs {
     const void *ref;        int64_t ref_stride[4];   // element type ref_dtype
     int ref_dtype;
     float *y;               int64_t y_stride[4];
-    int N, C, HW, W, Npad;
+    int N, C, HW, W, Npad, n_ref;             // item n reads ref item n % n_ref
     int z_residual, add_ref;
 };
 bool zgemm_supported(int C);
@@ -78,30 +79,35 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st);
 cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st);
 bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 size_t fusion_pipe_plan_record_bytes();
-int fusion_pipe_plan_records(int N, int H, int W);
+int fusion_pipe_plan_records(int N, int n_ref, int H, int W);   // N pairs on n_ref reference items
 bool fusion_tile_supported(const FusionArgs &a);
 bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in);
-cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, const GeomCfg &gc, cudaStream_t st);
+// pair n: P_ref item n % n_ref, P_src item n
+cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, const GeomCfg &gc, cudaStream_t st);
 // `dtype` (kF32 / kBF16 / kF16): element type of the source map(s)
 cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
                                 int H, int W, int *zero_me, int dtype, cudaStream_t st);
 
-// planes: [ref_hi | ref_lo | src_hi | src_lo] for fp32 / fp16 maps, [ref_hi | src_hi] for bf16 maps (their lo part is zero)
+// planes: [ref_hi | ref_lo | src_hi | src_lo] for fp32 / fp16 maps, [ref_hi | src_hi] for bf16 maps (their lo part is zero);
+// the reference planes hold n_ref items, the source planes (and the pair constants / orders) N pairs, pair n on reference n % n_ref
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
-                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int C,
-                         int H, int W, const GeomCfg &gc, cudaStream_t st);
+                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
+                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st);
 
 cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
                                 cudaStream_t st);
 cudaError_t launch_z_epilogue(const ZArgs &z, cudaStream_t st);
-// out_dtype != kF32 (a gradient rounded once) takes no residual
+// out_dtype != kF32 (a gradient rounded once) takes no residual; item n adds ref item n % n_ref
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
-                           const int64_t out_stride[4], int N, int C, int H, int W, cudaStream_t st);
+                           const int64_t out_stride[4], int N, int n_ref, int C, int H, int W, cudaStream_t st);
 cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, const float *b, const float *mean,
                              const float *var, float eps, int C, float *wf, float *bf, cudaStream_t st);
 cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, int J, int H, int W, float radius, float downsample,
                          float threshold, int int_div, cudaStream_t st);
+// heat [S,B,J,H,W]: per (b, j) the peak of the source with the highest score (first source on a tie); src_index may be null
+cudaError_t launch_peaks_best(const float *heat, float *locs, float *scores, int *src_index, int S, int B, int J, int H, int W,
+                              float radius, float downsample, float threshold, int int_div, cudaStream_t st);
 cudaError_t launch_sample_locs(const float *P_ref, const float *P_src, float *locs, int N, const GeomCfg &gc, cudaStream_t st);
 
 }  // namespace epi

@@ -15,12 +15,11 @@
 
 namespace epi {
 
-__global__ void __launch_bounds__(128) epi_peaks_kernel(const float *__restrict__ heat, float *__restrict__ locs,
-                                                        float *__restrict__ scores, int BJ, int H, int W, float radius,
-                                                        float downsample, float threshold, int int_div) {
-    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= BJ) return;
-    const float *m = heat + (size_t)warp * H * W;
+// One warp: the peak of heat-map m [H,W] -> image coordinates (x, y) and score, identical on every lane.  Both kernels below
+// call this one function, so a best-source result is bit for bit the single-source result of the winning source.
+__device__ __forceinline__ void peak_of(const float *__restrict__ m, int H, int W, float radius, float downsample, float threshold,
+                                        int int_div, float &out_x, float &out_y, float &out_score) {
+    const int lane = threadIdx.x & 31;
     const int HW = H * W;
     // ---- arg-max, first maximum (NaN never wins, like a plain comparison scan) ----
     float best = -INFINITY;
@@ -73,13 +72,55 @@ __global__ void __launch_bounds__(128) epi_peaks_kernel(const float *__restrict_
         sx += __shfl_xor_sync(0xffffffffu, sx, o);
         sy += __shfl_xor_sync(0xffffffffu, sy, o);
     }
+    const float den = sum + 2.220446049250313e-16f;                      // np.finfo(float).eps
+    const float x = sx / den + index_w, y = sy / den + index_h;
+    out_x = x * downsample + downsample * 0.5f - 0.5f;
+    out_y = y * downsample + downsample * 0.5f - 0.5f;
+    out_score = best;
+}
+
+__global__ void __launch_bounds__(128) epi_peaks_kernel(const float *__restrict__ heat, float *__restrict__ locs,
+                                                        float *__restrict__ scores, int BJ, int H, int W, float radius,
+                                                        float downsample, float threshold, int int_div) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= BJ) return;
+    float x, y, score;
+    peak_of(heat + (size_t)warp * H * W, H, W, radius, downsample, threshold, int_div, x, y, score);
     if (lane == 0) {
-        const float den = sum + 2.220446049250313e-16f;                  // np.finfo(float).eps
-        const float x = sx / den + index_w, y = sy / den + index_h;
-        locs[2 * warp] = x * downsample + downsample * 0.5f - 0.5f;
-        locs[2 * warp + 1] = y * downsample + downsample * 0.5f - 0.5f;
-        scores[warp] = best;
+        locs[2 * warp] = x;
+        locs[2 * warp + 1] = y;
+        scores[warp] = score;
     }
+}
+
+// Multi-view test (modeling/model.py:229-234): heat [S,B,J,H,W]; warp (b, j) runs the single-source peak of every source and
+// keeps the first one with the highest score — strict `>`, so a tie keeps the earlier source like torch.max.
+__global__ void __launch_bounds__(128) epi_peaks_best_kernel(const float *__restrict__ heat, float *__restrict__ locs,
+                                                             float *__restrict__ scores, int *__restrict__ src_index, int S, int BJ,
+                                                             int H, int W, float radius, float downsample, float threshold,
+                                                             int int_div) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= BJ) return;
+    float bx = 0.f, by = 0.f, bs = 0.f;
+    int bsrc = 0;
+    for (int s = 0; s < S; s++) {
+        float x, y, score;
+        peak_of(heat + ((size_t)s * BJ + warp) * H * W, H, W, radius, downsample, threshold, int_div, x, y, score);
+        if (s == 0 || score > bs) { bx = x; by = y; bs = score; bsrc = s; }
+    }
+    if (lane == 0) {
+        locs[2 * warp] = bx;
+        locs[2 * warp + 1] = by;
+        scores[warp] = bs;
+        if (src_index) src_index[warp] = bsrc;
+    }
+}
+
+cudaError_t launch_peaks_best(const float *heat, float *locs, float *scores, int *src_index, int S, int B, int J, int H, int W,
+                              float radius, float downsample, float threshold, int int_div, cudaStream_t st) {
+    const int BJ = B * J;
+    epi_peaks_best_kernel<<<(BJ + 3) / 4, 128, 0, st>>>(heat, locs, scores, src_index, S, BJ, H, W, radius, downsample, threshold, int_div);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, int J, int H, int W, float radius, float downsample,

@@ -1,6 +1,6 @@
 // epi_stage.cu — the ONE operand-staging launch in front of the fused attention kernel (epi_fusion_pipe.cu):
 //
-//   blocks [0, N)      per (ref, src) pair: fp64 pair constants (camera centre, epipole, infinite homography;
+//   blocks [0, N)      per (ref, src) pair (pair n: reference item n % n_ref, source item n): fp64 pair constants (camera centre, epipole, infinite homography;
 //                      /root/reference/vision/multiview.py:16-21, modeling/layers/epipolar.py:336-348) and the list of
 //                      reference pixels sorted by epipolar angle (counting sort on a 12-bit angle key, ties by pixel index
 //                      => deterministic).  Pixels on one epipolar line of the reference view share one epipolar line in
@@ -8,6 +8,8 @@
 //   remaining blocks   [N,C,H,W] (any strides; fp32, bf16 or fp16 elements) -> pixel-major bf16 (hi, lo) planes [N,H*W,C] with
 //                      x ≈ hi + lo, for BOTH feature maps (reference -> planes 0,1; source -> planes 2,3 of one buffer), 64 x 64
 //                      tiles through shared memory: coalesced 4-pixel vector reads along pixels, 16-byte writes along channels.
+//                      The reference map has n_ref items and the source map N (several source views per reference item:
+//                      N = S·n_ref), so a reference tile is staged once however many sources it is fused with.
 //                      fp16 values are split exactly like fp32 ones (hi + lo holds them exactly); a bf16 value is its own hi
 //                      part, so bf16 maps write hi planes only (reference -> plane 0, source -> plane 1).
 // Also zeroes the fused kernel's tile counter and error word.
@@ -58,7 +60,7 @@ template <typename T>
 struct StageArgs {
     const T *ref, *src;
     int64_t ref_stride[4], src_stride[4];
-    __nv_bfloat16 *planes;            // [4][N*HW][C]: ref_hi, ref_lo, src_hi, src_lo  (bf16 maps: [2][N*HW][C]: ref_hi, src_hi)
+    __nv_bfloat16 *planes;            // ref_hi, ref_lo [n_ref*HW][C], src_hi, src_lo [N*HW][C]  (bf16 maps: ref_hi, src_hi)
     const float *P_ref, *P_src;       // may be null (injected locations): no order, no pair constants
     PairGeom *pair_geom;              // [N]
     uint16_t *order;                  // [N][HW]
@@ -68,13 +70,19 @@ struct StageArgs {
     int w_add_identity;               // ZRESIDUAL folded into the weight: planes hold Wf + I
     __nv_bfloat16 *w_planes;
     int N, C, H, W;
+    int n_ref;                        // reference items; pair n reads reference item n % n_ref
+    int ref_tiles;                    // layout tiles of the reference map (n_ref items); the source map has N items
+    size_t ref_elems;                 // elements of one reference plane
+    size_t src_plane0;                // offset of the source hi plane in `planes`
     int do_ref, do_src, do_order;
     int persist;                      // > 0: whole vectorisable tiles only -> `persist` streaming blocks loop over the tiles
     GeomCfg gc;
 };
 
 // (min 5 blocks per SM: the layout-staging blocks need few registers; the rare order blocks may spill a little)
-template <typename T>
+// MULTI: several source views per reference item (n_ref < N).  The one-source instantiation keeps the single-map-size indexing,
+// so its code (and its register allocation, tight at 48 registers) does not pay for the general mapping.
+template <typename T, bool MULTI>
 __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T> s) {
     using namespace stg;
     constexpr bool LO = !std::is_same<T, __nv_bfloat16>::value;   // a bf16 value's lo part is zero: no lo planes
@@ -100,11 +108,11 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
 #ifdef EPI_PIPE_TIMERS
         long long st_prev = clock64();
 #endif
-        const int n = blockIdx.x;
+        const int n = blockIdx.x, nr = MULTI ? n % s.n_ref : n;         // pair, its reference item
         // cached order: the key is (P_ref, P_src, geometry configuration); an unchanged camera pair costs 32 compares
         float my_key = 0.f;
         if (t < 32) {
-            if (t < 12) my_key = s.P_ref[12 * n + t];
+            if (t < 12) my_key = s.P_ref[12 * nr + t];
             else if (t < 24) my_key = s.P_src[12 * n + t - 12];
             else if (t == 24) my_key = (float)H;
             else if (t == 25) my_key = (float)W;
@@ -122,7 +130,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
         __syncthreads();
         if (s_e[7] != 0.f) return;                               // hit: order and pair constants are already in place
         if (t == 0) {
-            const float *P1 = s.P_ref + 12 * n, *P2 = s.P_src + 12 * n;
+            const float *P1 = s.P_ref + 12 * nr, *P2 = s.P_src + 12 * n;
             PairGeom g;
             pair_geom_from_krt(P1, P2, g);
             s.pair_geom[n] = g;
@@ -284,11 +292,11 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     // layout staging: 64 channels x 64 pixels per block
     // ----------------------------------------------------------------------------------------------------
     const int tiles_p = (HW + TPX - 1) / TPX, tiles_c = (C + TC - 1) / TC;
-    const int per_map = tiles_p * tiles_c * s.N;
+    const int src_tiles = tiles_p * tiles_c * s.N, ref_tiles = MULTI ? s.ref_tiles : src_tiles;
     int lin = (int)blockIdx.x - nord;
     const int wblocks = (s.Wf && s.w_planes) ? (C * C / 8 + NT - 1) / NT : 0;
     // block roles after the order blocks: [tiles | weight blocks], or with streaming blocks [weight blocks | streaming blocks]
-    const int wlin = s.persist ? lin : lin - 2 * per_map;
+    const int wlin = s.persist ? lin : lin - (ref_tiles + src_tiles);
     if (wlin >= 0 && wlin < wblocks) {
         // folded z weight [C out][C in] fp32 -> bf16 (hi, lo) planes (B operand of the z GEMM), 8 elements per thread
         const size_t e0 = ((size_t)wlin * NT + t) * 8, tot = (size_t)C * C;
@@ -363,16 +371,25 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
             if (LO) *reinterpret_cast<uint4 *>(lon + o) = l4;
         }
     };
-    const size_t plane_elems_all = (size_t)s.N * HW * C;
+    // reference and source tiles alternate while both remain (see below); the source tiles of the further sources follow
+    // (tile index l -> map, tile of that map)
+    auto split_tile = [&](int &l) -> int {
+        if (!MULTI || l < 2 * ref_tiles) { const int mp = l & 1; l >>= 1; return mp; }
+        l -= ref_tiles;
+        return 1;
+    };
+    const size_t plane_elems_all = (size_t)s.N * HW * C;                 // one source plane (= one reference plane unless MULTI)
+    auto plane_hi = [&](int mp) { return MULTI ? s.planes + (mp ? s.src_plane0 : (size_t)0) : s.planes + (size_t)(NPL * mp) * plane_elems_all; };
+    auto plane_elems = [&](int mp) { return MULTI && !mp ? s.ref_elems : plane_elems_all; };
     if (s.persist) {
         // Streaming blocks: every tile is a whole, vectorisable NCHW tile (host check).  A block walks tiles lin, lin + stride, ...
         // and issues the loads of its NEXT tile before it stores the current one, so HBM reads stay in flight for the whole launch
         // (one tile per block left the memory system idle while each block converted and stored).
-        const int nt = 2 * per_map, stride = s.persist;
+        const int nt = ref_tiles + src_tiles, stride = s.persist;
         int cur = lin - wblocks;
         if (cur >= nt) return;
         auto decode = [&](int l, int &mp, int &nn, int &c0n, int &p0n) {
-            mp = l & 1; l >>= 1;                         // reference and source tiles alternate (see below)
+            mp = split_tile(l);
             nn = l / (tiles_p * tiles_c);
             const int rem = l - nn * (tiles_p * tiles_c);
             const int ct = rem / tiles_p;
@@ -391,8 +408,8 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
                 decode(nxt, mp2, nn2, c02, p02);
                 fast_load((mp2 ? s.src : s.ref) + (int64_t)nn2 * (mp2 ? s.src_stride[0] : s.ref_stride[0]), mp2 ? s.src_stride[1] : s.ref_stride[1], c02, p02, v);
             }
-            __nv_bfloat16 *hin = s.planes + (size_t)(NPL * mp) * plane_elems_all;
-            fast_store(hin, hin + plane_elems_all, nn, c0n, p0n);
+            __nv_bfloat16 *hin = plane_hi(mp);
+            fast_store(hin, hin + plane_elems(mp), nn, c0n, p0n);
             if (nxt >= nt) return;
             __syncthreads();
             cur = nxt; mp = mp2; nn = nn2; c0n = c02; p0n = p02;
@@ -401,7 +418,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     // reference and source tiles alternate in block order: when the source map is a peer-mapped tensor of another GPU its
     // NVLink reads (~0.77 TB/s, microsecond latency) overlap the local reference tiles instead of queueing behind them
     int map = 0;
-    if (s.do_ref && s.do_src) { map = lin & 1; lin >>= 1; }
+    if (s.do_ref && s.do_src) map = split_tile(lin);
     else map = s.do_src ? 1 : 0;
     const int n = lin / (tiles_p * tiles_c), rem = lin % (tiles_p * tiles_c);
     const int c0 = (rem / tiles_p) * TC, p0 = (rem % tiles_p) * TPX;
@@ -409,8 +426,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     const int64_t *strd = map ? s.src_stride : s.ref_stride;
     const int64_t sn = strd[0], sc = strd[1], sh = strd[2], sw = strd[3];
     const T *sp = base + (int64_t)n * sn;
-    const size_t plane_elems = (size_t)s.N * HW * C;
-    __nv_bfloat16 *hi = s.planes + (size_t)(NPL * map) * plane_elems, *lo = hi + plane_elems;
+    __nv_bfloat16 *hi = plane_hi(map), *lo = hi + plane_elems(map);
     const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(sp) & (4 * sizeof(T) - 1)) == 0);
     if (vec && sc != 1 && p0 + TPX <= HW && c0 + TC <= C) {
         float4 v[RPASS];
@@ -478,24 +494,30 @@ template <typename T>
 static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], const T *src, const int64_t src_stride[4],
                                   __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                                   float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
-                                  int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
+                                  int n_ref, int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
     StageArgs<T> s;
     s.ref = ref; s.src = src;
     for (int i = 0; i < 4; i++) { s.ref_stride[i] = ref_stride[i]; s.src_stride[i] = src_stride[i]; }
     s.planes = planes; s.P_ref = P_ref; s.P_src = P_src; s.pair_geom = pair_geom; s.order = order; s.order_key = order_key; s.Wf = Wf; s.w_planes = w_planes; s.w_add_identity = w_add_identity;
-    s.zero_words = zero_words; s.N = N; s.C = C; s.H = H; s.W = W; s.gc = gc;
+    s.zero_words = zero_words; s.N = N; s.n_ref = n_ref; s.C = C; s.H = H; s.W = W; s.gc = gc;
     s.do_ref = 1; s.do_src = 1; s.do_order = (P_ref && P_src && order) ? 1 : 0; s.persist = 0;
-    const int tiles = ((H * W + stg::TPX - 1) / stg::TPX) * ((C + stg::TC - 1) / stg::TC) * N;
+    const int tiles_pc = ((H * W + stg::TPX - 1) / stg::TPX) * ((C + stg::TC - 1) / stg::TC);
+    const int tiles = tiles_pc * n_ref + tiles_pc * N;                       // reference tiles + source tiles
+    s.ref_tiles = tiles_pc * n_ref;
+    s.ref_elems = (size_t)n_ref * H * W * C;
+    s.src_plane0 = (std::is_same<T, __nv_bfloat16>::value ? 1 : 2) * s.ref_elems;
     const int wblocks = (Wf && w_planes) ? (C * C / 8 + stg::NT - 1) / stg::NT : 0;        // C % 8 == 0
     // dynamic shared memory: the transposition tile, or (order blocks) 16 KB histogram + 2 B per pixel
     const size_t smem_tile = (size_t)stg::TC * stg::TPITCH * sizeof(float);
     const size_t smem_order = (size_t)stg::NBIN * 4 + (size_t)H * W * 2;
-    static thread_local size_t smem_set = 0;
+    const bool multi = n_ref != N;
+    void (*kern)(const StageArgs<T>) = multi ? epi_stage_kernel<T, true> : epi_stage_kernel<T, false>;
+    static thread_local size_t smem_set[2] = {0, 0};
     auto ensure = [&](size_t smem) -> cudaError_t {
-        if (smem + 1024 > 48 * 1024 && smem > smem_set) {        // (+ the kernel's small static arrays)
-            cudaError_t e = cudaFuncSetAttribute(epi_stage_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (smem + 1024 > 48 * 1024 && smem > smem_set[multi]) {        // (+ the kernel's small static arrays)
+            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
-            smem_set = smem;
+            smem_set[multi] = smem;
         }
         return cudaSuccess;
     };
@@ -506,7 +528,7 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
         o.do_ref = 0; o.do_src = 0; o.Wf = nullptr; o.w_planes = nullptr; o.persist = 0;
         cudaError_t e = ensure(smem_order);
         if (e != cudaSuccess) return e;
-        e = launch_pdl(epi_stage_kernel<T>, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o);
+        e = launch_pdl(kern, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o);
         if (e != cudaSuccess) return e;
         s.do_order = 0; s.zero_words = nullptr;                  // the order launch has zeroed the counters
     }
@@ -523,27 +545,27 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     s.persist = 0;
     if ((H * W) % stg::TPX == 0 && C % stg::TC == 0 && whole(ref, ref_stride) && whole(src, src_stride)) {
         const int slots = 5 * sms_cached;                      // 5 resident blocks per SM (__launch_bounds__)
-        s.persist = 2 * tiles < slots ? 2 * tiles : slots;
+        s.persist = tiles < slots ? tiles : slots;
     }
-    const int grid = (s.do_order ? N : 0) + wblocks + (s.persist ? s.persist : 2 * tiles);
+    const int grid = (s.do_order ? N : 0) + wblocks + (s.persist ? s.persist : tiles);
     const size_t smem = (s.do_order && smem_order > smem_tile) ? smem_order : smem_tile;
     cudaError_t e = ensure(smem);
     if (e != cudaSuccess) return e;
-    return launch_pdl(epi_stage_kernel<T>, dim3((unsigned)grid), dim3(stg::NT), smem, st, s);
+    return launch_pdl(kern, dim3((unsigned)grid), dim3(stg::NT), smem, st, s);
 }
 
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
-                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int C,
-                         int H, int W, const GeomCfg &gc, cudaStream_t st) {
+                         float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
+                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
     if (dtype == kBF16)
         return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
     if (dtype == kF16)
         return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
     return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
-                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, C, H, W, gc, st);
+                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
 }
 
 }  // namespace epi

@@ -18,6 +18,7 @@ from torch import nn
 
 from . import _lib
 from .config import get_global_cfg
+from .peaks import find_tensor_peak_best
 
 _EPSILON = 0.001          # epipolar.py:20
 
@@ -92,27 +93,99 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
     dcode = _check_feat_pair(feat_ref, feat_src, out)
     if feat_ref.shape != feat_src.shape or feat_ref.device != feat_src.device:
         raise ValueError("feat_ref and feat_src must have the same shape and device")
+    return _fusion(lib, dcode, 1, feat_ref, feat_src, P_ref, P_src, K=K, downsample=downsample, img_scale=img_scale,
+                   softmax_scale=softmax_scale, correct_normalize=correct_normalize, align_corners=align_corners,
+                   z_folded=z_folded, z_residual=z_residual, add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in,
+                   want_attn=want_attn, want_corr=want_corr, want_locs=want_locs, variant=variant, out=out, state=state)
+
+
+def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4.0, img_scale=1.0,
+                          softmax_scale=0.125, correct_normalize=False, align_corners=False,
+                          z_folded=None, z_residual=False, add_ref_residual=False,
+                          sample_locs_in=None, want_attn=True, want_corr=True, want_locs=False,
+                          variant="auto", out=None, state: Optional[FusionState] = None):
+    """Fuses every reference item with S source views in one call: the multi-view test path of the reference
+    (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239), where each reference batch is fused against every other view.
+    Source s of item n gives exactly what `epipolar_fusion(feat_ref, feat_srcs[s], P_ref, P_srcs[s])` gives, but the
+    reference map is staged once and the S pairs share one launch chain.
+
+    feat_ref: [N,C,H,W] as in `epipolar_fusion`; feat_srcs: [S,N,C,H,W], or a sequence of S [N,C,H,W] maps (stacked);
+    P_ref: [N,3,4]; P_srcs: [S,N,3,4]; sample_locs_in: optional [K,S,N,H,W,2]; out: optional float32 [S,N,C,H,W].
+    Every residual (add_ref_residual, also under z) adds feat_ref[n].  Returns
+    (out [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attn [S,N,K,H,W] | None, sample_locs [K,S,N,H,W,2] | None).
+    Inference only (no backward for several sources): inputs that require grad under grad mode raise RuntimeError."""
+    lib = _lib.load()
+    if isinstance(feat_srcs, (list, tuple)):
+        if not feat_srcs or not all(isinstance(t, torch.Tensor) for t in feat_srcs):
+            raise ValueError("feat_srcs must be a [S,N,C,H,W] tensor or a non-empty sequence of [N,C,H,W] tensors")
+        if len({(tuple(t.shape), t.dtype, t.device) for t in feat_srcs}) != 1:
+            raise ValueError("the maps in feat_srcs must share shape, dtype and device")
+        feat_srcs = torch.stack(list(feat_srcs))
+    if not isinstance(feat_srcs, torch.Tensor) or feat_srcs.dim() != 5:
+        raise ValueError("feat_srcs must be a [S,N,C,H,W] tensor or a sequence of [N,C,H,W] tensors")
+    S = feat_srcs.shape[0]
+    if S < 1:
+        raise ValueError("feat_srcs has no source view")
+    feat_src = feat_srcs.flatten(0, 1)                          # [S·N,C,H,W]: pair p = s·N + n
+    if out is not None:
+        if not isinstance(out, torch.Tensor) or out.dim() != 5 or out.shape != feat_srcs.shape:
+            raise ValueError("out must be a [S,N,C,H,W] tensor")
+        if out.shape[0] > 1 and out.shape[1] > 1 and out.stride(0) != out.shape[1] * out.stride(1):
+            raise ValueError("out must be viewable as [S*N,C,H,W] (stride(0) == N * stride(1))")
+    out4 = out.flatten(0, 1) if out is not None else None
+    if isinstance(feat_ref, torch.Tensor) and (tuple(feat_srcs.shape[1:]) != tuple(feat_ref.shape) or feat_ref.device != feat_src.device):
+        raise ValueError("feat_srcs must be [S,N,C,H,W] with [N,C,H,W] == feat_ref's shape, on feat_ref's device")
+    if not isinstance(feat_ref, torch.Tensor) or feat_ref.dim() != 4:
+        raise ValueError("feat_ref must be a 4-D tensor [N,C,H,W]")
     N, C, H, W = feat_ref.shape
+    if sample_locs_in is None:
+        if not isinstance(P_srcs, torch.Tensor) or tuple(P_srcs.shape) != (S, N, 3, 4):
+            raise ValueError("P_srcs must be [S,N,3,4]")
+        P_srcs = P_srcs.reshape(S * N, 3, 4)
+    else:
+        if tuple(sample_locs_in.shape) != (K, S, N, H, W, 2):
+            raise ValueError("sample_locs_in must be [K,S,N,H,W,2]")
+        sample_locs_in = sample_locs_in.reshape(K, S * N, H, W, 2)
+    dcode = _check_feat_pair(feat_ref, feat_src, out4)
+    if torch.is_grad_enabled() and (feat_ref.requires_grad or feat_src.requires_grad):
+        raise RuntimeError("epipolar_fusion_multi is inference only (several sources have no backward); run it under "
+                           "torch.no_grad(), or use epipolar_fusion (one source per call) for gradients")
+    o, corr, attn, locs = _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_srcs, K=K, downsample=downsample,
+                                  img_scale=img_scale, softmax_scale=softmax_scale, correct_normalize=correct_normalize,
+                                  align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
+                                  add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
+                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state)
+    return (out if out is not None else o.unflatten(0, (S, N)), None if corr is None else corr.unflatten(0, (S, N)),
+            None if attn is None else attn.unflatten(0, (S, N)), None if locs is None else locs.unflatten(1, (S, N)))
+
+
+def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, img_scale, softmax_scale, correct_normalize,
+            align_corners, z_folded, z_residual, add_ref_residual, sample_locs_in, want_attn, want_corr, want_locs, variant, out,
+            state):
+    """The forward of `epipolar_fusion` (S = 1) and `epipolar_fusion_multi`: feat_ref [N,C,H,W], feat_src / out [S·N,C,H,W],
+    P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n)."""
+    N, C, H, W = feat_ref.shape
+    NP = S * N
     dev = feat_ref.device
     if sample_locs_in is None:
         if P_ref.device != dev or P_ref.dtype != torch.float32 or not P_ref.is_contiguous():
             P_ref = P_ref.to(device=dev, dtype=torch.float32).contiguous()
         if P_src.device != dev or P_src.dtype != torch.float32 or not P_src.is_contiguous():
             P_src = P_src.to(device=dev, dtype=torch.float32).contiguous()
-        if tuple(P_ref.shape) != (N, 3, 4) or tuple(P_src.shape) != (N, 3, 4):
-            raise ValueError("P_ref/P_src must be [N,3,4]")
+        if tuple(P_ref.shape) != (N, 3, 4) or tuple(P_src.shape) != (NP, 3, 4):
+            raise ValueError("P_ref/P_src must be [N,3,4]" if S == 1 else "P_ref must be [N,3,4] and P_srcs [S,N,3,4]")
     else:
         sample_locs_in = sample_locs_in.to(device=dev, dtype=torch.float32).contiguous()
-        if tuple(sample_locs_in.shape) != (K, N, H, W, 2):
+        if tuple(sample_locs_in.shape) != (K, NP, H, W, 2):
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
     if out is None:
-        out = torch.empty_like(feat_ref, dtype=torch.float32)           # preserves NCHW / channels_last
-    attn = torch.empty((N, K, H, W), device=dev, dtype=torch.float32) if want_attn else None
-    corr = torch.empty((N, H, W, 2), device=dev, dtype=torch.float32) if want_corr else None
-    locs = torch.empty((K, N, H, W, 2), device=dev, dtype=torch.float32) if want_locs else None
+        out = torch.empty_like(feat_src, dtype=torch.float32)           # preserves NCHW / channels_last
+    attn = torch.empty((NP, K, H, W), device=dev, dtype=torch.float32) if want_attn else None
+    corr = torch.empty((NP, H, W, 2), device=dev, dtype=torch.float32) if want_corr else None
+    locs = torch.empty((K, NP, H, W, 2), device=dev, dtype=torch.float32) if want_locs else None
 
     vcode = _lib.VARIANTS[variant] if isinstance(variant, str) else int(variant)
-    key = (dev, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), z_folded is not None, vcode,
+    key = (dev, S, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
     if state is not None and state.key == key:
@@ -127,6 +200,7 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
         p.z_residual = int(bool(z_residual)); p.add_ref_residual = int(bool(add_ref_residual))
         p.variant = vcode
         p.feat_dtype = dcode
+        p.n_src = S if S > 1 else 0
     p.feat_ref = feat_ref.data_ptr(); p.feat_src = feat_src.data_ptr()
     p.P_ref = P_ref.data_ptr() if sample_locs_in is None else None
     p.P_src = P_src.data_ptr() if sample_locs_in is None else None
@@ -346,10 +420,10 @@ class Epipolar(nn.Module):
             seen.add(cur.cuda_stream)
         return folded
 
-    def _state_for(self, t):
+    def _state_for(self, t, slot="single"):
         if not (isinstance(t, torch.Tensor) and t.is_cuda):
             return None                                  # epipolar_fusion raises the proper error for CPU tensors
-        return self._states.setdefault((t.device, torch.cuda.current_stream(t.device).cuda_stream), FusionState())
+        return self._states.setdefault((t.device, torch.cuda.current_stream(t.device).cuda_stream, slot), FusionState())
 
     def forward(self, feat1, feat2, P1, P2, depth=None, camera=None, other_camera=None, ref1=None, ref2=None):
         """feat1/feat2: N x C x H x W; P1/P2: N x 3 x 4 (epipolar.py:82-89).
@@ -396,6 +470,30 @@ class Epipolar(nn.Module):
             finalout = out
         return finalout, corr, attn, (locs.transpose(0, 1) if want_locs else None)
 
+    def forward_multi(self, feat1, feats2, P1, P2s):
+        """`forward` of one reference batch against S source views in one fused call (the MULTITEST path,
+        modeling/model.py:213-239).  feat1 [N,C,H,W], feats2 [S,N,C,H,W] or a sequence of S [N,C,H,W] maps, P1 [N,3,4],
+        P2s [S,N,3,4].  Returns what S calls of `forward` return, stacked over the sources:
+        (finalout [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attention [S,N,K,H,W] | None, sample_locs [S,N,K,H,W,2] | None).
+        Inference only.  With the z projection the module must be in eval mode: training-mode BatchNorm would take its
+        batch statistics over all S·N items, which S separate calls do not."""
+        cfg = self.cfg
+        ep = cfg.EPIPOLAR
+        has_z = "z" in ep.PARAMETERIZED
+        if has_z and self.training:
+            raise RuntimeError("Epipolar.forward_multi with the z projection needs eval mode: training-mode BatchNorm statistics "
+                               "over S*N items differ from S separate forward calls")
+        want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+        out, corr, attn, locs = epipolar_fusion_multi(
+            feat1, feats2, P1, P2s, K=self.sample_size, downsample=self.downsample,
+            img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE,
+            softmax_scale=ep.SOFTMAXSCALE, correct_normalize=ep.USE_CORRECT_NORMALIZE,
+            align_corners=self.align_corners, z_folded=self._folded() if has_z else None,
+            z_residual=bool(ep.ZRESIDUAL) if has_z else False, add_ref_residual=self.fuse_ref_residual,
+            want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
+            state=self._state_for(feat1, "multi"))
+        return out, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
+
 
 def fused_other_feat(feat, other_features, KRT, other_KRT, sampler: Epipolar, camera=None, other_camera=None):
     """Caller-side mirror of getOtherFeat (modeling/backbones/resnet.py:377-388):
@@ -407,3 +505,21 @@ def fused_other_feat(feat, other_features, KRT, other_KRT, sampler: Epipolar, ca
     if not sampler.fuse_ref_residual:
         ret = ret + feat
     return ret, corr_pos, depth, locs
+
+
+def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma, downsample):
+    """The multi-view test of the reference (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239) from the fusion layer on:
+    every reference item is fused with each of the S other views, each fusion goes through the rest of the network and the
+    peak finder, and every joint keeps the location of the source whose peak scores highest (torch.max over the sources, then
+    gather).  Here the S fusions are one `Epipolar.forward_multi` call and the selection is one launch.
+
+    feat [N,C,H,W] (the reference views' features at the merge point), other_feats [S,N,C,H,W] or S [N,C,H,W] maps, KRT
+    [N,3,4], other_KRTs [S,N,3,4]; tail: everything after the merge point ([B,C,H,W] -> heat-maps [B,J,h,w]; `final_layer`
+    for MERGE='late'); sigma = cfg.KEYPOINT.SIGMA, downsample as for find_tensor_peak_batch.
+    Returns (locs [N,J,2], scores [N,J], source index [N,J]); the reference's final `squeeze()` is left to the caller."""
+    with torch.no_grad():
+        ret, _, _, _ = sampler.forward_multi(feat, other_feats, KRT, other_KRTs)
+        x = ret if sampler.fuse_ref_residual else ret + feat          # getOtherFeat's `ret + feat` (resnet.py:388), per source
+        S, N = x.shape[0], x.shape[1]
+        heat = tail(x.flatten(0, 1))
+        return find_tensor_peak_best(heat.unflatten(0, (S, N)), sigma, downsample)

@@ -39,3 +39,33 @@ def find_tensor_peak_batch(heatmap: torch.Tensor, radius, downsample, threshold:
                                           float(downsample), float(threshold), int(bool(int_div)), ctypes.c_void_p(stream)),
                    "epi_find_peaks_f32")
     return (locs, score) if batched else (locs[0], score[0])
+
+
+def find_tensor_peak_best(heatmaps: torch.Tensor, radius, downsample, threshold: float = 0.000001, int_div: bool = False):
+    """heatmaps [S,B,J,H,W] (S source views) -> (locs [B,J,2], scores [B,J], src_index [B,J] int64).
+
+    The best-source selection of the reference's multi-view test (modeling/model.py:229-234): every source's peaks are
+    `find_tensor_peak_batch` of its [B,J,H,W] stack, and each (b, j) keeps the peak of the source with the highest score,
+    the first one on a tie (torch.max over sources, then gather).  One launch for all sources."""
+    lib = _lib.load()
+    if not isinstance(heatmaps, torch.Tensor) or heatmaps.dim() != 5:
+        raise ValueError("heatmaps must be [S,B,J,H,W] (got %s)" % (tuple(getattr(heatmaps, "shape", ())),))
+    S, B, J, H, W = heatmaps.shape
+    if min(S, B, J) < 1:
+        raise ValueError("heatmaps has an empty dimension: %s" % (tuple(heatmaps.shape),))
+    if H <= 1 or W <= 1:
+        raise ValueError("To avoid the normalization function divide zero")
+    if not (radius > 0):
+        raise ValueError("The radius is not ok : %r" % (radius,))
+    if not heatmaps.is_cuda:
+        raise RuntimeError("heatmaps is on %s: the CUDA peak finder has no CPU implementation" % heatmaps.device)
+    h = heatmaps.detach().to(torch.float32).contiguous()
+    locs = torch.empty((B, J, 2), device=h.device, dtype=torch.float32)
+    score = torch.empty((B, J), device=h.device, dtype=torch.float32)
+    src = torch.empty((B, J), device=h.device, dtype=torch.int32)
+    with torch.cuda.device(h.device):
+        stream = torch.cuda.current_stream(h.device).cuda_stream
+        _lib.check(lib.epi_find_peaks_best_f32(h.data_ptr(), locs.data_ptr(), score.data_ptr(), src.data_ptr(), S, B, J, H, W,
+                                               float(radius), float(downsample), float(threshold), int(bool(int_div)),
+                                               ctypes.c_void_p(stream)), "epi_find_peaks_best_f32")
+    return locs, score, src.long()                       # int64 like the indices of torch.max

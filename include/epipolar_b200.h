@@ -84,7 +84,14 @@ typedef struct EpiFusionParams {
     int32_t add_ref_residual;     /* 1: also add feat_ref (the caller's `ret + feat`, resnet.py:388) */
     int32_t variant;              /* EPI_VARIANT_* */
     int32_t feat_dtype;           /* EPI_DTYPE_* of feat_ref and feat_src (ABI v3; 0 = float32) */
-    int32_t reserved[2];
+    int32_t n_src;                /* source views per reference item, S = max(n_src, 1) (ABI v3; 0 or 1 = one source).  Pair
+                                     p = s·N + n (0 <= s < S, 0 <= n < N) fuses reference item n with source item p:
+                                     feat_ref / P_ref keep N items; feat_src is logical [S·N,C,H,W] (src_stride), P_src [S·N,3,4];
+                                     out, attn, corr_pos have S·N items and sample_locs_in / sample_locs_out are [K,S·N,H,W,2].
+                                     Every residual (add_ref_residual, also under the z epilogue) reads feat_ref[n]; z_residual
+                                     adds pair p's own fused feature.  The reference map is staged once for all S sources.
+                                     The cfg.EPIPOLAR.MULTITEST path of the reference (modeling/model.py:213-239) in one call. */
+    int32_t reserved[1];
     /* ---- optional persistent state (ABI v2) -------------------------------------------- */
     void *cache;                  /* device memory the caller keeps alive ACROSS calls and zero-fills once, or NULL.  Holds the
                                      per-pair constants and the epipolar pixel order keyed by (P_ref, P_src, H, W, downsample,
@@ -99,10 +106,11 @@ int epi_version(void);
 /* Thread-local description of the last error returned on this thread. */
 const char *epi_last_error(void);
 
-/* Bytes of scratch the forward needs for these shapes/strides/flags (0 is possible). */
+/* Bytes of scratch the forward needs for these shapes/strides/flags (0 is possible).  With n_src > 1 it covers N reference items
+ * and S·N source items and pairs. */
 size_t epi_fusion_workspace_bytes(const EpiFusionParams *p);
 
-/* Bytes of the optional persistent cache for these shapes (0 when the selected kernel keeps no cross-call state). */
+/* Bytes of the optional persistent cache for these shapes (0 when the selected kernel keeps no cross-call state); S·N pairs. */
 size_t epi_fusion_cache_bytes(const EpiFusionParams *p);
 
 /* The fused forward: geometry + K bilinear taps + softmax(QK)·V (+ z/BN epilogue, + residuals).
@@ -155,6 +163,14 @@ int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_lo
  * 0 the true division of current torch (what the reference computes under the torch installed with this library). */
 int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_t B, int32_t J, int32_t H, int32_t W,
                        float radius, float downsample, float threshold, int32_t int_div, void *stream);
+
+/* The best-source selection of the reference's multi-view test (modeling/model.py:229-234: torch.max over the sources' peak
+ * scores, then gather of their locations): heat [S,B,J,H,W] contiguous -> for every (b, j) the peak of the source with the
+ * highest score, locs [B,J,2], scores [B,J] and optionally (src_index != NULL) that source's index [B,J] as int32.  Each source's
+ * peak is computed exactly as epi_find_peaks_f32 computes it; a tie keeps the first source (torch.max).  S = 1 returns
+ * epi_find_peaks_f32's result bit for bit. */
+int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32_t *src_index, int32_t S, int32_t B, int32_t J,
+                            int32_t H, int32_t W, float radius, float downsample, float threshold, int32_t int_div, void *stream);
 
 /* Fold conv1x1 z + eval BatchNorm into (Wf, bf) on the device, no host sync:
  *   Wf[o,c] = s[o]·Wz[o,c],  bf[o] = s[o]·(bz[o] − mean[o]) + beta[o],  s = gamma/sqrt(var+bn_eps). */
