@@ -1,5 +1,5 @@
 // epi_abi.cu — the extern "C" boundary declared in include/epipolar_b200.h.
-// Validates arguments, carves the caller's workspace, launches kernels on the caller's stream.
+// Validates arguments, plans the forward (kernels, staging, workspace and cache regions) and launches the plan on the caller's stream.
 #include <cstdio>
 #include <cstring>
 
@@ -20,6 +20,30 @@ int fail(int code, const char *fmt, const char *detail = "") {
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
+constexpr size_t NONE = ~(size_t)0;      // offset of a region the plan does not use
+
+template <typename T>
+T *at(void *base, size_t off) { return off == NONE ? nullptr : reinterpret_cast<T *>(static_cast<char *>(base) + off); }
+
+// Consecutive regions of one buffer, each starting on a 256-byte boundary.  part() places a buffer right behind the previous one
+// in the same region (planes a kernel addresses from one base, such as [hi | lo]); close() ends the region.
+struct Regions {
+    size_t end = 0;
+    size_t part(size_t bytes) { const size_t off = end; end += bytes; return off; }
+    void close() { end = align_up(end); }
+    size_t take(size_t bytes) { const size_t off = part(bytes); close(); return off; }
+};
+
+// Counts the kernels a call launches and turns a failed launch into EPI_ECUDA "<what> launch failed: <CUDA error>".
+struct Launches {
+    int n = 0;
+    int operator()(const char *what, cudaError_t e, int kernels = 1) {
+        if (e == cudaSuccess) { n += kernels; return EPI_OK; }
+        snprintf(g_err, sizeof(g_err), "%s launch failed: %s", what, cudaGetErrorString(e));
+        return EPI_ECUDA;
+    }
+};
+
 // source views per reference item (EpiFusionParams.n_src: 0 and 1 both mean one)
 inline int n_sources(const EpiFusionParams *p) { return p->n_src > 1 ? p->n_src : 1; }
 // (reference, source) pairs = items of feat_src, out, attn, corr_pos and the sample locations
@@ -32,18 +56,33 @@ bool src_is_channels_last(const EpiFusionParams *p) {
            (reinterpret_cast<uintptr_t>(p->feat_src) % 16 == 0);
 }
 
+enum class Kernel { Pipe, Sector, Tile, Warp };          // fused attention kernel (sector and 4x8 block tiles: epi_fusion_tile_kernel)
+enum class Staging { Pipe, Planes, Nhwc, InPlace };      // feat_src: the pipe's staging launch, bf16 (hi, lo) planes, fp32 channels-last, as is
+enum class RefCopy { None, Before, After };              // fp32 channels-last copy of a low-precision feat_ref, before / after the fused kernel
+enum class Epilogue { Direct, Unstage, ZGemm, ZFp32 };   // who writes `out`: the fused kernel, a transposition pass, the z GEMM / z epilogue
+
+// Everything the forward decides, made from the params alone.  Offsets are NONE for the regions the plan does not use.
 struct Plan {
-    size_t off_src = 0, off_prez = 0, off_counter = 0, off_ref = 0, off_order = 0, off_wplanes = 0, off_geom = 0, off_ref32 = 0, total = 0;
-    bool stage_src = false, has_z = false, tile = false, sector = false, pipe = false, unstage = false;
-    bool ref32 = false;     // fp32 channels-last copy of a low-precision feat_ref for the kernels that read feat_ref as fp32
+    const char *refusal = nullptr;       // a forced variant this shape cannot run
+    Kernel kernel = Kernel::Warp;
+    Staging staging = Staging::InPlace;
+    RefCopy ref_copy = RefCopy::None;
+    Epilogue epilogue = Epilogue::Direct;
+    bool cached = false;                 // pair constants, pixel order and work records live in the caller's persistent cache
+    size_t ref_hi = NONE, ref_lo = NONE, src_hi = NONE, src_lo = NONE, src_nhwc = NONE, ref32 = NONE;      // workspace
+    size_t fused = NONE, fused_lo = NONE, counter = NONE, w_hi = NONE, w_lo = NONE, workspace_bytes = 0;
+    size_t order = NONE, geom = NONE;    // pixel order and pair constants: in the cache when `cached`, else in the workspace
+    size_t key = NONE, records = NONE, cache_bytes = 0;     // cache: per pair a key of 32 words (word 31: epoch of its work records)
+    int n_records = 0;
 };
 
 bool want_pipe(const EpiFusionParams *p) {
     if (p->variant != EPI_VARIANT_AUTO && p->variant != EPI_VARIANT_PIPE) return false;
     if (!epi::fusion_pipe_shape_ok(p->C, p->H, p->W, p->K, p->sample_locs_in != nullptr)) return false;
     // Automatic selection leaves one corner to the other kernels: K > 48 on maps of 2K pixels or more a side.  There a single pixel's
-    // taps (4K, sampled sparsely along a long line) already fill the 256-row union, so every work item splits down to one pixel and
-    // the per-pixel CUDA-core kernel does less work (tools/gpu_mapsize.py times the kernels per map size).
+    // taps (4K, sampled sparsely along a long line) already fill the 256-row union, so every work item splits down to one pixel.
+    // The tile kernel takes that corner where its shape limits allow (C <= 256, at most 16384 pixels), the warp kernel otherwise
+    // (tools/gpu_mapsize.py times the kernels per map size).
     if (p->variant == EPI_VARIANT_AUTO && 4 * p->K > 192 && (p->H > p->W ? p->H : p->W) >= 2 * p->K) return false;
     return true;
 }
@@ -55,54 +94,71 @@ bool want_tile(const EpiFusionParams *p) {
 }
 
 // Sizes: `ref_map` is one fp32 copy of the N reference items, `map` one fp32 map of the S·N pairs (source items, fused features).
-// The reference planes are staged once however many sources they are fused with.
+// The reference planes are staged once however many sources they are fused with.  One bf16 plane of a map is half its fp32 bytes.
 Plan make_plan(const EpiFusionParams *p) {
     Plan pl;
-    const size_t ref_map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
-    const size_t map = (size_t)n_pairs(p) * p->C * p->H * p->W * sizeof(float);
-    const size_t NP = (size_t)n_pairs(p);
-    const bool lowp = p->feat_dtype != EPI_DTYPE_F32;
-    pl.pipe = want_pipe(p);
-    if (pl.pipe) {
-        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes (bytes of one fp32 reference map + one fp32 source map; bf16 maps:
-        // [ref_hi | src_hi], half of that), pre-z planes, pixel order, pair constants
-        pl.has_z = p->z_weight_folded != nullptr;
-        size_t off = 0;
-        pl.off_ref = off; off += align_up(p->feat_dtype == EPI_DTYPE_BF16 ? (ref_map + map) / 2 : ref_map + map);
-        // pre-z planes (z path) or the pixel-major fp32 plane the fused kernel writes when the caller's tensor is NCHW
-        pl.unstage = !pl.has_z && !(p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0);
-        if (pl.has_z || pl.unstage) { pl.off_prez = off; off += align_up(map); }
-        pl.off_counter = off; off += 256;
-        if (pl.has_z && epi::zgemm_supported(p->C)) { pl.off_wplanes = off; off += align_up((size_t)p->C * p->C * 4); }
-        pl.ref32 = lowp && pl.has_z && !epi::zgemm_supported(p->C) && p->add_ref_residual;      // the fp32 z epilogue's residual
-        if (pl.ref32) { pl.off_ref32 = off; off += align_up(ref_map); }
-        if (!p->cache) {               // no persistent cache: pixel order and pair constants are rebuilt in the workspace every call
-            pl.off_order = off; off += align_up(NP * p->H * p->W * sizeof(uint16_t));
-            pl.off_geom = off; off += align_up(NP * sizeof(epi::PairGeom));
-        }
-        pl.total = off;
-        return pl;
-    }
-    pl.tile = want_tile(p);
+    const size_t NP = (size_t)n_pairs(p), px = (size_t)p->H * p->W;
+    const size_t ref_map = (size_t)p->N * p->C * px * sizeof(float), map = NP * p->C * px * sizeof(float);
+    const size_t order_bytes = NP * px * sizeof(uint16_t), geom_bytes = NP * sizeof(epi::PairGeom);
+    const bool lowp = p->feat_dtype != EPI_DTYPE_F32, has_z = p->z_weight_folded != nullptr;
     // sector tiles (pixels grouped by epipolar angle) need the fused geometry; injected locations and an explicit
     // EPI_VARIANT_TILE request use the 4x8 block tiles
-    pl.sector = pl.tile && p->variant != EPI_VARIANT_TILE && p->sample_locs_in == nullptr;
-    // tile kernel: bf16 (hi, lo) planes, same bytes as one fp32 map; the warp kernel reads a channels-last fp32 source in place
-    pl.stage_src = pl.tile || !src_is_channels_last(p) || lowp;
-    pl.has_z = p->z_weight_folded != nullptr;
-    pl.ref32 = lowp;                                         // these kernels read the query (and the residual) as fp32
-    size_t off = 0;
-    if (pl.ref32) { pl.off_ref32 = off; off += align_up(ref_map); }
-    if (pl.stage_src) { pl.off_src = off; off += align_up(map); }
-    if (pl.has_z) { pl.off_prez = off; off += align_up(map); }
-    if (pl.tile) { pl.off_counter = off; off += 256; }
-    if (pl.sector) {
-        pl.off_ref = off; off += align_up(ref_map);
-        pl.off_order = off; off += align_up(NP * p->H * p->W * sizeof(uint16_t));
+    if (want_pipe(p)) pl.kernel = Kernel::Pipe;
+    else if (want_tile(p)) pl.kernel = p->variant != EPI_VARIANT_TILE && p->sample_locs_in == nullptr ? Kernel::Sector : Kernel::Tile;
+    if (p->variant == EPI_VARIANT_PIPE && pl.kernel != Kernel::Pipe) pl.refusal = "pipe variant does not support this shape";
+    if (p->variant == EPI_VARIANT_TILE && pl.kernel != Kernel::Tile) pl.refusal = "tile variant does not support this shape";
+    if (p->variant == EPI_VARIANT_SECTOR && pl.kernel != Kernel::Sector)
+        pl.refusal = "sector variant does not support this shape / injected locations";
+
+    Regions ws;
+    if (pl.kernel == Kernel::Pipe) {
+        // without z the fused kernel writes a channels-last `out` with 16-byte stores; any other `out` gets a pixel-major plane
+        const bool out_direct = p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0;
+        pl.staging = Staging::Pipe;
+        pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32) : (out_direct ? Epilogue::Direct : Epilogue::Unstage);
+        if (lowp && pl.epilogue == Epilogue::ZFp32 && p->add_ref_residual) pl.ref_copy = RefCopy::After;   // the fp32 z epilogue's residual
+        pl.cached = p->cache != nullptr;
+        // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes; bf16 maps have no lo part: [ref_hi | src_hi]
+        const bool lo = p->feat_dtype != EPI_DTYPE_BF16;
+        pl.ref_hi = ws.part(ref_map / 2);
+        if (lo) pl.ref_lo = ws.part(ref_map / 2);
+        pl.src_hi = ws.part(map / 2);
+        if (lo) pl.src_lo = ws.part(map / 2);
+        ws.close();
+        // fused feature: bf16 (hi, lo) planes for the z GEMM; fp32, contiguous NCHW for the z epilogue, pixel-major for the transposition
+        if (pl.epilogue == Epilogue::ZGemm) { pl.fused = ws.part(map / 2); pl.fused_lo = ws.take(map / 2); }
+        else if (pl.epilogue != Epilogue::Direct) pl.fused = ws.take(map);
+        pl.counter = ws.take(256);
+        // folded z weight (+ I with ZRESIDUAL) as bf16 (hi, lo) planes, written by the staging launch
+        if (pl.epilogue == Epilogue::ZGemm) { pl.w_hi = ws.part((size_t)p->C * p->C * 2); pl.w_lo = ws.take((size_t)p->C * p->C * 2); }
+        if (pl.ref_copy == RefCopy::After) pl.ref32 = ws.take(ref_map);
+        Regions cache;
+        pl.key = cache.take(NP * 32 * sizeof(float));
+        const size_t cache_geom = cache.take(geom_bytes), cache_order = cache.take(order_bytes);
+        pl.n_records = epi::fusion_pipe_plan_records((int)NP, p->N, p->H, p->W);
+        pl.records = cache.take((size_t)pl.n_records * epi::fusion_pipe_plan_record_bytes());
+        pl.cache_bytes = cache.end;
+        if (pl.cached) { pl.geom = cache_geom; pl.order = cache_order; }
+        else { pl.order = ws.take(order_bytes); pl.geom = ws.take(geom_bytes); }      // rebuilt every call
+    } else {
+        // the tile kernel reads bf16 (hi, lo) planes; the warp kernel reads a channels-last fp32 source in place
+        const bool tiles = pl.kernel != Kernel::Warp;
+        pl.staging = tiles ? Staging::Planes : (!src_is_channels_last(p) || lowp ? Staging::Nhwc : Staging::InPlace);
+        pl.epilogue = has_z ? Epilogue::ZFp32 : Epilogue::Direct;
+        pl.ref_copy = lowp ? RefCopy::Before : RefCopy::None;        // these kernels read the query (and the residual) as fp32
+        if (lowp) pl.ref32 = ws.take(ref_map);
+        if (tiles) { pl.src_hi = ws.part(map / 2); pl.src_lo = ws.take(map / 2); }
+        else if (pl.staging == Staging::Nhwc) pl.src_nhwc = ws.take(map);
+        if (has_z) pl.fused = ws.take(map);
+        if (tiles) pl.counter = ws.take(256);
+        if (pl.kernel == Kernel::Sector) { pl.ref_hi = ws.part(ref_map / 2); pl.ref_lo = ws.take(ref_map / 2); pl.order = ws.take(order_bytes); }
     }
-    pl.total = off;
+    pl.workspace_bytes = ws.end;
     return pl;
 }
+
+// the size queries answer 0 for params no plan is made for
+bool plannable(const EpiFusionParams *p) { return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0; }
 
 int validate(const EpiFusionParams *p) {
     if (!p) return fail(EPI_EINVAL, "params is null");
@@ -127,6 +183,30 @@ int validate(const EpiFusionParams *p) {
     if (p->z_weight_folded && (reinterpret_cast<uintptr_t>(p->z_weight_folded) % 16 != 0 || reinterpret_cast<uintptr_t>(p->z_bias_folded) % 4 != 0))
         return fail(EPI_EINVAL, "z_weight_folded must be 16-byte aligned (contiguous [C,C]) and z_bias_folded 4-byte aligned");
     return EPI_OK;
+}
+
+int validate_bwd(const EpiFusionBwdParams *p) {
+    if (!p) return fail(EPI_EINVAL, "params is null");
+    if (!p->feat_ref || !p->feat_src || !p->attn || !p->grad_out) return fail(EPI_EINVAL, "feat_ref/feat_src/attn/grad_out must be non-null");
+    if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
+    if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2 || p->K < 2 || p->K > 256) return fail(EPI_EINVAL, "bad shape");
+    if (p->C > 512 || (p->C > 128 && p->C % 4 != 0)) return fail(EPI_EINVAL, "backward supports C <= 128, or C <= 512 with C % 4 == 0");
+    if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    return EPI_OK;
+}
+
+// Backward workspace: pixel-major copy of feat_src + pixel-major accumulator of its gradient; low-precision maps: + a channels-last
+// fp32 copy of feat_ref and a pixel-major fp32 buffer of its gradient (rounded once to the maps' type by the transposition pass)
+struct BwdPlan { size_t map, src, dsrc, ref32 = NONE, gref32 = NONE, workspace_bytes; };
+
+BwdPlan make_bwd_plan(const EpiFusionBwdParams *p) {
+    BwdPlan pl;
+    Regions ws;
+    pl.map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
+    pl.src = ws.take(pl.map); pl.dsrc = ws.take(pl.map);
+    if (p->feat_dtype != EPI_DTYPE_F32) { pl.ref32 = ws.take(pl.map); pl.gref32 = ws.take(pl.map); }
+    pl.workspace_bytes = ws.end;
+    return pl;
 }
 
 epi::GeomCfg make_geom(int H, int W, int K, float ds, float r, float eps, int correct, int align) {
@@ -173,35 +253,27 @@ float epi_kernel_timing_last_ms(void) {
     return ms;
 }
 
-// per pair: key (32 words), constants, pixel order, work records of the pipelined kernel
-size_t epi_fusion_cache_bytes(const EpiFusionParams *p) {
-    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0 || p->n_src < 0 || !want_pipe(p)) return 0;
-    const size_t NP = (size_t)n_pairs(p);
-    return align_up(NP * 32 * sizeof(float)) + align_up(NP * sizeof(epi::PairGeom)) +
-           align_up(NP * p->H * p->W * sizeof(uint16_t)) +
-           align_up((size_t)epi::fusion_pipe_plan_records((int)NP, p->N, p->H, p->W) * epi::fusion_pipe_plan_record_bytes());
-}
+size_t epi_fusion_cache_bytes(const EpiFusionParams *p) { return plannable(p) ? make_plan(p).cache_bytes : 0; }
 
-size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) {
-    if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0 || p->n_src < 0) return 0;
-    return make_plan(p).total;
-}
+size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) { return plannable(p) ? make_plan(p).workspace_bytes : 0; }
 
 int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     int rc = validate(p);
     if (rc != EPI_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const Plan pl = make_plan(p);
-    if (pl.total > 0 && (!p->workspace || p->workspace_bytes < pl.total)) return fail(EPI_EWORKSPACE, "workspace too small");
-    if (pl.total > 0 && reinterpret_cast<uintptr_t>(p->workspace) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
-    char *ws = static_cast<char *>(p->workspace);
-    int launches = 0;
-    cudaError_t e;
-    const __nv_bfloat16 *w_hi = nullptr, *w_lo = nullptr;
+    void *ws = p->workspace;
+    if (pl.workspace_bytes > 0 && (!ws || p->workspace_bytes < pl.workspace_bytes)) return fail(EPI_EWORKSPACE, "workspace too small");
+    if (pl.workspace_bytes > 0 && reinterpret_cast<uintptr_t>(ws) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
     g_timing_valid = 0;
     if (g_timing) {
         if (!g_ev0) { cudaEventCreate(&g_ev0); cudaEventCreate(&g_ev1); cudaEventCreate(&g_evA); cudaEventCreate(&g_evB); }
         cudaEventRecord(g_evA, st);
+    }
+    if (pl.refusal) return fail(EPI_EINVAL, "%s", pl.refusal);
+    if (pl.cached) {
+        if (p->cache_bytes < pl.cache_bytes) return fail(EPI_EWORKSPACE, "cache too small");
+        if (reinterpret_cast<uintptr_t>(p->cache) % 256 != 0) return fail(EPI_EINVAL, "cache must be 256-byte aligned");
     }
 
     const int dt = p->feat_dtype;
@@ -214,192 +286,130 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     a.N = NP; a.n_ref = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale;
     for (int i = 0; i < 4; i++) a.ref_stride[i] = p->ref_stride[i];
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
-    // fp32 kernels that read feat_ref get a channels-last fp32 copy of a low-precision map
-    float *ref32 = pl.ref32 ? reinterpret_cast<float *>(ws + pl.off_ref32) : nullptr;
-    const int64_t ref32_stride[4] = {(int64_t)p->C * p->H * p->W, 1, (int64_t)p->W * p->C, p->C};
+    float *ref32 = at<float>(ws, pl.ref32);
+    const int64_t cl_stride[4] = {(int64_t)p->C * p->H * p->W, 1, (int64_t)p->W * p->C, p->C};      // channels-last / pixel-major
+    Launches run;
 
-    if (p->variant == EPI_VARIANT_PIPE && !pl.pipe) return fail(EPI_EINVAL, "pipe variant does not support this shape");
-    if (pl.pipe) {
-        const size_t ref_elems = (size_t)p->N * p->C * p->H * p->W, elems = (size_t)NP * p->C * p->H * p->W;
-        __nv_bfloat16 *planes = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_ref);
-        int *words = reinterpret_cast<int *>(ws + pl.off_counter);
-        const bool have_P = p->P_ref && p->P_src;
-        uint16_t *order = nullptr;
-        epi::PairGeom *pg = nullptr;
-        float *okey = nullptr;
-        if (p->cache) {
-            if (p->cache_bytes < epi_fusion_cache_bytes(p)) return fail(EPI_EWORKSPACE, "cache too small");
-            if (reinterpret_cast<uintptr_t>(p->cache) % 256 != 0) return fail(EPI_EINVAL, "cache must be 256-byte aligned");
-            char *cb = static_cast<char *>(p->cache);
-            okey = reinterpret_cast<float *>(cb);
-            pg = reinterpret_cast<epi::PairGeom *>(cb + align_up((size_t)NP * 32 * sizeof(float)));
-            order = reinterpret_cast<uint16_t *>(cb + align_up((size_t)NP * 32 * sizeof(float)) + align_up((size_t)NP * sizeof(epi::PairGeom)));
-            if (have_P) {                      // cached work items of the fused kernel, valid per pair for the epoch stored in key slot 31
-                a.plan_cache = reinterpret_cast<uint8_t *>(order) + align_up((size_t)NP * p->H * p->W * sizeof(uint16_t));
-                a.plan_records = epi::fusion_pipe_plan_records(NP, p->N, p->H, p->W);
-                a.pair_epoch = reinterpret_cast<const uint32_t *>(okey) + 31;
-            }
-        } else {
-            order = reinterpret_cast<uint16_t *>(ws + pl.off_order);
-            pg = reinterpret_cast<epi::PairGeom *>(ws + pl.off_geom);
-        }
-        if (!have_P) { order = nullptr; okey = nullptr; }
-        const bool z_planes = pl.has_z && epi::zgemm_supported(p->C);
-        __nv_bfloat16 *wpl = z_planes ? reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_wplanes) : nullptr;
-        e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, planes, p->P_ref, p->P_src, pg, order, okey,
-                              z_planes ? p->z_weight_folded : nullptr, wpl, p->z_residual ? 1 : 0, words, NP, p->N, p->C, p->H, p->W, a.geom, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
-        launches += (order && (size_t)p->H * p->W * 2 + 16384 > 64 * 1024) ? 2 : 1;      // large maps order their pixels in a launch of their own
-        w_hi = wpl; w_lo = wpl ? wpl + (size_t)p->C * p->C : nullptr;
-        if (dt == EPI_DTYPE_BF16) { a.ref_hi = planes; a.src_hi = planes + ref_elems; }       // no lo planes: the pipe kernel's LO = false form
-        else { a.ref_hi = planes; a.ref_lo = planes + ref_elems; a.src_hi = planes + 2 * ref_elems; a.src_lo = planes + 2 * ref_elems + elems; }
-        a.order = order; a.pair_geom = pg; a.tile_counter = words; a.err_flag = words + 1;
-    } else
-    if (p->variant == EPI_VARIANT_TILE && !pl.tile) return fail(EPI_EINVAL, "tile variant does not support this shape");
-    if (p->variant == EPI_VARIANT_SECTOR && !pl.sector) return fail(EPI_EINVAL, "sector variant does not support this shape / injected locations");
-    if (!pl.pipe && ref32) {
-        e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
-        launches++;
+    // operand staging (first timing group)
+    if (pl.ref_copy == RefCopy::Before) {
+        if ((rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
         a.feat_ref = ref32; a.ref_dtype = EPI_DTYPE_F32;
-        for (int i = 0; i < 4; i++) a.ref_stride[i] = ref32_stride[i];
+        for (int i = 0; i < 4; i++) a.ref_stride[i] = cl_stride[i];
     }
-    if (pl.tile) {
-        __nv_bfloat16 *hi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_src);
-        __nv_bfloat16 *lo = hi + (size_t)NP * p->C * p->H * p->W;
-        a.tile_counter = reinterpret_cast<int *>(ws + pl.off_counter);
-        e = epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, NP, p->C, p->H, p->W, a.tile_counter, dt, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "operand staging launch failed: %s", cudaGetErrorString(e));
-        launches++;
+    if (pl.staging == Staging::Pipe) {
+        const bool have_P = p->P_ref && p->P_src;
+        void *pairs = pl.cached ? p->cache : ws;
+        uint16_t *order = have_P ? at<uint16_t>(pairs, pl.order) : nullptr;
+        epi::PairGeom *pg = at<epi::PairGeom>(pairs, pl.geom);
+        float *okey = pl.cached && have_P ? at<float>(p->cache, pl.key) : nullptr;
+        if (okey) {                        // cached work items of the fused kernel, valid per pair for the epoch stored in key slot 31
+            a.plan_cache = at<uint8_t>(p->cache, pl.records);
+            a.plan_records = pl.n_records;
+            a.pair_epoch = reinterpret_cast<const uint32_t *>(okey) + 31;
+        }
+        int *words = at<int>(ws, pl.counter);
+        __nv_bfloat16 *w_hi = at<__nv_bfloat16>(ws, pl.w_hi);
+        int kernels = 0;
+        const cudaError_t e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, at<__nv_bfloat16>(ws, pl.ref_hi),
+                                                p->P_ref, p->P_src, pg, order, okey, w_hi ? p->z_weight_folded : nullptr, w_hi,
+                                                p->z_residual ? 1 : 0, words, NP, p->N, p->C, p->H, p->W, a.geom, st, kernels);
+        if ((rc = run("operand staging", e, kernels))) return rc;
+        a.ref_hi = at<__nv_bfloat16>(ws, pl.ref_hi); a.ref_lo = at<__nv_bfloat16>(ws, pl.ref_lo);
+        a.src_hi = at<__nv_bfloat16>(ws, pl.src_hi); a.src_lo = at<__nv_bfloat16>(ws, pl.src_lo);
+        a.order = order; a.pair_geom = pg; a.tile_counter = words; a.err_flag = words + 1;
+    } else if (pl.staging == Staging::Planes) {
+        __nv_bfloat16 *hi = at<__nv_bfloat16>(ws, pl.src_hi), *lo = at<__nv_bfloat16>(ws, pl.src_lo);
+        a.tile_counter = at<int>(ws, pl.counter);
+        if ((rc = run("operand staging", epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, NP, p->C, p->H, p->W, a.tile_counter, dt, st)))) return rc;
         a.src_hi = hi; a.src_lo = lo;
-        if (pl.sector) {
-            __nv_bfloat16 *rhi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_ref);
-            __nv_bfloat16 *rlo = rhi + (size_t)p->N * p->C * p->H * p->W;
-            e = epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st);
-            if (e != cudaSuccess) return fail(EPI_ECUDA, "reference staging launch failed: %s", cudaGetErrorString(e));
-            uint16_t *order = reinterpret_cast<uint16_t *>(ws + pl.off_order);
-            e = epi::launch_sector_order(p->P_ref, p->P_src, order, NP, p->N, a.geom, st);
-            if (e != cudaSuccess) return fail(EPI_ECUDA, "sector ordering launch failed: %s", cudaGetErrorString(e));
-            launches += 2;
+        if (pl.kernel == Kernel::Sector) {
+            __nv_bfloat16 *rhi = at<__nv_bfloat16>(ws, pl.ref_hi), *rlo = at<__nv_bfloat16>(ws, pl.ref_lo);
+            uint16_t *order = at<uint16_t>(ws, pl.order);
+            if ((rc = run("reference staging", epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st)))) return rc;
+            if ((rc = run("sector ordering", epi::launch_sector_order(p->P_ref, p->P_src, order, NP, p->N, a.geom, st)))) return rc;
             a.ref_hi = rhi; a.ref_lo = rlo; a.order = order;
         }
-    } else if (pl.stage_src) {
-        float *nhwc = reinterpret_cast<float *>(ws + pl.off_src);
-        e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, NP, p->C, p->H, p->W, dt, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "layout staging launch failed: %s", cudaGetErrorString(e));
-        launches++;
+    } else if (pl.staging == Staging::Nhwc) {
+        float *nhwc = at<float>(ws, pl.src_nhwc);
+        if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, NP, p->C, p->H, p->W, dt, st)))) return rc;
         a.src_nhwc = nhwc;
     } else {
         a.src_nhwc = static_cast<const float *>(p->feat_src);
     }
 
-    const bool z_tc = pl.has_z && pl.pipe && epi::zgemm_supported(p->C);      // tensor-core z GEMM (operand planes come from the staging launch)
-    if (z_tc) {         // fused feature leaves the tile kernel as bf16 (hi, lo) planes: the A operand of the z GEMM
-        a.out = nullptr;
-        a.out_hi = reinterpret_cast<__nv_bfloat16 *>(ws + pl.off_prez);
-        a.out_lo = a.out_hi + (size_t)NP * p->C * p->H * p->W;
-        a.add_ref = 0;
-    } else if (pl.pipe && pl.unstage) {   // fused feature leaves the kernel pixel-major (full 128-byte lines); a transposition pass writes `out`
-        a.out = reinterpret_cast<float *>(ws + pl.off_prez);
-        a.out_stride[0] = (int64_t)p->C * p->H * p->W; a.out_stride[1] = 1;
-        a.out_stride[2] = (int64_t)p->W * p->C; a.out_stride[3] = p->C;
-        a.add_ref = 0;
-    } else if (pl.has_z) {     // fused feature goes to the pre-z buffer (contiguous NCHW), epilogue writes `out`
-        a.out = reinterpret_cast<float *>(ws + pl.off_prez);
-        a.out_stride[0] = (int64_t)p->C * p->H * p->W; a.out_stride[1] = (int64_t)p->H * p->W;
-        a.out_stride[2] = p->W; a.out_stride[3] = 1;
-        a.add_ref = 0;
+    // where the fused kernel writes
+    if (pl.epilogue == Epilogue::ZGemm) {
+        a.out_hi = at<__nv_bfloat16>(ws, pl.fused); a.out_lo = at<__nv_bfloat16>(ws, pl.fused_lo);
+    } else if (pl.epilogue != Epilogue::Direct) {    // pixel-major (full 128-byte lines) for the transposition pass, NCHW for the z epilogue
+        const int64_t nchw_stride[4] = {(int64_t)p->C * p->H * p->W, (int64_t)p->H * p->W, p->W, 1};
+        a.out = at<float>(ws, pl.fused);
+        for (int i = 0; i < 4; i++) a.out_stride[i] = pl.epilogue == Epilogue::Unstage ? cl_stride[i] : nchw_stride[i];
     } else {
         a.out = p->out;
         for (int i = 0; i < 4; i++) a.out_stride[i] = p->out_stride[i];
         a.add_ref = p->add_ref_residual;
     }
 
-    const bool use_tile = pl.tile && epi::fusion_tile_supported(a);
-    if (pl.tile && !use_tile) return fail(EPI_EINVAL, "internal: tile plan without tile support");
     if (g_timing) cudaEventRecord(g_ev0, st);
-    e = pl.pipe ? epi::launch_fusion_pipe(a, st) : (use_tile ? epi::launch_fusion_tile(a, st) : epi::launch_fusion_warp(a, st));
-    if (e != cudaSuccess) return fail(EPI_ECUDA, "fusion kernel launch failed: %s", cudaGetErrorString(e));
+    const cudaError_t e = pl.kernel == Kernel::Pipe ? epi::launch_fusion_pipe(a, st)
+                        : pl.kernel == Kernel::Warp ? epi::launch_fusion_warp(a, st) : epi::launch_fusion_tile(a, st);
+    if ((rc = run("fusion kernel", e))) return rc;
     if (g_timing) cudaEventRecord(g_ev1, st);
-    launches++;
 
-    if (pl.pipe && pl.unstage) {
-        e = epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out, EPI_DTYPE_F32, p->out_stride,
-                                NP, p->N, p->C, p->H, p->W, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "output transposition launch failed: %s", cudaGetErrorString(e));
-        launches++;
-    }
-    if (z_tc) {
+    // epilogue (third timing group)
+    if (pl.ref_copy == RefCopy::After &&
+        (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
+    if (pl.epilogue == Epilogue::Unstage) {
+        if ((rc = run("output transposition", epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out,
+                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, p->C, p->H, p->W, st)))) return rc;
+    } else if (pl.epilogue == Epilogue::ZGemm) {
         epi::ZGemmArgs z;
         memset(&z, 0, sizeof(z));
-        z.x_hi = a.out_hi; z.x_lo = a.out_lo; z.w_hi = w_hi; z.w_lo = w_lo; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
+        z.x_hi = a.out_hi; z.x_lo = a.out_lo; z.w_hi = at<__nv_bfloat16>(ws, pl.w_hi); z.w_lo = at<__nv_bfloat16>(ws, pl.w_lo);
+        z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.ref = p->feat_ref; z.ref_dtype = dt; z.y = p->out;
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
         z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
-        e = epi::launch_zgemm(z, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "z GEMM launch failed: %s", cudaGetErrorString(e));
-        launches++;
-    } else if (pl.has_z) {
-        if (pl.pipe && ref32) {            // (the other kernels' plans made the copy before the fused kernel)
-            e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
-            if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
-            launches++;
-        }
+        if ((rc = run("z GEMM", epi::launch_zgemm(z, st)))) return rc;
+    } else if (pl.epilogue == Epilogue::ZFp32) {
         epi::ZArgs z;
         memset(&z, 0, sizeof(z));
         z.x = a.out;
-        for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? ref32_stride[i] : p->ref_stride[i]; }
+        for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? cl_stride[i] : p->ref_stride[i]; }
         z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
-        e = epi::launch_z_epilogue(z, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "z epilogue launch failed: %s", cudaGetErrorString(e));
-        launches++;
+        if ((rc = run("z epilogue", epi::launch_z_epilogue(z, st)))) return rc;
     }
     if (g_timing) { cudaEventRecord(g_evB, st); g_timing_valid = 1; }
-    g_launches = launches;
+    g_launches = run.n;
     return EPI_OK;
 }
 
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p) {
     if (!p || p->N <= 0 || p->C <= 0 || p->H <= 0 || p->W <= 0) return 0;
-    const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
-    // pixel-major copy of feat_src + pixel-major accumulator of its gradient; low-precision maps: + a channels-last fp32 copy of
-    // feat_ref and a pixel-major fp32 buffer of its gradient (rounded once to the maps' type by the transposition pass)
-    return (p->feat_dtype != EPI_DTYPE_F32 ? 4 : 2) * align_up(map);
+    return make_bwd_plan(p).workspace_bytes;
 }
 
 int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
-    if (!p) return fail(EPI_EINVAL, "params is null");
-    if (!p->feat_ref || !p->feat_src || !p->attn || !p->grad_out) return fail(EPI_EINVAL, "feat_ref/feat_src/attn/grad_out must be non-null");
-    if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
-    if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2 || p->K < 2 || p->K > 256) return fail(EPI_EINVAL, "bad shape");
-    if (p->C > 512 || (p->C > 128 && p->C % 4 != 0)) return fail(EPI_EINVAL, "backward supports C <= 128, or C <= 512 with C % 4 == 0");
-    if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    int rc = validate_bwd(p);
+    if (rc != EPI_OK) return rc;
     if (!p->grad_ref && !p->grad_src) return EPI_OK;
-    const size_t need = epi_fusion_backward_workspace_bytes(p);
-    if (!p->workspace || p->workspace_bytes < need) return fail(EPI_EWORKSPACE, "workspace too small");
-    if (reinterpret_cast<uintptr_t>(p->workspace) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
+    const BwdPlan pl = make_bwd_plan(p);
+    void *ws = p->workspace;
+    if (!ws || p->workspace_bytes < pl.workspace_bytes) return fail(EPI_EWORKSPACE, "workspace too small");
+    if (reinterpret_cast<uintptr_t>(ws) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const size_t map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
     const int dt = p->feat_dtype;
     const bool lowp = dt != EPI_DTYPE_F32;
-    float *nhwc = reinterpret_cast<float *>(p->workspace);
-    float *dsrc = reinterpret_cast<float *>(static_cast<char *>(p->workspace) + align_up(map));
-    float *ref32 = lowp ? reinterpret_cast<float *>(static_cast<char *>(p->workspace) + 2 * align_up(map)) : nullptr;
-    float *gref32 = lowp ? reinterpret_cast<float *>(static_cast<char *>(p->workspace) + 3 * align_up(map)) : nullptr;
+    float *nhwc = at<float>(ws, pl.src), *dsrc = at<float>(ws, pl.dsrc), *ref32 = at<float>(ws, pl.ref32), *gref32 = at<float>(ws, pl.gref32);
     const int64_t pm_stride[4] = {(int64_t)p->C * p->H * p->W, 1, (int64_t)p->W * p->C, p->C};      // pixel-major / channels-last
-    cudaError_t e = epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st);
-    if (e != cudaSuccess) return fail(EPI_ECUDA, "layout staging launch failed: %s", cudaGetErrorString(e));
-    int launches = 1;
-    if (lowp) {
-        e = epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "reference conversion launch failed: %s", cudaGetErrorString(e));
-        launches++;
-    }
+    Launches run;
+    if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st)))) return rc;
+    if (lowp && (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
     if (p->grad_src) {
-        e = cudaMemsetAsync(dsrc, 0, map, st);
+        const cudaError_t e = cudaMemsetAsync(dsrc, 0, pl.map, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "memset failed: %s", cudaGetErrorString(e));
     }
     epi::BwdArgs a;
@@ -414,20 +424,14 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     }
     a.N = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale; a.grad_keys = p->grad_keys; a.grad_vals = p->grad_vals;
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
-    e = epi::launch_fusion_bwd(a, st);
-    if (e != cudaSuccess) return fail(EPI_ECUDA, "backward kernel launch failed: %s", cudaGetErrorString(e));
-    launches++;
-    if (p->grad_src) {
-        e = epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride, p->N, p->N, p->C, p->H, p->W, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
-        launches++;
-    }
-    if (p->grad_ref && lowp) {         // fp32 gradient of a low-precision reference map, rounded once to its type
-        e = epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride, p->N, p->N, p->C, p->H, p->W, st);
-        if (e != cudaSuccess) return fail(EPI_ECUDA, "gradient transposition launch failed: %s", cudaGetErrorString(e));
-        launches++;
-    }
-    g_launches = launches;
+    if ((rc = run("backward kernel", epi::launch_fusion_bwd(a, st)))) return rc;
+    if (p->grad_src &&
+        (rc = run("gradient transposition", epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride,
+                                                                p->N, p->N, p->C, p->H, p->W, st)))) return rc;
+    if (p->grad_ref && lowp &&         // fp32 gradient of a low-precision reference map, rounded once to its type
+        (rc = run("gradient transposition", epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride,
+                                                                p->N, p->N, p->C, p->H, p->W, st)))) return rc;
+    g_launches = run.n;
     return EPI_OK;
 }
 

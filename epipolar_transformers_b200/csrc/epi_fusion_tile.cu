@@ -589,16 +589,14 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
   }
 }
 
-bool fusion_tile_supported(const FusionArgs &a) {
-    const int H = a.geom.H, W = a.geom.W, K = a.geom.K, C = a.C;
+bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in) {
     if (C % 8 != 0 || C > 256) return false;
     if (H * W > MAXWORDS * 32 || H * W > 65535) return false;
     if (K > 32 * MAXKPL) return false;
     // a single pixel's union must fit DMAX: 4 taps per sample, and (fused geometry) a straight line
     // crosses at most H+W pixel rows/columns, 2 pixels wide, plus the footprint ends
-    const int single = a.locs_in ? 4 * K : min(4 * K, 2 * (H + W) + 8);
-    if (single > DMAX) return false;
-    return a.src_hi != nullptr && a.src_lo != nullptr;
+    const int single = has_locs_in ? 4 * K : min(4 * K, 2 * (H + W) + 8);
+    return single <= DMAX;
 }
 
 cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
@@ -710,13 +708,5 @@ extern "C" void epi_tile_timers_read(unsigned long long *out16, int reset) {
     if (reset) { unsigned long long z[16] = {0}; cudaMemcpyToSymbol(g_tile_timers, z, sizeof(z)); }
 }
 #endif
-
-bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in) {
-    FusionArgs a{};
-    a.C = C; a.geom.H = H; a.geom.W = W; a.geom.K = K;
-    a.locs_in = has_locs_in ? reinterpret_cast<const float *>(1) : nullptr;
-    a.src_hi = reinterpret_cast<const __nv_bfloat16 *>(1); a.src_lo = a.src_hi;
-    return fusion_tile_supported(a);
-}
 
 }  // namespace epi

@@ -80,7 +80,6 @@ cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st);
 bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 size_t fusion_pipe_plan_record_bytes();
 int fusion_pipe_plan_records(int N, int n_ref, int H, int W);   // N pairs on n_ref reference items
-bool fusion_tile_supported(const FusionArgs &a);
 bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 // pair n: P_ref item n % n_ref, P_src item n
 cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, const GeomCfg &gc, cudaStream_t st);
@@ -89,11 +88,12 @@ cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_b
                                 int H, int W, int *zero_me, int dtype, cudaStream_t st);
 
 // planes: [ref_hi | ref_lo | src_hi | src_lo] for fp32 / fp16 maps, [ref_hi | src_hi] for bf16 maps (their lo part is zero);
-// the reference planes hold n_ref items, the source planes (and the pair constants / orders) N pairs, pair n on reference n % n_ref
+// the reference planes hold n_ref items, the source planes (and the pair constants / orders) N pairs, pair n on reference n % n_ref;
+// `launched`: kernels started on success (2 when a large map orders its pixels in a launch of its own)
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
-                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st);
+                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched);
 
 cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
                                 cudaStream_t st);

@@ -494,7 +494,7 @@ template <typename T>
 static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], const T *src, const int64_t src_stride[4],
                                   __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                                   float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
-                                  int n_ref, int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
+                                  int n_ref, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
     StageArgs<T> s;
     s.ref = ref; s.src = src;
     for (int i = 0; i < 4; i++) { s.ref_stride[i] = ref_stride[i]; s.src_stride[i] = src_stride[i]; }
@@ -523,7 +523,9 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     };
     // Shared memory is a per-launch size: above 64 KB the order blocks' pixel list would cut the residency of every transposition
     // block of the same launch, so maps that large order their pixels in a launch of their own (a no-op on a cached camera pair).
-    if (s.do_order && smem_order > 64 * 1024) {
+    const bool order_apart = s.do_order && smem_order > 64 * 1024;
+    launched = order_apart ? 2 : 1;
+    if (order_apart) {
         StageArgs<T> o = s;
         o.do_ref = 0; o.do_src = 0; o.Wf = nullptr; o.w_planes = nullptr; o.persist = 0;
         cudaError_t e = ensure(smem_order);
@@ -557,15 +559,15 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
-                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st) {
+                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
     if (dtype == kBF16)
         return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
     if (dtype == kF16)
         return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
     return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
-                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st);
+                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
 }
 
 }  // namespace epi

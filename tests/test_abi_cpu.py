@@ -125,6 +125,20 @@ def test_kernel_selection_by_shape(lib):
     assert lib.epi_fusion_workspace_bytes(ctypes.byref(p)) == 2 * m + 256 + 1024 * 2 + 256
 
 
+def test_plan_sizes_match_golden(lib):
+    """Forward workspace, cache and backward workspace bytes over a sweep of every variant, dtype, epilogue, cache, n_src and
+    layout on shapes on both sides of each kernel's limits, plus invalid params, equal the table recorded by
+    oracle/make_golden_plan.py.  A planning change that moves a region shows up here."""
+    import numpy as np
+    from oracle import make_golden_plan as g
+    want = np.load(g.GOLDEN)["sizes"]
+    got = g.sizes(lib)
+    assert got.shape == want.shape
+    bad = np.flatnonzero((got != want).any(axis=1))
+    cases = g.rows() + list(g.INVALID)
+    assert bad.size == 0, "%d rows differ, first: %s got %s want %s" % (bad.size, cases[bad[0]], got[bad[0]], want[bad[0]])
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     monkeypatch.setattr(_lib, "_lib", None)
     monkeypatch.setattr(_lib, "LIB_PATH", str(tmp_path / "nope.so"))
