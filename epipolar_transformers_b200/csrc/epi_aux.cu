@@ -44,68 +44,17 @@ cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float 
 
 // ------------------------------------------------------------------------------------------
 // [N,C,H,W] (any strides, element type T) -> two bf16 planes [N,H,W,C] with src ≈ hi + lo (operands of the
-// tensor-core kernel; |src - hi - lo| <~ 2^-17 |src|, exact for bf16 and fp16 inputs).
+// tensor-core kernel).  Lo planes are written for bf16 maps too: the tile kernel reads them.
 // ------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) split_planes_kernel(const T *__restrict__ src, int64_t sn, int64_t sc, int64_t sh,
                                                            int64_t sw, __nv_bfloat16 *__restrict__ hi,
                                                            __nv_bfloat16 *__restrict__ lo, int C, int H, int W, int *zero_me) {
-    // tile: 64 channels x 64 pixels.  NCHW sources are read as float4 (a warp covers two 256-byte runs, which also
-    // keeps NVLink requests large when `src` is a peer-mapped map of another GPU); planes are written as 16-byte
-    // chunks of 8 channels.
     __shared__ float tile[64][65];
     if (zero_me && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0) *zero_me = 0;   // tile scheduler counter
-    const int HW = H * W;
-    const int n = blockIdx.z, c0 = blockIdx.y * 64, p0 = blockIdx.x * 64;
-    const int t = threadIdx.x;
+    const int n = blockIdx.z;
     const T *s = src + (int64_t)n * sn;
-    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(s) & (4 * sizeof(T) - 1)) == 0);
-    if (sc != 1) {
-        const int q = t & 15, cy = t >> 4;                      // 16 float4 per channel row, 16 channels per pass
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int c = c0 + cy + i * 16, p = p0 + q * 4;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c < C) {
-                if (vec && p + 3 < HW) v = ld4_nc(s + c * sc + p);
-                else {
-                    float e[4] = {0.f, 0.f, 0.f, 0.f};
-                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = to_f32(__ldg(s + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw));
-                    v = make_float4(e[0], e[1], e[2], e[3]);
-                }
-            }
-            float *row = &tile[cy + i * 16][q * 4];
-            row[0] = v.x; row[1] = v.y; row[2] = v.z; row[3] = v.w;
-        }
-    } else {
-        const int cx = t & 63, py = t >> 6;                     // channels-last: a warp reads 32 consecutive channels
-#pragma unroll
-        for (int i = 0; i < 16; i++) {
-            const int p = p0 + py + i * 4, c = c0 + cx;
-            tile[cx][py + i * 4] = (c < C && p < HW) ? to_f32(__ldg(s + c + (p / W) * sh + (p % W) * sw)) : 0.f;
-        }
-    }
-    __syncthreads();
-    const int cg = t & 7, pl = t >> 3;                          // 8 channel groups x 32 pixels per pass
-#pragma unroll
-    for (int i = 0; i < 2; i++) {
-        const int pp = pl + i * 32, p = p0 + pp, c = c0 + cg * 8;
-        if (p < HW && c < C) {                                  // C % 8 == 0 on this path
-            uint32_t h[4], l[4];
-#pragma unroll
-            for (int u = 0; u < 4; u++) {
-                const float f0 = tile[cg * 8 + 2 * u][pp], f1 = tile[cg * 8 + 2 * u + 1][pp];
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
-                const float2 hf = __bfloat1622float2(hv);
-                const __nv_bfloat162 lv = __floats2bfloat162_rn(f0 - hf.x, f1 - hf.y);
-                h[u] = *reinterpret_cast<const uint32_t *>(&hv);
-                l[u] = *reinterpret_cast<const uint32_t *>(&lv);
-            }
-            const size_t o = ((size_t)n * HW + p) * C + c;
-            *reinterpret_cast<uint4 *>(hi + o) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4 *>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
-        }
-    }
+    stage_planes_tile<T, true>(tile, s, sc, sh, sw, nchw_vec4(s, sc, sh, sw, W, H * W), hi, lo, n, blockIdx.y * 64, blockIdx.x * 64, C, H, W);
 }
 
 cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,

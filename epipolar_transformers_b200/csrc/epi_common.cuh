@@ -69,6 +69,85 @@ __device__ __forceinline__ float ld_feat(const void *p, int64_t i, int dtype) {
 }
 __host__ __device__ __forceinline__ int feat_esize(int dtype) { return dtype == kF32 ? 4 : 2; }
 
+// The bf16 (hi, lo) operand format of the tensor-core kernels: x ≈ hi + lo with hi = bf16(x), lo = bf16(x - hi)
+// (|x - hi - lo| <~ 2^-17 |x|, exact for bf16 and fp16 values).  Every operand plane is split here, so all of them round alike.
+// Two floats -> one bf16x2 word of hi parts and one of lo parts (a in the low 16 bits).
+__device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t &hi, uint32_t &lo) {
+    const __nv_bfloat162 hv = __floats2bfloat162_rn(a, b);
+    const float2 hf = __bfloat1622float2(hv);
+    const __nv_bfloat162 lv = __floats2bfloat162_rn(a - hf.x, b - hf.y);
+    hi = *reinterpret_cast<const uint32_t *>(&hv);
+    lo = *reinterpret_cast<const uint32_t *>(&lv);
+}
+// 8 floats -> one 16-byte chunk of hi parts and one of lo parts
+__device__ __forceinline__ void split8(const float *f, uint4 &hi, uint4 &lo) {
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) split_bf16x2(f[2 * u], f[2 * u + 1], h[u], l[u]);
+    hi = make_uint4(h[0], h[1], h[2], h[3]);
+    lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
+// an [N,C,H,W] item at s can be read as 4-element vectors along pixels (pixel-contiguous rows, 4-element aligned)
+template <typename T>
+__device__ __forceinline__ bool nchw_vec4(const T *s, int64_t sc, int64_t sh, int64_t sw, int W, int HW) {
+    return (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(s) & (4 * sizeof(T) - 1)) == 0);
+}
+
+// One tile of 64 channels x 64 pixels (from c0, p0) of item n of an [N,C,H,W] map -> pixel-major bf16 (hi, lo) planes
+// [N,H*W,C]; LO = false writes the hi plane only (bf16 maps, whose lo part is zero).  s: the item (any strides, element type
+// T); vec: nchw_vec4 of it; tile: [64][65] fp32 in shared memory; 256 threads; C % 8 == 0.  NCHW items are read as 4-pixel
+// vectors where vec allows (a warp covers two 256-byte runs, which also keeps NVLink requests large when the map is a
+// peer-mapped tensor of another GPU), channels-last ones along channels; the planes are written as 16-byte chunks of 8 channels.
+template <typename T, bool LO>
+__device__ __forceinline__ void stage_planes_tile(float (*tile)[65], const T *s, int64_t sc, int64_t sh, int64_t sw, bool vec,
+                                                  __nv_bfloat16 *hi, __nv_bfloat16 *lo, int n, int c0, int p0, int C, int H, int W) {
+    const int HW = H * W, t = threadIdx.x;
+    if (sc != 1) {
+        const int q = t % 16, cy = t / 16;                      // 16 float4 per channel row, 16 channels per pass
+        float4 v[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int c = c0 + cy + i * 16, p = p0 + q * 4;
+            v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (c < C) {
+                if (vec && p + 3 < HW) v[i] = ld4_nc(s + c * sc + p);
+                else {
+                    float e[4] = {0.f, 0.f, 0.f, 0.f};
+                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = to_f32(__ldg(s + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw));
+                    v[i] = make_float4(e[0], e[1], e[2], e[3]);
+                }
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            float *row = &tile[cy + i * 16][q * 4];
+            row[0] = v[i].x; row[1] = v[i].y; row[2] = v[i].z; row[3] = v[i].w;
+        }
+    } else {
+        const int cx = t % 64, py = t / 64;                     // channels-last: a warp reads 32 consecutive channels of one pixel
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            const int p = p0 + py + i * 4, c = c0 + cx;
+            tile[cx][py + i * 4] = (c < C && p < HW) ? to_f32(__ldg(s + c + (p / W) * sh + (p % W) * sw)) : 0.f;
+        }
+    }
+    __syncthreads();
+    const int cg = t % 8, pl = t / 8;                           // 8 channel groups x 32 pixels per pass
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int pp = pl + i * 32, p = p0 + pp, c = c0 + cg * 8;
+        if (p < HW && c < C) {
+            uint32_t h[4], l[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) split_bf16x2(tile[cg * 8 + 2 * u][pp], tile[cg * 8 + 2 * u + 1][pp], h[u], l[u]);
+            const size_t o = ((size_t)n * HW + p) * C + c;
+            *reinterpret_cast<uint4 *>(hi + o) = make_uint4(h[0], h[1], h[2], h[3]);
+            if (LO) *reinterpret_cast<uint4 *>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
+        }
+    }
+}
+
 // Per-(ref,src)-pair constants: M = A2·A1^-1 (row-major 3x3) and the epipole e2/e2.z.
 struct PairGeom {
     float M[9];
@@ -90,23 +169,46 @@ __host__ __device__ __forceinline__ float pix2coord(int i, float ds, float r) {
     return ((float)i * ds + ds * 0.5f - 0.5f) * r;           // multiview.py:154-157, epipolar.py:35-38
 }
 
-// One thread: fp64 3x3 inverse + products (≈100 flops), so the per-pixel fp32 math starts
-// from correctly rounded constants (SURVEY fact 10: the reference's fp32 pinv path is noisy).
+// fp64 pieces of a camera P = [A | t] (row-major 3x4): one thread each, so the per-pixel fp32 math starts from correctly
+// rounded constants (SURVEY fact 10: the reference's fp32 pinv path is noisy).  Every pair constant and every epipole of a
+// pixel order is computed by these, with one operation order.
+// A and t in fp64
+__device__ __forceinline__ void cam_load(const float *P, double A[9], double t[3]) {
+    for (int r = 0; r < 3; r++) {
+        for (int q = 0; q < 3; q++) A[r * 3 + q] = (double)P[r * 4 + q];
+        t[r] = (double)P[r * 4 + 3];
+    }
+}
+// A^-1 (row-major) by cofactors
+__device__ __forceinline__ void cam_inverse(const double a[9], double ai[9]) {
+    const double c00 = a[4] * a[8] - a[5] * a[7], c01 = a[5] * a[6] - a[3] * a[8], c02 = a[3] * a[7] - a[4] * a[6];
+    const double id = 1.0 / (a[0] * c00 + a[1] * c01 + a[2] * c02);
+    ai[0] = c00 * id; ai[1] = (a[2] * a[7] - a[1] * a[8]) * id; ai[2] = (a[1] * a[5] - a[2] * a[4]) * id;
+    ai[3] = c01 * id; ai[4] = (a[0] * a[8] - a[2] * a[6]) * id; ai[5] = (a[2] * a[3] - a[0] * a[5]) * id;
+    ai[6] = c02 * id; ai[7] = (a[1] * a[6] - a[0] * a[7]) * id; ai[8] = (a[0] * a[4] - a[1] * a[3]) * id;
+}
+// camera centre -A^-1 t (multiview.py:16-21), ai = A^-1
+__device__ __forceinline__ void cam_centre(const double ai[9], const double t[3], double c[3]) {
+    for (int r = 0; r < 3; r++) c[r] = -(ai[r * 3] * t[0] + ai[r * 3 + 1] * t[1] + ai[r * 3 + 2] * t[2]);
+}
+// row r of the homogeneous projection [A | t]·[x; 1]
+__device__ __forceinline__ double cam_project(const double A[9], const double t[3], const double x[3], int r) {
+    return A[r * 3] * x[0] + A[r * 3 + 1] * x[1] + A[r * 3 + 2] * x[2] + t[r];
+}
+
+// pair constants: M = A2·A1^-1 and the epipole P2·[C1; 1] of the reference camera in the source view
 __device__ inline void pair_geom_from_krt(const float *__restrict__ P1, const float *__restrict__ P2, PairGeom &g) {
-    double a[9], b[9], ai[9], t1[3], t2[3];
+    double a[9], b[9], ai[9], t1[3], t2[3], c[3], e[3];
+    // both cameras in one loop, not two cam_load calls: the same values, but loading one camera after the other
+    // reschedules (and re-spills) every kernel that inlines this, the staging kernel's hot streaming path included
     for (int r = 0; r < 3; r++) {
         for (int q = 0; q < 3; q++) { a[r * 3 + q] = (double)P1[r * 4 + q]; b[r * 3 + q] = (double)P2[r * 4 + q]; }
         t1[r] = (double)P1[r * 4 + 3]; t2[r] = (double)P2[r * 4 + 3];
     }
-    double c00 = a[4] * a[8] - a[5] * a[7], c01 = a[5] * a[6] - a[3] * a[8], c02 = a[3] * a[7] - a[4] * a[6];
-    double id = 1.0 / (a[0] * c00 + a[1] * c01 + a[2] * c02);
-    ai[0] = c00 * id; ai[1] = (a[2] * a[7] - a[1] * a[8]) * id; ai[2] = (a[1] * a[5] - a[2] * a[4]) * id;
-    ai[3] = c01 * id; ai[4] = (a[0] * a[8] - a[2] * a[6]) * id; ai[5] = (a[2] * a[3] - a[0] * a[5]) * id;
-    ai[6] = c02 * id; ai[7] = (a[1] * a[6] - a[0] * a[7]) * id; ai[8] = (a[0] * a[4] - a[1] * a[3]) * id;
-    double c[3], e[3];
-    for (int r = 0; r < 3; r++) c[r] = -(ai[r * 3] * t1[0] + ai[r * 3 + 1] * t1[1] + ai[r * 3 + 2] * t1[2]);   // camera centre
+    cam_inverse(a, ai);
+    cam_centre(ai, t1, c);
     for (int r = 0; r < 3; r++) {
-        e[r] = b[r * 3] * c[0] + b[r * 3 + 1] * c[1] + b[r * 3 + 2] * c[2] + t2[r];                          // epipole P2·[C;1]
+        e[r] = cam_project(b, t2, c, r);
         for (int q = 0; q < 3; q++)
             g.M[r * 3 + q] = (float)(b[r * 3] * ai[q] + b[r * 3 + 1] * ai[3 + q] + b[r * 3 + 2] * ai[6 + q]);
     }
@@ -193,6 +295,11 @@ __device__ __forceinline__ Taps make_taps(float gx, float gy, int H, int W, int 
     t.any = (xin0 || xin1) && (yin0 || yin1);
     return t;
 }
+
+// arg-max over the samples (DESIGN a6): the first maximum wins, like torch.argmax, so a candidate (v, k) replaces the best
+// (bv, bk) so far when it is larger, or equal at a lower sample index.  Every merge of partial arg-maxes uses this rule.
+// (A macro: as a function returning bool it leaves the kernels' branch structure, and so their machine code, different.)
+#define EPI_FIRST_MAX_BEATS(v, k, bv, bk) ((v) > (bv) || ((v) == (bv) && (k) < (bk)))
 
 
 // Programmatic dependent launch (the three launches of a forward are chained with

@@ -108,22 +108,6 @@ __device__ __forceinline__ void wait_n(uint64_t *bar, uint32_t n) {
         if (it > (1u << 24)) __trap();
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo_elem, hi_elem);
-    return *reinterpret_cast<uint32_t *>(&v);
-}
-__device__ __forceinline__ void split8(const float *f, uint4 &hi, uint4 &lo) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-        const __nv_bfloat162 hv = __floats2bfloat162_rn(f[2 * u], f[2 * u + 1]);
-        const float2 hf = __bfloat1622float2(hv);
-        h[u] = *reinterpret_cast<const uint32_t *>(&hv);
-        l[u] = pack_bf16x2(f[2 * u] - hf.x, f[2 * u + 1] - hf.y);
-    }
-    hi = make_uint4(h[0], h[1], h[2], h[3]);
-    lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
 }  // namespace pipe
 
 using namespace pipe;
@@ -276,12 +260,12 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                         if (c0 >= C) continue;
                         const float4 o = *reinterpret_cast<const float4 *>(table + i * 256 + ct0);
                         if (a.out_hi) {
-                            const __nv_bfloat162 h0 = __floats2bfloat162_rn(o.x, o.y), h1 = __floats2bfloat162_rn(o.z, o.w);
-                            const float2 f0 = __bfloat1622float2(h0), f1 = __bfloat1622float2(h1);
-                            const __nv_bfloat162 l0 = __floats2bfloat162_rn(o.x - f0.x, o.y - f0.y), l1 = __floats2bfloat162_rn(o.z - f1.x, o.w - f1.y);
+                            uint2 h2, l2;
+                            split_bf16x2(o.x, o.y, h2.x, l2.x);
+                            split_bf16x2(o.z, o.w, h2.y, l2.y);
                             const size_t off = ((size_t)d.n * HW + y * W + x) * C + c0;
-                            *reinterpret_cast<uint2 *>(a.out_hi + off) = make_uint2(*reinterpret_cast<const uint32_t *>(&h0), *reinterpret_cast<const uint32_t *>(&h1));
-                            *reinterpret_cast<uint2 *>(a.out_lo + off) = make_uint2(*reinterpret_cast<const uint32_t *>(&l0), *reinterpret_cast<const uint32_t *>(&l1));
+                            *reinterpret_cast<uint2 *>(a.out_hi + off) = h2;
+                            *reinterpret_cast<uint2 *>(a.out_lo + off) = l2;
                         } else if (a.out_stride[1] == 1 && !a.add_ref) {
                             // channel-contiguous output (channels_last, or the library's pixel-major plane): one 16-byte store per lane
                             *reinterpret_cast<float4 *>(a.out + (int64_t)d.n * a.out_stride[0] + (int64_t)y * a.out_stride[2] + (int64_t)x * a.out_stride[3] + c0) = o;
@@ -508,7 +492,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
 #pragma unroll
                 for (int w = 0; w < NWORK; w++) {
                     const float v = red_bv[w * 32 + lane]; const int kk = red_bk[w * 32 + lane];
-                    if (v > bv || (v == bv && kk < bk)) { bv = v; bk = kk; }
+                    if (EPI_FIRST_MAX_BEATS(v, kk, bv, bk)) { bv = v; bk = kk; }
                 }
                 float gx, gy;
                 if (a.locs_in) {
@@ -963,7 +947,6 @@ cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st) {
     const bool lo = a.src_lo != nullptr;
     void (*kern)(const FusionArgs) = lo ? (kpl <= 1 ? epi_fusion_pipe_kernel<1, true> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, true> : epi_fusion_pipe_kernel<4, true>))
                                         : (kpl <= 1 ? epi_fusion_pipe_kernel<1, false> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, false> : epi_fusion_pipe_kernel<4, false>));
-    static thread_local int sms_cached = 0;
     static thread_local bool attr_set[6] = {false, false, false, false, false, false};
     const int ki = (kpl <= 1 ? 0 : (kpl <= 2 ? 1 : 2)) + (lo ? 0 : 3);
     if (!attr_set[ki]) {
@@ -971,13 +954,8 @@ cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st) {
         if (e != cudaSuccess) return e;
         attr_set[ki] = true;
     }
-    if (!sms_cached) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev);
-        if (sms_cached <= 0) sms_cached = 132;
-    }
-    const int grid = tiles < sms_cached ? tiles : sms_cached;      // one persistent CTA per SM
+    const int sms = sm_count();
+    const int grid = tiles < sms ? tiles : sms;                    // one persistent CTA per SM
     cudaError_t le = launch_pdl(kern, dim3((unsigned)grid), dim3(NT_ALL), (size_t)SMEM_ALLOC, st, a);
     if (le != cudaSuccess) return le;
     return cudaGetLastError();

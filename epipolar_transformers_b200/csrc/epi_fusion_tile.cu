@@ -60,23 +60,6 @@ struct Misc {
 };
 static_assert(sizeof(Misc) <= 512, "Misc too large");
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
-    __nv_bfloat162 v = __floats2bfloat162_rn(lo_elem, hi_elem);     // .x = lo_elem (low 16 bits)
-    return *reinterpret_cast<uint32_t *>(&v);
-}
-// 8 floats -> one 16-byte chunk of bf16 hi parts and one of lo parts
-__device__ __forceinline__ void split8(const float *f, uint4 &hi, uint4 &lo) {
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) {
-        const __nv_bfloat162 hv = __floats2bfloat162_rn(f[2 * u], f[2 * u + 1]);
-        const float2 hf = __bfloat1622float2(hv);
-        h[u] = *reinterpret_cast<const uint32_t *>(&hv);
-        l[u] = pack_bf16x2(f[2 * u] - hf.x, f[2 * u + 1] - hf.y);
-    }
-    hi = make_uint4(h[0], h[1], h[2], h[3]);
-    lo = make_uint4(l[0], l[1], l[2], l[3]);
-}
 }  // namespace tile
 
 using namespace tile;
@@ -441,7 +424,7 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
                         const float ov = __shfl_xor_sync(0xffffffffu, best_v, o);
                         const int ok = __shfl_xor_sync(0xffffffffu, best_k, o);
                         const float ogx = __shfl_xor_sync(0xffffffffu, best_gx, o), ogy = __shfl_xor_sync(0xffffffffu, best_gy, o);
-                        if (ov > best_v || (ov == best_v && ok < best_k)) { best_v = ov; best_k = ok; best_gx = ogx; best_gy = ogy; }
+                        if (EPI_FIRST_MAX_BEATS(ov, ok, best_v, best_k)) { best_v = ov; best_k = ok; best_gx = ogx; best_gy = ogy; }
                     }
                     if (lane == 0)
                         reinterpret_cast<float2 *>(a.corr_pos)[(size_t)n * HW + pix_y(i) * W + pix_x(i)] =
@@ -609,9 +592,7 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
     else        kern = kpl <= 1 ? epi_fusion_tile_kernel<1, false> : (kpl <= 2 ? epi_fusion_tile_kernel<2, false> : epi_fusion_tile_kernel<4, false>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_ALLOC);
     if (e != cudaSuccess) return e;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
     const int grid = a.tile_counter ? (tiles < sms ? tiles : sms) : tiles;     // one persistent CTA per SM
     kern<<<grid, NT, SMEM_ALLOC, st>>>(a);
     return cudaGetLastError();
@@ -632,17 +613,12 @@ __global__ void __launch_bounds__(1024) sector_order_kernel(const float *__restr
     while (npad < HW) npad <<= 1;
     if (threadIdx.x == 0) {
         const float *P1 = P_ref + 12 * (n % n_ref), *P2 = P_src + 12 * n;
-        double b[9], t2[3];
-        for (int r = 0; r < 3; r++) { for (int q = 0; q < 3; q++) b[r * 3 + q] = (double)P2[r * 4 + q]; t2[r] = (double)P2[r * 4 + 3]; }
-        const double c00 = b[4] * b[8] - b[5] * b[7], c01 = b[5] * b[6] - b[3] * b[8], c02 = b[3] * b[7] - b[4] * b[6];
-        const double id = 1.0 / (b[0] * c00 + b[1] * c01 + b[2] * c02);
-        double bi[9];
-        bi[0] = c00 * id; bi[1] = (b[2] * b[7] - b[1] * b[8]) * id; bi[2] = (b[1] * b[5] - b[2] * b[4]) * id;
-        bi[3] = c01 * id; bi[4] = (b[0] * b[8] - b[2] * b[6]) * id; bi[5] = (b[2] * b[3] - b[0] * b[5]) * id;
-        bi[6] = c02 * id; bi[7] = (b[1] * b[6] - b[0] * b[7]) * id; bi[8] = (b[0] * b[4] - b[1] * b[3]) * id;
-        double cs[3], e[3];
-        for (int r = 0; r < 3; r++) cs[r] = -(bi[r * 3] * t2[0] + bi[r * 3 + 1] * t2[1] + bi[r * 3 + 2] * t2[2]);      // source camera centre
-        for (int r = 0; r < 3; r++) e[r] = (double)P1[r * 4] * cs[0] + (double)P1[r * 4 + 1] * cs[1] + (double)P1[r * 4 + 2] * cs[2] + (double)P1[r * 4 + 3];
+        double a[9], t1[3], b[9], t2[3], bi[9], cs[3], e[3];
+        cam_load(P2, b, t2);
+        cam_inverse(b, bi);
+        cam_centre(bi, t2, cs);                     // source camera centre
+        cam_load(P1, a, t1);
+        for (int r = 0; r < 3; r++) e[r] = cam_project(a, t1, cs, r);
         const double cx = 0.5 * ((double)gc.xmin + gc.xmax), cy = 0.5 * ((double)gc.ymin + gc.ymax);
         const double nrm = fabs(e[0]) + fabs(e[1]) + 1e-300;
         if (!(fabs(e[2]) > 1e-9 * nrm)) {        // epipole at infinity (or NaN): lines are parallel to (e0, e1): sort by the offset across them

@@ -186,11 +186,11 @@ epi_fusion_warp_kernel(const FusionArgs a) {
         }
         if (a.corr_pos) {
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {                               // first max wins (torch.argmax on CPU)
+            for (int o = 16; o > 0; o >>= 1) {
                 float ov = __shfl_xor_sync(0xffffffffu, best_v, o);
                 int ok = __shfl_xor_sync(0xffffffffu, best_k, o);
                 float ogx = __shfl_xor_sync(0xffffffffu, best_gx, o), ogy = __shfl_xor_sync(0xffffffffu, best_gy, o);
-                if (ov > best_v || (ov == best_v && ok < best_k)) { best_v = ov; best_k = ok; best_gx = ogx; best_gy = ogy; }
+                if (EPI_FIRST_MAX_BEATS(ov, ok, best_v, best_k)) { best_v = ov; best_k = ok; best_gx = ogx; best_gy = ogy; }
             }
             if (lane == 0)
                 reinterpret_cast<float2 *>(a.corr_pos)[(size_t)n * HW + p] =

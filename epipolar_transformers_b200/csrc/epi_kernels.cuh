@@ -6,6 +6,17 @@
 
 namespace epi {
 
+// SMs of the current device, for persistent grids: queried once per host thread, 132 (an H100 SXM) if the query fails
+inline int sm_count() {
+    static thread_local int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    }
+    return sms;
+}
+
 // Device-side view of one fused forward (built from EpiFusionParams by the ABI layer).
 struct FusionArgs {
     const float *feat_ref;  int64_t ref_stride[4];   // fp32 (the caller's map, or a fp32 copy of a low-precision one) ...

@@ -25,7 +25,7 @@ namespace stg {
 constexpr int NT = 256;
 constexpr int NBIN = 4096;
 constexpr int SMALL = 32;
-constexpr int TC = 64, TPX = 64, TPITCH = 65;       // layout-staging tile: 64 channels x 64 pixels
+constexpr int TC = 64, TPX = 64, TPITCH = 65;       // layout-staging tile: 64 channels x 64 pixels (stage_planes_tile's)
 
 // Monotone pseudo-angle of (u, v) in [-2, 2] (diamond angle): same ordering as atan2(v, u) at the price of one division.
 __device__ __forceinline__ float pseudo_angle(float u, float v) {
@@ -135,17 +135,12 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
             pair_geom_from_krt(P1, P2, g);
             s.pair_geom[n] = g;
             // epipole of the SOURCE camera in the reference view: e1 = P_ref·[C_src; 1]
-            double b[9], t2[3];
-            for (int r = 0; r < 3; r++) { for (int q = 0; q < 3; q++) b[r * 3 + q] = (double)P2[r * 4 + q]; t2[r] = (double)P2[r * 4 + 3]; }
-            const double c00 = b[4] * b[8] - b[5] * b[7], c01 = b[5] * b[6] - b[3] * b[8], c02 = b[3] * b[7] - b[4] * b[6];
-            const double id = 1.0 / (b[0] * c00 + b[1] * c01 + b[2] * c02);
-            double bi[9];
-            bi[0] = c00 * id; bi[1] = (b[2] * b[7] - b[1] * b[8]) * id; bi[2] = (b[1] * b[5] - b[2] * b[4]) * id;
-            bi[3] = c01 * id; bi[4] = (b[0] * b[8] - b[2] * b[6]) * id; bi[5] = (b[2] * b[3] - b[0] * b[5]) * id;
-            bi[6] = c02 * id; bi[7] = (b[1] * b[6] - b[0] * b[7]) * id; bi[8] = (b[0] * b[4] - b[1] * b[3]) * id;
-            double cs[3], e[3];
-            for (int r = 0; r < 3; r++) cs[r] = -(bi[r * 3] * t2[0] + bi[r * 3 + 1] * t2[1] + bi[r * 3 + 2] * t2[2]);
-            for (int r = 0; r < 3; r++) e[r] = (double)P1[r * 4] * cs[0] + (double)P1[r * 4 + 1] * cs[1] + (double)P1[r * 4 + 2] * cs[2] + (double)P1[r * 4 + 3];
+            double a[9], t1[3], b[9], t2[3], bi[9], cs[3], e[3];
+            cam_load(P2, b, t2);
+            cam_inverse(b, bi);
+            cam_centre(bi, t2, cs);
+            cam_load(P1, a, t1);
+            for (int r = 0; r < 3; r++) e[r] = cam_project(a, t1, cs, r);
             const double cx = 0.5 * ((double)s.gc.xmin + s.gc.xmax), cy = 0.5 * ((double)s.gc.ymin + s.gc.ymax);
             const double nrm = fabs(e[0]) + fabs(e[1]) + 1e-300;
             // range of the key over the image: the four corners bound it unless the epipole lies inside the image
@@ -307,17 +302,10 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
                 const int o = (int)(e0 / C), c_first = (int)(e0 % C);
                 if (o >= c_first && o < c_first + 8) f[o - c_first] += 1.f;
             }
-            uint32_t h[4], l[4];
-#pragma unroll
-            for (int u = 0; u < 4; u++) {
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(f[2 * u], f[2 * u + 1]);
-                const float2 hf = __bfloat1622float2(hv);
-                const __nv_bfloat162 lv = __floats2bfloat162_rn(f[2 * u] - hf.x, f[2 * u + 1] - hf.y);
-                h[u] = *reinterpret_cast<const uint32_t *>(&hv);
-                l[u] = *reinterpret_cast<const uint32_t *>(&lv);
-            }
-            *reinterpret_cast<uint4 *>(s.w_planes + e0) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4 *>(s.w_planes + tot + e0) = make_uint4(l[0], l[1], l[2], l[3]);
+            uint4 h4, l4;
+            split8(f, h4, l4);
+            *reinterpret_cast<uint4 *>(s.w_planes + e0) = h4;
+            *reinterpret_cast<uint4 *>(s.w_planes + tot + e0) = l4;
         }
         return;
     }
@@ -346,14 +334,12 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
             const int cpair = fw + 8 * i, g = cpair >> 2, k = cpair & 3;
 #pragma unroll
             for (int u = 0; u < 2; u++) {
-                const float fe = u ? e1 : e0, fo = u ? o1 : o0;
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(fe, fo);
-                const float2 hf = __bfloat1622float2(hv);
-                const __nv_bfloat162 lv = __floats2bfloat162_rn(fe - hf.x, fo - hf.y);
+                uint32_t hw, lw;
+                split_bf16x2(u ? e1 : e0, u ? o1 : o0, hw, lw);
                 const int px = 4 * fq + 2 * hsel + u, sw5 = (px >> 1) & 31;
                 const int pos = px * 32 + (((g ^ (sw5 >> 2)) << 2) | (k ^ (sw5 & 3)));
-                whi[pos] = *reinterpret_cast<const uint32_t *>(&hv);
-                if (LO) wlo[pos] = *reinterpret_cast<const uint32_t *>(&lv);
+                whi[pos] = hw;
+                if (LO) wlo[pos] = lw;
             }
         }
     };
@@ -427,7 +413,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     const int64_t sn = strd[0], sc = strd[1], sh = strd[2], sw = strd[3];
     const T *sp = base + (int64_t)n * sn;
     __nv_bfloat16 *hi = plane_hi(map), *lo = hi + plane_elems(map);
-    const bool vec = (sw == 1) && (sh == W) && (HW % 4 == 0) && (sc % 4 == 0) && ((reinterpret_cast<uintptr_t>(sp) & (4 * sizeof(T) - 1)) == 0);
+    const bool vec = nchw_vec4(sp, sc, sh, sw, W, HW);
     if (vec && sc != 1 && p0 + TPX <= HW && c0 + TC <= C) {
         float4 v[RPASS];
         fast_load(sp, sc, c0, p0, v);
@@ -436,58 +422,8 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
         fast_store(hi, lo, n, c0, p0);
         return;
     }
-    if (sc != 1) {
-        const int q = t % QW, cy = t / QW;
-        float4 v[RPASS];
-#pragma unroll
-        for (int i = 0; i < RPASS; i++) {
-            const int c = c0 + cy + i * RPP, p = p0 + q * 4;
-            v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c < C) {
-                if (vec && p + 3 < HW) v[i] = ld4_nc(sp + c * sc + p);
-                else {
-                    float e[4] = {0.f, 0.f, 0.f, 0.f};
-                    for (int j = 0; j < 4; j++) if (p + j < HW) e[j] = to_f32(__ldg(sp + c * sc + ((p + j) / W) * sh + ((p + j) % W) * sw));
-                    v[i] = make_float4(e[0], e[1], e[2], e[3]);
-                }
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < RPASS; i++) {
-            float *row = &tile[cy + i * RPP][q * 4];
-            row[0] = v[i].x; row[1] = v[i].y; row[2] = v[i].z; row[3] = v[i].w;
-        }
-    } else {
-        const int cx = t % TC, py = t / TC;                     // channels-last: a warp reads 32 consecutive channels of one pixel
-        constexpr int PPP = NT / TC;
-#pragma unroll
-        for (int i = 0; i < TPX / PPP; i++) {
-            const int p = p0 + py + i * PPP, c = c0 + cx;
-            tile[cx][py + i * PPP] = (c < C && p < HW) ? to_f32(__ldg(sp + c + (p / W) * sh + (p % W) * sw)) : 0.f;
-        }
-    }
-    __syncthreads();
-    constexpr int CG = TC / 8, PXP = NT / CG;                    // groups of 8 channels (16 bytes per plane), pixels per pass
-    const int cg = t % CG, pl = t / CG;
-#pragma unroll
-    for (int i = 0; i < TPX / PXP; i++) {
-        const int pp = pl + i * PXP, p = p0 + pp, c = c0 + cg * 8;
-        if (p < HW && c < C) {                                  // C % 8 == 0 on this path
-            uint32_t h[4], l[4];
-#pragma unroll
-            for (int u = 0; u < 4; u++) {
-                const float f0 = tile[cg * 8 + 2 * u][pp], f1 = tile[cg * 8 + 2 * u + 1][pp];
-                const __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
-                const float2 hf = __bfloat1622float2(hv);
-                const __nv_bfloat162 lv = __floats2bfloat162_rn(f0 - hf.x, f1 - hf.y);
-                h[u] = *reinterpret_cast<const uint32_t *>(&hv);
-                l[u] = *reinterpret_cast<const uint32_t *>(&lv);
-            }
-            const size_t o = ((size_t)n * HW + p) * C + c;
-            *reinterpret_cast<uint4 *>(hi + o) = make_uint4(h[0], h[1], h[2], h[3]);
-            if (LO) *reinterpret_cast<uint4 *>(lo + o) = make_uint4(l[0], l[1], l[2], l[3]);
-        }
-    }
+    static_assert(NT == 256 && TC == 64 && TPX == 64 && TPITCH == 65, "stage_planes_tile's block and tile");
+    stage_planes_tile<T, LO>(tile, sp, sc, sh, sw, vec, hi, lo, n, c0, p0, C, H, W);
 }
 
 template <typename T>
@@ -538,15 +474,9 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     auto whole = [&](const T *b, const int64_t *sd) {
         return sd[3] == 1 && sd[2] == W && sd[1] % 4 == 0 && sd[0] % 4 == 0 && sd[1] != 1 && (reinterpret_cast<uintptr_t>(b) & (4 * sizeof(T) - 1)) == 0;
     };
-    static thread_local int sms_cached = 0;
-    if (!sms_cached) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms_cached, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms_cached <= 0) sms_cached = 132;
-    }
     s.persist = 0;
     if ((H * W) % stg::TPX == 0 && C % stg::TC == 0 && whole(ref, ref_stride) && whole(src, src_stride)) {
-        const int slots = 5 * sms_cached;                      // 5 resident blocks per SM (__launch_bounds__)
+        const int slots = 5 * sm_count();                      // 5 resident blocks per SM (__launch_bounds__)
         s.persist = tiles < slots ? tiles : slots;
     }
     const int grid = (s.do_order ? N : 0) + wblocks + (s.persist ? s.persist : tiles);
