@@ -10,7 +10,7 @@ import epipolar_transformers_b200 as epi
 from epipolar_transformers_b200 import synthetic as syn
 from epipolar_transformers_b200.epipolar import _FusionFn, epipolar_fusion_backward
 from oracle import golden_cases as gc
-from tests.util import rel_max
+from tests.util import edge_locs, rel_max
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4
@@ -183,30 +183,6 @@ def test_backward_envelope_vs_autograd_fp64(case, other_grad):
     assert rel_max(out.detach().cpu().numpy(), ro.cpu().numpy()) < TOL
     assert rel_max(g1.cpu().numpy(), e1.cpu().numpy()) < TOL
     assert rel_max(g2.cpu().numpy(), e2.cpu().numpy()) < TOL
-
-
-def edge_locs(K, N, H, W, seed):
-    """[K,N,H,W,2] hand-built sample locations: random points in the map mixed with exact pixel centres (three zero-weight
-    taps), points on the border, just beyond it and a pixel or more beyond it, and far-off points; pixel column 3 has only
-    far-off samples.  Every value that is not random is a short dyadic fraction, so fp32 and fp64 find the same taps and
-    the same zero weights (a tap weight of 1e-7 on one side only would flip the sim == 0 mask)."""
-    rng = np.random.default_rng(seed)
-    g = rng.uniform(-1, 1, size=(K, N, H, W, 2))
-    kind = rng.integers(0, 4, size=(K, N, H, W))                 # 0 random, 1 pixel centre, 2 border, 3 far
-    border = np.array([-1, 1, -1 + 1 / 64, 1 - 1 / 64, -1 - 1 / 32, 1 + 1 / 32, -1 - 1 / 16, 1 + 1 / 16, -1.25, 1.25])
-    border_axis = rng.integers(0, 2, size=kind.shape)
-    for axis, size in ((0, W), (1, H)):
-        centres = np.array([(2 * i + 1) / size - 1 for i in range(size) if (2 * i + 1) * 4 % size == 0])   # multiples of 1/4
-        assert centres.size
-        on = kind == 1
-        g[..., axis][on] = rng.choice(centres, size=on.sum())
-        on = (kind == 2) & (border_axis == axis)
-        g[..., axis][on] = rng.choice(border, size=on.sum())
-    far = np.array([(-312.5, -312.5), (1e4, 0.25), (0.5, -700.0), (40.0, 40.0)])
-    on = kind == 3
-    g[on] = far[rng.integers(0, len(far), size=on.sum())]
-    g[:, :, :, 3] = far[rng.integers(0, len(far), size=(K, N, H))]
-    return g.astype(np.float32)
 
 
 LAYOUT_SHAPES = [pytest.param((2, 64, 12, 20, 48), id="vec4_c64_k48"), pytest.param((2, 17, 12, 20, 40), id="vec1_c17_k40")]
