@@ -11,6 +11,7 @@ namespace {
 thread_local char g_err[512] = "";
 thread_local int g_launches = 0;
 thread_local int g_timing = 0, g_timing_valid = 0;
+thread_local int g_items32 = 0;          // epi_pipe_force_items32: test and A/B-timing hook, not part of the public API
 thread_local cudaEvent_t g_ev0 = nullptr, g_ev1 = nullptr, g_evA = nullptr, g_evB = nullptr;   // A: call start, B: call end
 
 int fail(int code, const char *fmt, const char *detail = "") {
@@ -74,6 +75,7 @@ struct Plan {
     size_t order = NONE, geom = NONE;    // pixel order and pair constants: in the cache when `cached`, else in the workspace
     size_t key = NONE, records = NONE, cache_bytes = 0;     // cache: per pair a key of 32 words (word 31: epoch of its work records)
     int n_records = 0;
+    int item_px = 32;                    // pipe kernel: reference pixels per work item
 };
 
 bool want_pipe(const EpiFusionParams *p) {
@@ -118,6 +120,7 @@ Plan make_plan(const EpiFusionParams *p) {
         pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32) : (out_direct ? Epilogue::Direct : Epilogue::Unstage);
         if (lowp && pl.epilogue == Epilogue::ZFp32 && p->add_ref_residual) pl.ref_copy = RefCopy::After;   // the fp32 z epilogue's residual
         pl.cached = p->cache != nullptr;
+        pl.item_px = g_items32 ? 32 : epi::fusion_pipe_item_pixels(p->C, p->H, p->W);
         // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes; bf16 maps have no lo part: [ref_hi | src_hi]
         const bool lo = p->feat_dtype != EPI_DTYPE_BF16;
         pl.ref_hi = ws.part(ref_map / 2);
@@ -235,6 +238,10 @@ int epi_last_launch_count(void) { return g_launches; }
 
 int epi_kernel_timing_enable(int on) { g_timing = on ? 1 : 0; return EPI_OK; }
 
+// Not declared in the public header: forces the pipe kernel's 32-pixel work items on every shape (on = 1) or restores the
+// planned item size (on = 0), so that tests and timings can compare the two on one shape in one process.
+int epi_pipe_force_items32(int on) { g_items32 = on ? 1 : 0; return EPI_OK; }
+
 int epi_kernel_timing_last3(float *ms3) {
     if (!ms3) return fail(EPI_EINVAL, "null pointer");
     ms3[0] = ms3[1] = ms3[2] = -1.f;
@@ -283,7 +290,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     a.feat_ref = static_cast<const float *>(p->feat_ref); a.ref_dtype = dt;
     a.P_ref = p->P_ref; a.P_src = p->P_src; a.locs_in = p->sample_locs_in;
     a.attn = p->attn; a.corr_pos = p->corr_pos; a.locs_out = p->sample_locs_out;
-    a.N = NP; a.n_ref = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale;
+    a.N = NP; a.n_ref = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale; a.item_px = pl.item_px;
     for (int i = 0; i < 4; i++) a.ref_stride[i] = p->ref_stride[i];
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
     float *ref32 = at<float>(ws, pl.ref32);

@@ -42,6 +42,7 @@ struct FusionArgs {
     int plan_records;                         // capacity of plan_cache in records of fusion_pipe_plan_record_bytes()
     const uint32_t *pair_epoch;               // [N] stride 32 words: epoch of each pair's cached plan (bumped by the staging kernel on a key miss)
     GeomCfg geom;
+    int item_px;                              // pipe kernel: reference pixels per work item, 32 or 64 (fusion_pipe_item_pixels)
 };
 
 // Backward of the fused attention (epi_fusion_bwd.cu)
@@ -90,6 +91,7 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st);
 cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st);
 bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 size_t fusion_pipe_plan_record_bytes();
+int fusion_pipe_item_pixels(int C, int H, int W);                  // 32 or 64
 int fusion_pipe_plan_records(int N, int n_ref, int H, int W);   // N pairs on n_ref reference items
 bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 // pair n: P_ref item n % n_ref, P_src item n
