@@ -20,7 +20,8 @@ VARIANTS = {"auto": EPI_VARIANT_AUTO, "warp": EPI_VARIANT_WARP, "tile": EPI_VARI
 EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_fusion_cache_bytes", "epi_fusion_forward_f32",
            "epi_fusion_backward_workspace_bytes", "epi_fusion_backward_f32", "epi_find_peaks_f32", "epi_find_peaks_best_f32",
            "epi_sample_locs_f32", "epi_fold_z_bn_f32", "epi_last_launch_count", "epi_umma_selftest",
-           "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3")
+           "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3",
+           "epi_fusion_backward_deterministic")
 
 _fp = ctypes.POINTER(ctypes.c_float)
 
@@ -60,7 +61,7 @@ class EpiFusionBwdParams(ctypes.Structure):
         ("downsample", ctypes.c_float), ("img_scale", ctypes.c_float), ("eps", ctypes.c_float), ("softmax_scale", ctypes.c_float),
         ("align_corners", ctypes.c_int32), ("correct_normalize", ctypes.c_int32),
         ("grad_keys", ctypes.c_int32), ("grad_vals", ctypes.c_int32), ("feat_dtype", ctypes.c_int32),
-        ("reserved", ctypes.c_int32 * 3),
+        ("deterministic", ctypes.c_int32), ("reserved", ctypes.c_int32 * 2),
     ]
 
 
@@ -79,7 +80,9 @@ def load():
     lib = ctypes.CDLL(LIB_PATH)
     missing = [s for s in EXPORTS if not hasattr(lib, s)]
     if missing:
-        raise RuntimeError("libepipolar_b200.so does not export %s" % missing)
+        # e.g. a library built before EpiFusionBwdParams.deterministic, which would ignore the field
+        raise RuntimeError("libepipolar_b200.so does not export %s; rebuild it with "
+                           "`python -m epipolar_transformers_b200.build --force`" % missing)
     lib.epi_version.restype = ctypes.c_int
     lib.epi_last_error.restype = ctypes.c_char_p
     lib.epi_last_launch_count.restype = ctypes.c_int
@@ -114,6 +117,7 @@ def load():
     lib.epi_kernel_timing_last_ms.restype = ctypes.c_float
     lib.epi_kernel_timing_last3.restype = ctypes.c_int
     lib.epi_kernel_timing_last3.argtypes = [ctypes.POINTER(ctypes.c_float)]
+    lib.epi_fusion_backward_deterministic.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))

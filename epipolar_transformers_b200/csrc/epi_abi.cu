@@ -195,12 +195,15 @@ int validate_bwd(const EpiFusionBwdParams *p) {
     if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2 || p->K < 2 || p->K > 256) return fail(EPI_EINVAL, "bad shape");
     if (p->C > 512 || (p->C > 128 && p->C % 4 != 0)) return fail(EPI_EINVAL, "backward supports C <= 128, or C <= 512 with C % 4 == 0");
     if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    if (p->deterministic != 0 && p->deterministic != 1) return fail(EPI_EINVAL, "deterministic must be 0 or 1");
     return EPI_OK;
 }
 
 // Backward workspace: pixel-major copy of feat_src + pixel-major accumulator of its gradient; low-precision maps: + a channels-last
-// fp32 copy of feat_ref and a pixel-major fp32 buffer of its gradient (rounded once to the maps' type by the transposition pass)
-struct BwdPlan { size_t map, src, dsrc, ref32 = NONE, gref32 = NONE, workspace_bytes; };
+// fp32 copy of feat_ref and a pixel-major fp32 buffer of its gradient (rounded once to the maps' type by the transposition pass);
+// deterministic: + the int64 fixed-point accumulator of dL/dfeat_src, one bound word per pair and the [N,K,H·W] float2
+// coefficients (accumulator and words adjacent, so that one memset zeroes both)
+struct BwdPlan { size_t map, src, dsrc, ref32 = NONE, gref32 = NONE, acc = NONE, words = NONE, coef = NONE, workspace_bytes; };
 
 BwdPlan make_bwd_plan(const EpiFusionBwdParams *p) {
     BwdPlan pl;
@@ -208,6 +211,12 @@ BwdPlan make_bwd_plan(const EpiFusionBwdParams *p) {
     pl.map = (size_t)p->N * p->C * p->H * p->W * sizeof(float);
     pl.src = ws.take(pl.map); pl.dsrc = ws.take(pl.map);
     if (p->feat_dtype != EPI_DTYPE_F32) { pl.ref32 = ws.take(pl.map); pl.gref32 = ws.take(pl.map); }
+    if (p->deterministic == 1) {
+        const size_t px = (size_t)p->N * p->H * p->W;
+        pl.acc = ws.take(2 * pl.map);
+        pl.words = ws.take((size_t)p->N * sizeof(uint32_t));
+        pl.coef = ws.take(px * p->K * sizeof(float2));
+    }
     pl.workspace_bytes = ws.end;
     return pl;
 }
@@ -235,6 +244,8 @@ int epi_version(void) { return EPI_ABI_VERSION; }
 const char *epi_last_error(void) { return g_err; }
 
 int epi_last_launch_count(void) { return g_launches; }
+
+int epi_fusion_backward_deterministic(void) { return 1; }
 
 int epi_kernel_timing_enable(int on) { g_timing = on ? 1 : 0; return EPI_OK; }
 
@@ -415,8 +426,10 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     Launches run;
     if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, p->N, p->C, p->H, p->W, dt, st)))) return rc;
     if (lowp && (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
+    const bool det = p->deterministic == 1 && p->grad_src;      // dL/dfeat_ref alone is the same launch on both paths
     if (p->grad_src) {
-        const cudaError_t e = cudaMemsetAsync(dsrc, 0, pl.map, st);
+        const cudaError_t e = det ? cudaMemsetAsync(at<char>(ws, pl.acc), 0, pl.words + p->N * sizeof(uint32_t) - pl.acc, st)
+                                  : cudaMemsetAsync(dsrc, 0, pl.map, st);
         if (e != cudaSuccess) return fail(EPI_ECUDA, "memset failed: %s", cudaGetErrorString(e));
     }
     epi::BwdArgs a;
@@ -431,7 +444,16 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     }
     a.N = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale; a.grad_keys = p->grad_keys; a.grad_vals = p->grad_vals;
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
-    if ((rc = run("backward kernel", epi::launch_fusion_bwd(a, st)))) return rc;
+    if (det) {
+        a.dsrc_nhwc = nullptr;
+        a.coef = at<float2>(ws, pl.coef); a.pair_max = at<unsigned>(ws, pl.words); a.acc = at<long long>(ws, pl.acc);
+        int kernels = 0;
+        const cudaError_t e = epi::launch_fusion_bwd_det(a, st, kernels);
+        if ((rc = run("deterministic backward kernels", e, kernels))) return rc;
+        if ((rc = run("fixed-point conversion", epi::launch_acc_to_f32(a.acc, a.pair_max, dsrc, p->N, p->H * p->W, p->C, st)))) return rc;
+    } else if ((rc = run("backward kernel", epi::launch_fusion_bwd(a, st)))) {
+        return rc;
+    }
     if (p->grad_src &&
         (rc = run("gradient transposition", epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride,
                                                                 p->N, p->N, p->C, p->H, p->W, st)))) return rc;

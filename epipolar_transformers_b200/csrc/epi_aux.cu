@@ -148,6 +148,30 @@ cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, cons
 }
 
 // ------------------------------------------------------------------------------------------
+// Deterministic backward: fixed-point sums [N,HW,C] (int64, scale 2^s of pair n, det_scale) -> the pixel-major fp32 gradient
+// buffer the transposition pass reads, each value rounded once: fp32(acc·2^-s).  A pair whose bound is not finite was not
+// scattered and comes out all NaN; a pair with a zero bound comes out zero.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) acc_to_f32_kernel(const long long *__restrict__ acc, const unsigned *__restrict__ pair_max,
+                                                         float *__restrict__ dsrc, int HW, int C) {
+    const int n = blockIdx.y;
+    const size_t len = (size_t)HW * C, base = (size_t)n * len;
+    const unsigned word = __ldg(pair_max + n);
+    int s = 0;
+    const bool scaled = det_scale(word, HW, s);
+    const float fill = __uint_as_float(word) == 0.f ? 0.f : __int_as_float(0x7fffffff);     // zero bound: zeros; else NaN
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += (size_t)gridDim.x * blockDim.x)
+        dsrc[base + i] = scaled ? (float)ldexp((double)__ldg(acc + base + i), -s) : fill;
+}
+
+cudaError_t launch_acc_to_f32(const long long *acc, const unsigned *pair_max, float *dsrc, int N, int HW, int C, cudaStream_t st) {
+    const size_t len = (size_t)HW * C;
+    const int blocks = (int)((len + 255) / 256 < 1024 ? (len + 255) / 256 : 1024);
+    acc_to_f32_kernel<<<dim3(blocks, N), 256, 0, st>>>(acc, pair_max, dsrc, HW, C);
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
 // Fold conv1x1 z + eval BN (epipolar.py:250-251, BN.py:79 with training=False) into Wf, bf.
 // ------------------------------------------------------------------------------------------
 __global__ void fold_z_bn_kernel(const float *__restrict__ zw, const float *__restrict__ zb,

@@ -296,6 +296,19 @@ __device__ __forceinline__ Taps make_taps(float gx, float gy, int H, int W, int 
     return t;
 }
 
+// Fixed-point scale of the deterministic backward's source-gradient sums for one pair: `word` holds the bits of M_max, the
+// pair's bound on Σ_pixels |contribution| to any one element.  With M_max in [2^(e-1), 2^e) and HW <= 2^L, s = 61 - L - e keeps
+// every sum below HW·M_max·2^s < 2^61, inside int64 with headroom for the fp32 rounding of the contributions.  Returns false
+// (no scatter) for M_max = 0 and for a non-finite bound.
+__device__ __forceinline__ bool det_scale(unsigned word, int HW, int &s) {
+    const float m = __uint_as_float(word);
+    if (!(m > 0.f && m <= 3.402823466e38f)) return false;
+    int e;
+    frexpf(m, &e);
+    s = 61 - (32 - __clz(HW - 1)) - e;
+    return true;
+}
+
 // arg-max over the samples (DESIGN a6): the first maximum wins, like torch.argmax, so a candidate (v, k) replaces the best
 // (bv, bk) so far when it is larger, or equal at a lower sample index.  Every merge of partial arg-maxes uses this rule.
 // (A macro: as a function returning bool it leaves the kernels' branch structure, and so their machine code, different.)

@@ -59,8 +59,17 @@ struct BwdArgs {
     float softmax_scale;
     int grad_keys, grad_vals;
     GeomCfg geom;
+    // deterministic path (dsrc_nhwc unused): per-(pair, sample, pixel) scatter coefficients, the per-pair bound word (float bits,
+    // zeroed, folded with atomicMax) and the zeroed [N,H,W,C] fixed-point accumulator of dL/dfeat_src
+    float2 *coef;
+    unsigned *pair_max;
+    long long *acc;
 };
 cudaError_t launch_fusion_bwd(const BwdArgs &a, cudaStream_t st);
+// deterministic backward: coefficient pass + fixed-point scatter into a.acc (a.coef, a.pair_max, a.acc set; a.dsrc_nhwc unused)
+cudaError_t launch_fusion_bwd_det(const BwdArgs &a, cudaStream_t st, int &launched);
+// fixed-point accumulator [N,HW,C] + per-pair bound words -> pixel-major fp32 dsrc (NaN for a pair whose bound is not finite)
+cudaError_t launch_acc_to_f32(const long long *acc, const unsigned *pair_max, float *dsrc, int N, int HW, int C, cudaStream_t st);
 
 // z-projection epilogue:  y[n,o,p] = sum_c Wf[o,c]·x[n,c,p] + bf[o] (+x[n,o,p]) (+ref[n,o,p])
 struct ZArgs {

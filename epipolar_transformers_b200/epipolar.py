@@ -235,11 +235,21 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
 
 def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *, K, downsample=4.0, img_scale=1.0,
                              softmax_scale=0.125, correct_normalize=False, align_corners=False, grad_attn=None,
-                             sample_locs_in=None, grad_keys=True, grad_vals=True, need_ref=True, need_src=True):
+                             sample_locs_in=None, grad_keys=True, grad_vals=True, need_ref=True, need_src=True,
+                             deterministic=None):
     """Backward of `epipolar_fusion` without the z epilogue: returns (dL/dfeat_ref | None, dL/dfeat_src | None).
     Restates autograd through epipolar.py:188-247 (grid_sample x2, mul/sum, ==0 mask, softmax, weighted sum);
     grad_keys / grad_vals = 'other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD (:141-153).
-    The gradients have the maps' dtype (computed in float32, rounded once); grad_out is float32 like the forward's `out`."""
+    The gradients have the maps' dtype (computed in float32, rounded once); grad_out is float32 like the forward's `out`.
+
+    deterministic: None follows torch.are_deterministic_algorithms_enabled(); True / False force the path.  The deterministic
+    path sums dL/dfeat_src in per-pair int64 fixed point, so identical inputs give identical bits whatever the rest of the batch
+    and the layouts; it costs two more launches and more workspace (DESIGN.md §5).  A pair whose maps or gradients hold a NaN
+    or inf gets an all-NaN dL/dfeat_src there.  dL/dfeat_ref is order-fixed, and the same bits, on both paths."""
+    if deterministic is None:
+        deterministic = torch.are_deterministic_algorithms_enabled()
+    elif not isinstance(deterministic, bool):
+        raise TypeError("deterministic must be None or a bool (got %s)" % type(deterministic).__name__)
     lib = _lib.load()
     dcode = _check_feat_pair(feat_ref, feat_src)
     N, C, H, W = feat_ref.shape
@@ -273,6 +283,7 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
     p.align_corners = int(bool(align_corners)); p.correct_normalize = int(bool(correct_normalize))
     p.grad_keys = int(bool(grad_keys)); p.grad_vals = int(bool(grad_vals))
     p.feat_dtype = dcode
+    p.deterministic = int(deterministic)
     nbytes = lib.epi_fusion_backward_workspace_bytes(ctypes.byref(p))
     ws = torch.empty(max(nbytes, 1), device=dev, dtype=torch.uint8)
     p.workspace = ws.data_ptr(); p.workspace_bytes = nbytes
@@ -315,7 +326,7 @@ class _FusionFn(torch.autograd.Function):
             feat_ref, feat_src, P_ref, P_src, attn, g_out, K=f["K"], downsample=f["downsample"], img_scale=f["img_scale"],
             softmax_scale=f["softmax_scale"], correct_normalize=f["correct_normalize"], align_corners=f["align_corners"],
             grad_attn=g_attn, sample_locs_in=locs, grad_keys=o["grad_keys"], grad_vals=o["grad_vals"], need_ref=need_ref,
-            need_src=need_src)
+            need_src=need_src, deterministic=None)          # read torch's flag now, as PyTorch's own ops do in their backward
         if ctx.needs_input_grad[1] and g_src is None:
             g_src = torch.zeros_like(feat_src)
         return g_ref, g_src, None, None, None
@@ -362,6 +373,9 @@ class Epipolar(nn.Module):
       align_corners     grid_sample semantics; False = what the reference does under torch>=1.3
       fuse_ref_residual also add feat1 inside the kernel (use `fused_other_feat` as the caller)
       variant           'auto' | 'warp' | 'tile' kernel selection
+
+    Under torch.use_deterministic_algorithms(True) the training backward is bit-reproducible (see
+    `epipolar_fusion_backward`); the flag is read when the backward runs.  The z conv and BatchNorm stay PyTorch's.
     """
 
     def __init__(self, debug=False, *, cfg=None, align_corners=False, fuse_ref_residual=False, variant="auto",

@@ -145,11 +145,18 @@ typedef struct EpiFusionBwdParams {
     int32_t align_corners, correct_normalize;
     int32_t grad_keys, grad_vals; /* 'other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD */
     int32_t feat_dtype;           /* EPI_DTYPE_* of feat_ref, feat_src, grad_ref and grad_src (ABI v3; 0 = float32) */
-    int32_t reserved[3];
+    int32_t deterministic;        /* 0: dL/dfeat_src is summed with float atomics, whose order (and so last bits) varies from run to
+                                     run.  1: bit-reproducible: the same inputs give the same bits, whatever the batch around a
+                                     pair and the layouts; sums in per-pair int64 fixed point (DESIGN.md §5), more workspace and two
+                                     more launches.  A pair whose gradients or maps hold a NaN or inf gets an all-NaN dL/dfeat_src.
+                                     dL/dfeat_ref is order-fixed on both paths and the same bits on both.  Other values: EPI_EINVAL. */
+    int32_t reserved[2];
 } EpiFusionBwdParams;
 
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p);
 int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream);
+/* 1: this library honours EpiFusionBwdParams.deterministic (a library built before the field read it as a reserved word). */
+int epi_fusion_backward_deterministic(void);
 
 /* Only the geometry: sample locations [K,N,H,W,2] for (P_ref,P_src)  (grid2sample_locs). */
 int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_locs_out, int32_t N,
@@ -191,7 +198,7 @@ float epi_kernel_timing_last_ms(void);
 /* same, per launch group: ms3[0] operand staging, ms3[1] fused attention kernel, ms3[2] epilogue pass */
 int epi_kernel_timing_last3(float *ms3);
 
-/* Number of kernels the last successful epi_fusion_forward_f32 on this thread launched. */
+/* Number of kernels the last successful epi_fusion_forward_f32 or epi_fusion_backward_f32 on this thread launched. */
 int epi_last_launch_count(void);
 
 #ifdef __cplusplus
