@@ -114,8 +114,10 @@ Plan make_plan(const EpiFusionParams *p) {
 
     Regions ws;
     if (pl.kernel == Kernel::Pipe) {
-        // without z the fused kernel writes a channels-last `out` with 16-byte stores; any other `out` gets a pixel-major plane
-        const bool out_direct = p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0;
+        // without z the fused kernel writes a channels-last, 16-byte-aligned `out` with 16-byte stores; any other `out` gets a
+        // pixel-major plane and the transposition pass, which checks the alignment of each store itself
+        const bool out_direct = p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0 &&
+                                reinterpret_cast<uintptr_t>(p->out) % 16 == 0;
         pl.staging = Staging::Pipe;
         pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32) : (out_direct ? Epilogue::Direct : Epilogue::Unstage);
         if (lowp && pl.epilogue == Epilogue::ZFp32 && p->add_ref_residual) pl.ref_copy = RefCopy::After;   // the fp32 z epilogue's residual
@@ -160,6 +162,9 @@ Plan make_plan(const EpiFusionParams *p) {
     return pl;
 }
 
+// a null pointer (an absent optional buffer) or one that (x, y) float pairs can be loaded from and stored to as float2
+inline bool aligned8(const void *q) { return reinterpret_cast<uintptr_t>(q) % 8 == 0; }
+
 // the size queries answer 0 for params no plan is made for
 bool plannable(const EpiFusionParams *p) { return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0; }
 
@@ -185,6 +190,9 @@ int validate(const EpiFusionParams *p) {
     }
     if (p->z_weight_folded && (reinterpret_cast<uintptr_t>(p->z_weight_folded) % 16 != 0 || reinterpret_cast<uintptr_t>(p->z_bias_folded) % 4 != 0))
         return fail(EPI_EINVAL, "z_weight_folded must be 16-byte aligned (contiguous [C,C]) and z_bias_folded 4-byte aligned");
+    // every kernel reads and writes the (x, y) pairs of these three as one 8-byte vector
+    if (!aligned8(p->sample_locs_in) || !aligned8(p->sample_locs_out) || !aligned8(p->corr_pos))
+        return fail(EPI_EINVAL, "sample_locs_in, sample_locs_out and corr_pos must be 8-byte aligned (whole (x, y) float pairs)");
     return EPI_OK;
 }
 
@@ -196,6 +204,7 @@ int validate_bwd(const EpiFusionBwdParams *p) {
     if (p->C > 512 || (p->C > 128 && p->C % 4 != 0)) return fail(EPI_EINVAL, "backward supports C <= 128, or C <= 512 with C % 4 == 0");
     if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
     if (p->deterministic != 0 && p->deterministic != 1) return fail(EPI_EINVAL, "deterministic must be 0 or 1");
+    if (!aligned8(p->sample_locs_in)) return fail(EPI_EINVAL, "sample_locs_in must be 8-byte aligned (whole (x, y) float pairs)");
     return EPI_OK;
 }
 
@@ -469,6 +478,7 @@ int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_lo
                         int32_t correct_normalize, void *stream) {
     if (!P_ref || !P_src || !sample_locs_out) return fail(EPI_EINVAL, "null pointer");
     if (N <= 0 || H < 2 || W < 2 || K < 2) return fail(EPI_EINVAL, "bad shape");
+    if (!aligned8(sample_locs_out)) return fail(EPI_EINVAL, "sample_locs_out must be 8-byte aligned (whole (x, y) float pairs)");
     epi::GeomCfg g = make_geom(H, W, K, downsample, img_scale, eps, correct_normalize, 0);
     cudaError_t e = epi::launch_sample_locs(P_ref, P_src, sample_locs_out, N, g, reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(EPI_ECUDA, "sample_locs launch failed: %s", cudaGetErrorString(e));

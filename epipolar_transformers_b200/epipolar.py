@@ -38,6 +38,13 @@ def _strides4(t: torch.Tensor):
     return (ctypes.c_int64 * 4)(*t.stride())
 
 
+def _aligned_locs(t: torch.Tensor) -> torch.Tensor:
+    """sample locations as the ABI takes them: contiguous float32 on the device, 8-byte aligned (the kernels load (x, y) as one
+    pair).  `.contiguous()` keeps a contiguous view that starts at an odd element, so such a view is copied."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 8 == 0 else t.clone()
+
+
 # element types the kernels read natively (EPI_DTYPE_*); bf16 / fp16 maps give the fp32 result of their exact values
 FEAT_DTYPES = {torch.float32: _lib.EPI_DTYPE_F32, torch.bfloat16: _lib.EPI_DTYPE_BF16, torch.float16: _lib.EPI_DTYPE_F16}
 
@@ -175,7 +182,7 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
         if tuple(P_ref.shape) != (N, 3, 4) or tuple(P_src.shape) != (NP, 3, 4):
             raise ValueError("P_ref/P_src must be [N,3,4]" if S == 1 else "P_ref must be [N,3,4] and P_srcs [S,N,3,4]")
     else:
-        sample_locs_in = sample_locs_in.to(device=dev, dtype=torch.float32).contiguous()
+        sample_locs_in = _aligned_locs(sample_locs_in.to(device=dev, dtype=torch.float32))
         if tuple(sample_locs_in.shape) != (K, NP, H, W, 2):
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
     if out is None:
@@ -185,7 +192,9 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     locs = torch.empty((K, NP, H, W, 2), device=dev, dtype=torch.float32) if want_locs else None
 
     vcode = _lib.VARIANTS[variant] if isinstance(variant, str) else int(variant)
-    key = (dev, S, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), z_folded is not None, vcode,
+    # the plan (and so the workspace size) also depends on whether `out` and feat_src start on a 16-byte boundary
+    key = (dev, S, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), out.data_ptr() % 16 == 0,
+           feat_src.data_ptr() % 16 == 0, z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
     if state is not None and state.key == key:
@@ -267,7 +276,7 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
         P_ref = P_ref.to(device=dev, dtype=torch.float32).contiguous(); P_src = P_src.to(device=dev, dtype=torch.float32).contiguous()
         p.P_ref = P_ref.data_ptr(); p.P_src = P_src.data_ptr()
     else:
-        sample_locs_in = sample_locs_in.to(device=dev, dtype=torch.float32).contiguous()
+        sample_locs_in = _aligned_locs(sample_locs_in.to(device=dev, dtype=torch.float32))
         p.sample_locs_in = sample_locs_in.data_ptr()
     p.attn = attn.data_ptr()
     p.grad_out = grad_out.data_ptr(); p.gout_stride = _strides4(grad_out)

@@ -19,6 +19,15 @@
  * device memory; the caller passes a workspace.  Every entry point is re-entrant, takes the
  * CUDA stream explicitly, never synchronises the device, and returns 0 on success or a
  * negative EPI_E* code (epi_last_error() gives a thread-local message).
+ *
+ * Alignment.  Every tensor pointer must be aligned to its element size.  Strides are in elements and may describe any
+ * non-negative view: crops, channel slices, transposes, batch steps, and stride 0 on an input (a broadcast map).  Stricter:
+ *   sample_locs_in, sample_locs_out, corr_pos   8 bytes (read and written as (x, y) float pairs): else EPI_EINVAL
+ *   z_weight_folded                            16 bytes: else EPI_EINVAL
+ *   workspace, cache                           256 bytes: else EPI_EINVAL
+ * Nothing else is required: the library takes a 16-byte vector path only where it has checked the pointer and the strides
+ * (e.g. an `out` that is not 16-byte aligned is written through a transposition pass instead of directly), so any other
+ * alignment only costs speed.  Outputs must not overlap each other or the inputs.
  */
 #ifndef EPIPOLAR_B200_H_
 #define EPIPOLAR_B200_H_
@@ -58,14 +67,14 @@ typedef struct EpiFusionParams {
     int64_t src_stride[4];
     const float *P_ref;           /* [N,3,4] contiguous: KRT of the reference view  (forward arg P1) */
     const float *P_src;           /* [N,3,4] contiguous: KRT of the source view     (forward arg P2) */
-    const float *sample_locs_in;  /* optional [K,N,H,W,2] normalised grid coords: replaces the fused
+    const float *sample_locs_in;  /* optional [K,N,H,W,2] contiguous, 8-byte aligned: normalised grid coords replacing the fused
                                      geometry (parity protocol T1: inject the reference's own locations) */
     /* ---- outputs --------------------------------------------------------------------- */
-    float *out;                   /* [N,C,H,W] logical, strides below */
+    float *out;                   /* [N,C,H,W] logical, strides below, 4-byte aligned */
     int64_t out_stride[4];
     float *attn;                  /* optional [N,K,H,W] contiguous: softmax weights ("depth", epipolar.py:263) */
-    float *corr_pos;              /* optional [N,H,W,2] contiguous: arg-max correspondence, feature px (:237-242) */
-    float *sample_locs_out;       /* optional [K,N,H,W,2] contiguous: locations actually sampled (:183) */
+    float *corr_pos;              /* optional [N,H,W,2] contiguous, 8-byte aligned: arg-max correspondence, feature px (:237-242) */
+    float *sample_locs_out;       /* optional [K,N,H,W,2] contiguous, 8-byte aligned: locations actually sampled (:183) */
     /* ---- optional folded eval-mode epilogue:  y = Wf·o + bf  (+ o if z_residual) ------ */
     const float *z_weight_folded; /* [C,C] row-major (out_ch, in_ch) = diag(gamma/sqrt(var+eps))·Wz, or NULL */
     const float *z_bias_folded;   /* [C] */
@@ -129,7 +138,7 @@ typedef struct EpiFusionBwdParams {
     const void *feat_src;         /* element type feat_dtype */
     int64_t src_stride[4];
     const float *P_ref, *P_src;   /* [N,3,4] */
-    const float *sample_locs_in;  /* optional, as in the forward */
+    const float *sample_locs_in;  /* optional, as in the forward (contiguous, 8-byte aligned) */
     const float *attn;            /* [N,K,H,W] contiguous: the forward's attention output */
     const float *grad_out;        /* [N,C,H,W] logical: dL/d(fused feature) */
     int64_t gout_stride[4];

@@ -214,6 +214,100 @@ def fp64_reference(f1, f2, locs, scale, correct, align_corners=False, pixels=Non
     return np.stack(outs), np.stack(attns), np.stack(corrs)
 
 
+# ---- a test-local driver of the C ABI ------------------------------------------------------------------------------------
+# Fills EpiFusionParams / EpiFusionBwdParams from tensors the test owns, the way epipolar_fusion and epipolar_fusion_backward
+# do, so that a test decides every buffer: its strides, its base address, what it holds before the call and what lies
+# around it.  None of these helpers allocates an output, and none keeps a tensor alive: the caller holds every tensor it
+# passes until `launch` has returned (a temporary freed earlier can be handed out again as the workspace).
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _strides(t):
+    import ctypes
+    return (ctypes.c_int64 * 4)(*(t.stride() if t is not None else (0, 0, 0, 0)))
+
+
+def _feat_dtype(t):
+    import torch
+    from epipolar_transformers_b200 import _lib
+    return {torch.float32: _lib.EPI_DTYPE_F32, torch.bfloat16: _lib.EPI_DTYPE_BF16, torch.float16: _lib.EPI_DTYPE_F16}[t.dtype]
+
+
+def fusion_params(f1, f2, out, *, K, P1=None, P2=None, locs_in=None, attn=None, corr=None, locs_out=None, z=None,
+                  z_residual=False, add_ref=False, variant="auto", n_src=0, align_corners=False, correct=True, downsample=4.0,
+                  img_scale=1.0, scale=0.125):
+    """EpiFusionParams of one forward: f1 [N,C,H,W], f2 / out [S·N,C,H,W] (any strides), z = (Wf, bf) or None."""
+    from epipolar_transformers_b200 import _lib
+    p = _lib.EpiFusionParams()
+    N, C, H, W = f1.shape
+    p.feat_ref, p.ref_stride = f1.data_ptr(), _strides(f1)
+    p.feat_src, p.src_stride = f2.data_ptr(), _strides(f2)
+    p.out, p.out_stride = out.data_ptr(), _strides(out)
+    p.P_ref, p.P_src, p.sample_locs_in = _ptr(P1), _ptr(P2), _ptr(locs_in)
+    p.attn, p.corr_pos, p.sample_locs_out = _ptr(attn), _ptr(corr), _ptr(locs_out)
+    if z is not None:
+        p.z_weight_folded, p.z_bias_folded = z[0].data_ptr(), z[1].data_ptr()
+    p.N, p.C, p.H, p.W, p.K = N, C, H, W, K
+    p.downsample, p.img_scale, p.eps, p.softmax_scale = downsample, img_scale, 1e-3, scale
+    p.align_corners, p.correct_normalize = int(align_corners), int(correct)
+    p.z_residual, p.add_ref_residual = int(z_residual), int(add_ref)
+    p.variant = _lib.VARIANTS[variant]
+    p.feat_dtype = _feat_dtype(f1)
+    p.n_src = n_src
+    return p
+
+
+def bwd_params(f1, f2, attn, g_out, *, K, P1=None, P2=None, locs_in=None, grad_ref=None, grad_src=None, deterministic=False,
+               correct=True, scale=0.125):
+    """EpiFusionBwdParams of one backward (grad_keys and grad_vals on, no attention gradient)."""
+    from epipolar_transformers_b200 import _lib
+    b = _lib.EpiFusionBwdParams()
+    N, C, H, W = f1.shape
+    b.feat_ref, b.ref_stride = f1.data_ptr(), _strides(f1)
+    b.feat_src, b.src_stride = f2.data_ptr(), _strides(f2)
+    b.P_ref, b.P_src, b.sample_locs_in = _ptr(P1), _ptr(P2), _ptr(locs_in)
+    b.attn = attn.data_ptr()
+    b.grad_out, b.gout_stride = g_out.data_ptr(), _strides(g_out)
+    b.grad_ref, b.gref_stride = _ptr(grad_ref), _strides(grad_ref)
+    b.grad_src, b.gsrc_stride = _ptr(grad_src), _strides(grad_src)
+    b.N, b.C, b.H, b.W, b.K = N, C, H, W, K
+    b.downsample, b.img_scale, b.eps, b.softmax_scale = 4.0, 1.0, 1e-3, scale
+    b.correct_normalize = int(correct)
+    b.grad_keys = b.grad_vals = 1
+    b.feat_dtype = _feat_dtype(f1)
+    b.deterministic = int(deterministic)
+    return b
+
+
+def workspace_bytes(p):
+    """the forward's workspace size for these params (a pure query: nothing is launched)"""
+    import ctypes
+    from epipolar_transformers_b200 import _lib
+    return _lib.load().epi_fusion_workspace_bytes(ctypes.byref(p))
+
+
+def launch(p, workspace=None, cache=None, backward=False):
+    """Runs the forward (or backward) on the current stream with the given uint8 workspace / cache tensors (None: none) and
+    synchronises.  -> number of kernels launched."""
+    import ctypes
+    import torch
+    from epipolar_transformers_b200 import _lib
+    lib = _lib.load()
+    if workspace is not None:
+        p.workspace, p.workspace_bytes = workspace.data_ptr(), workspace.numel()
+    if cache is not None:
+        p.cache, p.cache_bytes = cache.data_ptr(), cache.numel()
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    if backward:
+        _lib.check(lib.epi_fusion_backward_f32(ctypes.byref(p), stream), "epi_fusion_backward_f32")
+    else:
+        _lib.check(lib.epi_fusion_forward_f32(ctypes.byref(p), stream), "epi_fusion_forward_f32")
+    torch.cuda.synchronize()
+    return lib.epi_last_launch_count()
+
+
 def corr_close(a, b):
     """corr_pos equality: 1e-4 feature px, relaxed by 1e-6 relative for the de-normalised far / huge locations (whose fp32 ulp
     exceeds it); NaN equals NaN and inf equals inf."""
