@@ -21,7 +21,7 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_fusion_backward_workspace_bytes", "epi_fusion_backward_f32", "epi_find_peaks_f32", "epi_find_peaks_best_f32",
            "epi_sample_locs_f32", "epi_fold_z_bn_f32", "epi_last_launch_count", "epi_umma_selftest",
            "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3",
-           "epi_fusion_backward_deterministic")
+           "epi_fusion_backward_deterministic", "epi_fusion_views")
 
 _fp = ctypes.POINTER(ctypes.c_float)
 
@@ -43,6 +43,15 @@ class EpiFusionParams(ctypes.Structure):
         ("n_src", ctypes.c_int32), ("reserved", ctypes.c_int32 * 1),
         ("cache", ctypes.c_void_p), ("cache_bytes", ctypes.c_size_t),
     ]
+
+    # n_views shares its word with reserved[0] (an anonymous union in the header keeps the old name)
+    @property
+    def n_views(self):
+        return self.reserved[0]
+
+    @n_views.setter
+    def n_views(self, v):
+        self.reserved[0] = v
 
 
 class EpiFusionBwdParams(ctypes.Structure):
@@ -80,7 +89,8 @@ def load():
     lib = ctypes.CDLL(LIB_PATH)
     missing = [s for s in EXPORTS if not hasattr(lib, s)]
     if missing:
-        # e.g. a library built before EpiFusionBwdParams.deterministic, which would ignore the field
+        # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
+        # (a views call would silently run as a one-source call)
         raise RuntimeError("libepipolar_b200.so does not export %s; rebuild it with "
                            "`python -m epipolar_transformers_b200.build --force`" % missing)
     lib.epi_version.restype = ctypes.c_int
@@ -118,6 +128,7 @@ def load():
     lib.epi_kernel_timing_last3.restype = ctypes.c_int
     lib.epi_kernel_timing_last3.argtypes = [ctypes.POINTER(ctypes.c_float)]
     lib.epi_fusion_backward_deterministic.restype = ctypes.c_int
+    lib.epi_fusion_views.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))

@@ -47,14 +47,22 @@ struct Launches {
 
 // source views per reference item (EpiFusionParams.n_src: 0 and 1 both mean one)
 inline int n_sources(const EpiFusionParams *p) { return p->n_src > 1 ? p->n_src : 1; }
-// (reference, source) pairs = items of feat_src, out, attn, corr_pos and the sample locations
-inline int n_pairs(const EpiFusionParams *p) { return n_sources(p) * p->N; }
+// (query, source) pairs = items of out, attn, corr_pos and the sample locations: S·N, or V·(V−1)·N in the views form
+inline int64_t n_pairs64(const EpiFusionParams *p) {
+    return p->n_views ? (int64_t)p->n_views * (p->n_views - 1) * p->N : (int64_t)n_sources(p) * p->N;
+}
+inline int n_pairs(const EpiFusionParams *p) { return (int)n_pairs64(p); }
+// The views form (n_views = V) has one map, feat_ref with its V·N view items, that is both the query and the source map.
+inline int n_ref_items(const EpiFusionParams *p) { return p->n_views ? p->n_views * p->N : p->N; }
+inline int n_src_items(const EpiFusionParams *p) { return p->n_views ? p->n_views * p->N : n_pairs(p); }
+inline const void *src_map(const EpiFusionParams *p) { return p->n_views ? p->feat_ref : p->feat_src; }
+inline const int64_t *src_strides(const EpiFusionParams *p) { return p->n_views ? p->ref_stride : p->src_stride; }
 
 bool src_is_channels_last(const EpiFusionParams *p) {
-    const int64_t *s = p->src_stride;
+    const int64_t *s = src_strides(p);
     const int64_t C = p->C, H = p->H, W = p->W;
-    return s[1] == 1 && s[3] == C && s[2] == W * C && (n_pairs(p) == 1 || s[0] == H * W * C) &&
-           (reinterpret_cast<uintptr_t>(p->feat_src) % 16 == 0);
+    return s[1] == 1 && s[3] == C && s[2] == W * C && (n_src_items(p) == 1 || s[0] == H * W * C) &&
+           (reinterpret_cast<uintptr_t>(src_map(p)) % 16 == 0);
 }
 
 enum class Kernel { Pipe, Sector, Tile, Warp };          // fused attention kernel (sector and 4x8 block tiles: epi_fusion_tile_kernel)
@@ -97,10 +105,14 @@ bool want_tile(const EpiFusionParams *p) {
 
 // Sizes: `ref_map` is one fp32 copy of the N reference items, `map` one fp32 map of the S·N pairs (source items, fused features).
 // The reference planes are staged once however many sources they are fused with.  One bf16 plane of a map is half its fp32 bytes.
+// The views form stages its V·N items once (`ref_map`): they are both the query and the source planes, and `map` covers the
+// V·(V−1)·N pairs' fused features only.
 Plan make_plan(const EpiFusionParams *p) {
     Plan pl;
+    const bool views = p->n_views != 0;
     const size_t NP = (size_t)n_pairs(p), px = (size_t)p->H * p->W;
-    const size_t ref_map = (size_t)p->N * p->C * px * sizeof(float), map = NP * p->C * px * sizeof(float);
+    const size_t ref_map = (size_t)n_ref_items(p) * p->C * px * sizeof(float), map = NP * p->C * px * sizeof(float);
+    const size_t src_map_bytes = (size_t)n_src_items(p) * p->C * px * sizeof(float);
     const size_t order_bytes = NP * px * sizeof(uint16_t), geom_bytes = NP * sizeof(epi::PairGeom);
     const bool lowp = p->feat_dtype != EPI_DTYPE_F32, has_z = p->z_weight_folded != nullptr;
     // sector tiles (pixels grouped by epipolar angle) need the fused geometry; injected locations and an explicit
@@ -127,8 +139,10 @@ Plan make_plan(const EpiFusionParams *p) {
         const bool lo = p->feat_dtype != EPI_DTYPE_BF16;
         pl.ref_hi = ws.part(ref_map / 2);
         if (lo) pl.ref_lo = ws.part(ref_map / 2);
-        pl.src_hi = ws.part(map / 2);
-        if (lo) pl.src_lo = ws.part(map / 2);
+        if (!views) {
+            pl.src_hi = ws.part(map / 2);
+            if (lo) pl.src_lo = ws.part(map / 2);
+        }
         ws.close();
         // fused feature: bf16 (hi, lo) planes for the z GEMM; fp32, contiguous NCHW for the z epilogue, pixel-major for the transposition
         if (pl.epilogue == Epilogue::ZGemm) { pl.fused = ws.part(map / 2); pl.fused_lo = ws.take(map / 2); }
@@ -140,7 +154,7 @@ Plan make_plan(const EpiFusionParams *p) {
         Regions cache;
         pl.key = cache.take(NP * 32 * sizeof(float));
         const size_t cache_geom = cache.take(geom_bytes), cache_order = cache.take(order_bytes);
-        pl.n_records = epi::fusion_pipe_plan_records((int)NP, p->N, p->H, p->W);
+        pl.n_records = epi::fusion_pipe_plan_records((int)NP, p->N, p->H, p->W);       // N: the pairs of one source (or view pair)
         pl.records = cache.take((size_t)pl.n_records * epi::fusion_pipe_plan_record_bytes());
         pl.cache_bytes = cache.end;
         if (pl.cached) { pl.geom = cache_geom; pl.order = cache_order; }
@@ -151,12 +165,18 @@ Plan make_plan(const EpiFusionParams *p) {
         pl.staging = tiles ? Staging::Planes : (!src_is_channels_last(p) || lowp ? Staging::Nhwc : Staging::InPlace);
         pl.epilogue = has_z ? Epilogue::ZFp32 : Epilogue::Direct;
         pl.ref_copy = lowp ? RefCopy::Before : RefCopy::None;        // these kernels read the query (and the residual) as fp32
+        // views form: a low-precision map's fp32 copy is the warp kernel's source as it stands, and the sector tiles query the
+        // source planes
+        if (views && lowp && !tiles) pl.staging = Staging::InPlace;
         if (lowp) pl.ref32 = ws.take(ref_map);
-        if (tiles) { pl.src_hi = ws.part(map / 2); pl.src_lo = ws.take(map / 2); }
-        else if (pl.staging == Staging::Nhwc) pl.src_nhwc = ws.take(map);
+        if (tiles) { pl.src_hi = ws.part(src_map_bytes / 2); pl.src_lo = ws.take(src_map_bytes / 2); }
+        else if (pl.staging == Staging::Nhwc) pl.src_nhwc = ws.take(src_map_bytes);
         if (has_z) pl.fused = ws.take(map);
         if (tiles) pl.counter = ws.take(256);
-        if (pl.kernel == Kernel::Sector) { pl.ref_hi = ws.part(ref_map / 2); pl.ref_lo = ws.take(ref_map / 2); pl.order = ws.take(order_bytes); }
+        if (pl.kernel == Kernel::Sector) {
+            if (!views) { pl.ref_hi = ws.part(ref_map / 2); pl.ref_lo = ws.take(ref_map / 2); }
+            pl.order = ws.take(order_bytes);
+        }
     }
     pl.workspace_bytes = ws.end;
     return pl;
@@ -166,12 +186,23 @@ Plan make_plan(const EpiFusionParams *p) {
 inline bool aligned8(const void *q) { return reinterpret_cast<uintptr_t>(q) % 8 == 0; }
 
 // the size queries answer 0 for params no plan is made for
-bool plannable(const EpiFusionParams *p) { return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0; }
+bool plannable(const EpiFusionParams *p) {
+    return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0 &&
+           (p->n_views == 0 || (p->n_views >= 2 && p->n_views <= 256 && p->n_src <= 1 && n_pairs64(p) <= 65535));
+}
 
 int validate(const EpiFusionParams *p) {
     if (!p) return fail(EPI_EINVAL, "params is null");
-    if (!p->feat_ref || !p->feat_src || !p->out) return fail(EPI_EINVAL, "feat_ref/feat_src/out must be non-null");
-    if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
+    if (p->n_views < 0 || p->n_views == 1) return fail(EPI_EINVAL, "n_views must be 0 or >= 2 (every view against every other)");
+    if (p->n_views) {
+        if (p->feat_src || p->P_src) return fail(EPI_EINVAL, "n_views >= 2: feat_src and P_src must be null (feat_ref / P_ref hold the views)");
+        if (p->n_src > 1) return fail(EPI_EINVAL, "n_views >= 2 needs n_src 0 or 1");
+        if (!p->feat_ref || !p->out) return fail(EPI_EINVAL, "feat_ref/out must be non-null");
+        if (!p->sample_locs_in && !p->P_ref) return fail(EPI_EINVAL, "P_ref required without sample_locs_in");
+    } else {
+        if (!p->feat_ref || !p->feat_src || !p->out) return fail(EPI_EINVAL, "feat_ref/feat_src/out must be non-null");
+        if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
+    }
     if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2) return fail(EPI_EINVAL, "need N,C >= 1 and H,W >= 2");
     if (p->K < 2 || p->K > 256) return fail(EPI_EINVAL, "K (SAMPLESIZE) must be in [2,256]");
     if (p->C > 1024 || (p->C > 512 && p->C % 4 != 0)) return fail(EPI_EINVAL, "C must be <= 512, or <= 1024 and a multiple of 4");
@@ -180,13 +211,13 @@ int validate(const EpiFusionParams *p) {
     if (p->variant < EPI_VARIANT_AUTO || p->variant > EPI_VARIANT_PIPE) return fail(EPI_EINVAL, "unknown variant");
     if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
     if (p->n_src < 0) return fail(EPI_EINVAL, "n_src must be >= 0 (0 or 1: one source view per reference item)");
-    if (p->n_src > 1) {
+    if (p->n_src > 1 || p->n_views) {
         // the layout, transposition and z epilogue kernels put the item in the grid's z dimension; the pipelined kernel numbers
         // its per-pair work records, and the staging kernel its tiles, in 32-bit ints
-        const int64_t np = (int64_t)p->n_src * p->N, hw = (int64_t)p->H * p->W;
-        if (np > 65535) return fail(EPI_EINVAL, "n_src * N must be <= 65535 (grid z dimension of the per-item kernels)");
-        if (np * ((hw + 31) / 32 + 1) + p->n_src * 256 > INT32_MAX || 2 * np * ((hw + 63) / 64) * ((p->C + 63) / 64) > INT32_MAX || np * hw > INT32_MAX)
-            return fail(EPI_EINVAL, "n_src * N * H * W too large: per-pair work records and staging tiles are counted in int32");
+        const int64_t np = p->n_views > 256 ? INT64_MAX : n_pairs64(p), hw = (int64_t)p->H * p->W;
+        if (np > 65535) return fail(EPI_EINVAL, "pairs (n_src * N, or n_views * (n_views - 1) * N) must be <= 65535 (grid z dimension of the per-item kernels)");
+        if (np * ((hw + 31) / 32 + 1) + np / p->N * 256 > INT32_MAX || 2 * np * ((hw + 63) / 64) * ((p->C + 63) / 64) > INT32_MAX || np * hw > INT32_MAX)
+            return fail(EPI_EINVAL, "pairs * H * W too large: per-pair work records and staging tiles are counted in int32");
     }
     if (p->z_weight_folded && (reinterpret_cast<uintptr_t>(p->z_weight_folded) % 16 != 0 || reinterpret_cast<uintptr_t>(p->z_bias_folded) % 4 != 0))
         return fail(EPI_EINVAL, "z_weight_folded must be 16-byte aligned (contiguous [C,C]) and z_bias_folded 4-byte aligned");
@@ -256,6 +287,8 @@ int epi_last_launch_count(void) { return g_launches; }
 
 int epi_fusion_backward_deterministic(void) { return 1; }
 
+int epi_fusion_views(void) { return 1; }
+
 int epi_kernel_timing_enable(int on) { g_timing = on ? 1 : 0; return EPI_OK; }
 
 // Not declared in the public header: forces the pipe kernel's 32-pixel work items on every shape (on = 1) or restores the
@@ -304,13 +337,15 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     }
 
     const int dt = p->feat_dtype;
-    const int NP = n_pairs(p);          // pairs: items of feat_src and of every output; feat_ref has p->N items
+    const int NP = n_pairs(p);          // pairs: items of every output (and of feat_src unless n_views)
+    const int NR = n_ref_items(p), V = p->n_views;
+    const float *P_src = V ? p->P_ref : p->P_src;      // the views form takes both cameras of a pair from P_ref
     epi::FusionArgs a;
     memset(&a, 0, sizeof(a));
     a.feat_ref = static_cast<const float *>(p->feat_ref); a.ref_dtype = dt;
-    a.P_ref = p->P_ref; a.P_src = p->P_src; a.locs_in = p->sample_locs_in;
+    a.P_ref = p->P_ref; a.P_src = P_src; a.locs_in = p->sample_locs_in;
     a.attn = p->attn; a.corr_pos = p->corr_pos; a.locs_out = p->sample_locs_out;
-    a.N = NP; a.n_ref = p->N; a.C = p->C; a.softmax_scale = p->softmax_scale; a.item_px = pl.item_px;
+    a.N = NP; a.n_ref = p->N; a.n_views = V; a.C = p->C; a.softmax_scale = p->softmax_scale; a.item_px = pl.item_px;
     for (int i = 0; i < 4; i++) a.ref_stride[i] = p->ref_stride[i];
     a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
     float *ref32 = at<float>(ws, pl.ref32);
@@ -319,12 +354,12 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
 
     // operand staging (first timing group)
     if (pl.ref_copy == RefCopy::Before) {
-        if ((rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
+        if ((rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, NR, p->C, p->H, p->W, dt, st)))) return rc;
         a.feat_ref = ref32; a.ref_dtype = EPI_DTYPE_F32;
         for (int i = 0; i < 4; i++) a.ref_stride[i] = cl_stride[i];
     }
     if (pl.staging == Staging::Pipe) {
-        const bool have_P = p->P_ref && p->P_src;
+        const bool have_P = p->P_ref && P_src;
         void *pairs = pl.cached ? p->cache : ws;
         uint16_t *order = have_P ? at<uint16_t>(pairs, pl.order) : nullptr;
         epi::PairGeom *pg = at<epi::PairGeom>(pairs, pl.geom);
@@ -338,30 +373,33 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         __nv_bfloat16 *w_hi = at<__nv_bfloat16>(ws, pl.w_hi);
         int kernels = 0;
         const cudaError_t e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, at<__nv_bfloat16>(ws, pl.ref_hi),
-                                                p->P_ref, p->P_src, pg, order, okey, w_hi ? p->z_weight_folded : nullptr, w_hi,
-                                                p->z_residual ? 1 : 0, words, NP, p->N, p->C, p->H, p->W, a.geom, st, kernels);
+                                                p->P_ref, P_src, pg, order, okey, w_hi ? p->z_weight_folded : nullptr, w_hi,
+                                                p->z_residual ? 1 : 0, words, NP, p->N, V, p->C, p->H, p->W, a.geom, st, kernels);
         if ((rc = run("operand staging", e, kernels))) return rc;
         a.ref_hi = at<__nv_bfloat16>(ws, pl.ref_hi); a.ref_lo = at<__nv_bfloat16>(ws, pl.ref_lo);
-        a.src_hi = at<__nv_bfloat16>(ws, pl.src_hi); a.src_lo = at<__nv_bfloat16>(ws, pl.src_lo);
+        a.src_hi = V ? a.ref_hi : at<__nv_bfloat16>(ws, pl.src_hi); a.src_lo = V ? a.ref_lo : at<__nv_bfloat16>(ws, pl.src_lo);
         a.order = order; a.pair_geom = pg; a.tile_counter = words; a.err_flag = words + 1;
     } else if (pl.staging == Staging::Planes) {
         __nv_bfloat16 *hi = at<__nv_bfloat16>(ws, pl.src_hi), *lo = at<__nv_bfloat16>(ws, pl.src_lo);
         a.tile_counter = at<int>(ws, pl.counter);
-        if ((rc = run("operand staging", epi::launch_split_planes(p->feat_src, p->src_stride, hi, lo, NP, p->C, p->H, p->W, a.tile_counter, dt, st)))) return rc;
+        if ((rc = run("operand staging", epi::launch_split_planes(src_map(p), src_strides(p), hi, lo, n_src_items(p), p->C, p->H, p->W, a.tile_counter, dt, st))))
+            return rc;
         a.src_hi = hi; a.src_lo = lo;
         if (pl.kernel == Kernel::Sector) {
-            __nv_bfloat16 *rhi = at<__nv_bfloat16>(ws, pl.ref_hi), *rlo = at<__nv_bfloat16>(ws, pl.ref_lo);
+            // the views form queries the source planes: the split of a bf16 / fp16 value equals that of its fp32 copy
+            __nv_bfloat16 *rhi = V ? hi : at<__nv_bfloat16>(ws, pl.ref_hi), *rlo = V ? lo : at<__nv_bfloat16>(ws, pl.ref_lo);
             uint16_t *order = at<uint16_t>(ws, pl.order);
-            if ((rc = run("reference staging", epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st)))) return rc;
-            if ((rc = run("sector ordering", epi::launch_sector_order(p->P_ref, p->P_src, order, NP, p->N, a.geom, st)))) return rc;
+            if (!V && (rc = run("reference staging", epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st))))
+                return rc;
+            if ((rc = run("sector ordering", epi::launch_sector_order(p->P_ref, P_src, order, NP, p->N, V, a.geom, st)))) return rc;
             a.ref_hi = rhi; a.ref_lo = rlo; a.order = order;
         }
     } else if (pl.staging == Staging::Nhwc) {
         float *nhwc = at<float>(ws, pl.src_nhwc);
-        if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(p->feat_src, p->src_stride, nhwc, NP, p->C, p->H, p->W, dt, st)))) return rc;
+        if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(src_map(p), src_strides(p), nhwc, n_src_items(p), p->C, p->H, p->W, dt, st)))) return rc;
         a.src_nhwc = nhwc;
     } else {
-        a.src_nhwc = static_cast<const float *>(p->feat_src);
+        a.src_nhwc = V ? a.feat_ref : static_cast<const float *>(p->feat_src);     // views form: the map itself or its fp32 copy
     }
 
     // where the fused kernel writes
@@ -385,10 +423,10 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
 
     // epilogue (third timing group)
     if (pl.ref_copy == RefCopy::After &&
-        (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, p->N, p->C, p->H, p->W, dt, st)))) return rc;
+        (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, NR, p->C, p->H, p->W, dt, st)))) return rc;
     if (pl.epilogue == Epilogue::Unstage) {
         if ((rc = run("output transposition", epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out,
-                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, p->C, p->H, p->W, st)))) return rc;
+                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, V, p->C, p->H, p->W, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZGemm) {
         epi::ZGemmArgs z;
         memset(&z, 0, sizeof(z));
@@ -396,7 +434,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.ref = p->feat_ref; z.ref_dtype = dt; z.y = p->out;
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
-        z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
+        z.N = NP; z.n_ref = p->N; z.n_views = V; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         if ((rc = run("z GEMM", epi::launch_zgemm(z, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZFp32) {
@@ -405,7 +443,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         z.x = a.out;
         for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? cl_stride[i] : p->ref_stride[i]; }
         z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
-        z.N = NP; z.n_ref = p->N; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
+        z.N = NP; z.n_ref = p->N; z.n_views = V; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         if ((rc = run("z epilogue", epi::launch_z_epilogue(z, st)))) return rc;
     }
@@ -465,10 +503,10 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     }
     if (p->grad_src &&
         (rc = run("gradient transposition", epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride,
-                                                                p->N, p->N, p->C, p->H, p->W, st)))) return rc;
+                                                                p->N, p->N, 0, p->C, p->H, p->W, st)))) return rc;
     if (p->grad_ref && lowp &&         // fp32 gradient of a low-precision reference map, rounded once to its type
         (rc = run("gradient transposition", epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride,
-                                                                p->N, p->N, p->C, p->H, p->W, st)))) return rc;
+                                                                p->N, p->N, 0, p->C, p->H, p->W, st)))) return rc;
     g_launches = run.n;
     return EPI_OK;
 }

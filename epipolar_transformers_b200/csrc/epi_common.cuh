@@ -148,6 +148,17 @@ __device__ __forceinline__ void stage_planes_tile(float (*tile)[65], const T *s,
     }
 }
 
+// The two map items a (query, source) pair reads: every kernel maps pair p through this one function.
+//   n_views == 0: p fuses reference item p % n_ref with source item p (n_src sources per reference item: p = s·n_ref + n).
+//   n_views == V >= 2 (every view against every other): one map holds the V·n_ref view items and is both the query and the
+//   source map; p = (v·(V−1) + j)·n_ref + n fuses item v·n_ref + n with item u·n_ref + n, u = j + (j >= v).
+struct PairItems { int q, s; };
+__host__ __device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n_views) {
+    if (n_views == 0) return {p % n_ref, p};
+    const int vj = p / n_ref, n = p - vj * n_ref, v = vj / (n_views - 1), j = vj - v * (n_views - 1);
+    return {v * n_ref + n, (j + (j >= v)) * n_ref + n};
+}
+
 // Per-(ref,src)-pair constants: M = A2·A1^-1 (row-major 3x3) and the epipole e2/e2.z.
 struct PairGeom {
     float M[9];

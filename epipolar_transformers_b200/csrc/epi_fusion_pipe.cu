@@ -194,8 +194,8 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
     const int total_tiles = a.N * tiles_per_item;
     // tail balancing: the tiles of the last, partial round over the grid are handed out as half items (P/2 pixels).  How a tile
     // is split changes the union rows its pixels share, hence the order of the GEMM sums, so with several sources per reference
-    // item (n_ref < N) the split is the one a call with the n_ref pairs of a single source makes on its own grid: every source
-    // gets, bit for bit, what a separate call gives it.  A 64-pixel half costs well over half an item (the union barely shrinks),
+    // item (n_ref < N), or several view pairs (n_views), the split is the one a call with the n_ref pairs of a single source makes
+    // on its own grid: every source gets, bit for bit, what a separate call gives it.  A 64-pixel half costs well over half an item (the union barely shrinks),
     // so 64-pixel items split the last round only when it is at most half full: the halves then still fit one round.
     const int grid1 = min(a.n_ref * tiles_per_item, (int)gridDim.x);
     const int tail_tiles = a.tile_counter ? (a.n_ref * tiles_per_item) % grid1 : 0;
@@ -335,7 +335,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                         } else {
                             const float ov[4] = {o.x, o.y, o.z, o.w};
                             float *ob = a.out + (int64_t)d.n * a.out_stride[0] + (int64_t)y * a.out_stride[2] + (int64_t)x * a.out_stride[3];
-                            const int64_t rb = (int64_t)(d.n % a.n_ref) * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
+                            const int64_t rb = (int64_t)pair_items(d.n, a.n_ref, a.n_views).q * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
 #pragma unroll
                             for (int e = 0; e < 4; e++) {
                                 float val = ov[e];
@@ -906,8 +906,8 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         // =====================================================================================================
         const int gt = tid - W_GATHER * 32, gj = gt & 7, gr = gt >> 3;
         // [ref_hi | ref_lo | src_hi | src_lo] (LO) or [ref_hi | src_hi]; a lo plane follows its hi plane.  Reference planes are
-        // [n_ref*HW][C], source planes [N*HW][C] (pair n queries reference item n % n_ref)
-        const size_t plane_elems = (size_t)a.N * HW * C, ref_plane_elems = (size_t)a.n_ref * HW * C;
+        // [n_ref*HW][C], source planes [N*HW][C]; the views form has one pair of planes [n_views*n_ref*HW][C] (pair_items)
+        const size_t plane_elems = LO ? (size_t)(a.src_lo - a.src_hi) : 0, ref_plane_elems = LO ? (size_t)(a.ref_lo - a.ref_hi) : 0;
         uint32_t qcount = 0, fcount = 0;
         const bool pt_on = gt == 0; (void)pt_on;
         PT_DECL;
@@ -930,10 +930,9 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
         auto cp16 = [&](uint32_t dst, const __nv_bfloat16 *srcp, bool valid) {
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(srcp), "r"(valid ? 16 : 0) : "memory");
         };
-        auto gemm2_stages = [&](int jj) {
+        auto gemm2_stages = [&](int jj, const __nv_bfloat16 *src) {      // src: the hi plane of the item's source map
             const Desc &d = desc_at(jj);
             const int D16 = (d.D + 15) & ~15, nblk = (D16 + 63) >> 6;
-            const __nv_bfloat16 *src = a.src_hi + (size_t)d.n * HW * C;
             for (int blk = 0; blk < nblk; blk++) {               // (block of 64 union rows) outer, channel half inner: row addresses are
                 const int rows = min(64, D16 - blk * 64);        // computed once per block
                 uint32_t roff[4];
@@ -968,11 +967,12 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
             PT(15);
             const Desc &d = desc_at(j);
             const bool last = d.tile < 0;
+            const PairItems items = pair_items(d.n, a.n_ref, a.n_views);
+            const __nv_bfloat16 *src = a.src_hi + (size_t)items.s * HW * C;
             if (!last && d.D > 0) {
                 // ---- per half of the query panels (one half unless C > 256): the item's query rows as stacked panels
                 //      [hi 32 rows | lo 32 rows], then the GEMM1 stages (chunk, 64-channel panel) that multiply with them ----
                 const int D16 = (d.D + 15) & ~15, nch = (d.D + CHUNK - 1) / CHUNK;
-                const __nv_bfloat16 *src = a.src_hi + (size_t)d.n * HW * C;
                 for (int qh = 0; qh < NQH; qh++) {
                     const int npq = min(4, NP - qh * 4);
                     if (qcount >= 1) {
@@ -981,7 +981,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                     }
                     PT(16);
                     {
-                        const __nv_bfloat16 *ref = a.ref_hi + (size_t)(d.n % a.n_ref) * HW * C;
+                        const __nv_bfloat16 *ref = a.ref_hi + (size_t)items.q * HW * C;
 #pragma unroll
                         for (int it = 0; it < P / 16; it++) {           // pixel r goes to row r % 32 of query half r / 32
                             const int r = gr + 16 * it;
@@ -1028,7 +1028,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
             }
             if (gt == 0) TR(j, 2);
             if (last) break;
-            if (d.D > 0) gemm2_stages(j);                   // the workers run GEMM2(j) before GEMM1(j+1)
+            if (d.D > 0) gemm2_stages(j, src);                   // the workers run GEMM2(j) before GEMM1(j+1)
             if (gt == 0) TR(j, 8);
             named_bar(3, NGATHER);                          // every gather thread has read item j's row list
             if (gt == 0) mbar_arrive(&ct.desc_free[j % NDESC]);

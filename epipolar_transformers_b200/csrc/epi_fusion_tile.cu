@@ -89,6 +89,7 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
     const int tiles_per_item = SECTOR ? (HW + TM - 1) / TM : tiles_x * tiles_y;
     const int total_tiles = a.N * tiles_per_item;
     int n = 0, ty0 = 0, tx0 = 0;                    // current tile (persistent CTA, dynamic tile scheduler)
+    PairItems items = {0, 0};                       // its pair's query and source items
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int wg = warp >> 2, t128 = tid & 127;     // warpgroup (MMA issue unit), thread within it
     const int nwords = (HW + 31) >> 5;
@@ -122,11 +123,12 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
         } else {
             ty0 = (trem / tiles_x) * TH; tx0 = (trem % tiles_x) * TW;
         }
-        src_hi = a.src_hi + (size_t)n * HW * C; src_lo = a.src_lo + (size_t)n * HW * C;
+        items = pair_items(n, a.n_ref, a.n_views);
+        src_hi = a.src_hi + (size_t)items.s * HW * C; src_lo = a.src_lo + (size_t)items.s * HW * C;
     }
     if (tid == 32) {
         ms.sp = 1; ms.stack[0] = 0 | (TM << 8);
-        if (!a.locs_in && n != cur_n) pair_geom_from_krt(a.P_ref + 12 * (n % a.n_ref), a.P_src + 12 * n, ms.geom);
+        if (!a.locs_in && n != cur_n) pair_geom_from_krt(a.P_ref + 12 * items.q, a.P_src + 12 * items.s, ms.geom);
     }
     if (tid == 64)      // claim the next tile now; its index is consumed after this tile (hides the atomic's latency)
         ms.next_tile = a.tile_counter ? (int)gridDim.x + atomicAdd(a.tile_counter, 1) : tile + (int)gridDim.x;
@@ -228,14 +230,14 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
                     uint4 v = make_uint4(0u, 0u, 0u, 0u);
                     if (i >= g0 && i < g0 + gn && pix_ok(i) && j < C8)
                         v = __ldg(reinterpret_cast<const uint4 *>((plane ? a.ref_lo : a.ref_hi) +
-                                                                  ((size_t)(n % a.n_ref) * HW + pix_y(i) * W + pix_x(i)) * C + j * 8));
+                                                                  ((size_t)items.q * HW + pix_y(i) * W + pix_x(i)) * C + j * 8));
                     *reinterpret_cast<uint4 *>(qb + (j >> 3) * PANEL_B2 + plane * 4096u + i * 128u + (((j & 7) ^ (i & 7)) << 4)) = v;
                 }
         } else
         {
             const int i = lane;
             const bool ok = i >= g0 && i < g0 + gn && pix_ok(i);
-            const float *rb = a.feat_ref + (int64_t)(n % a.n_ref) * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
+            const float *rb = a.feat_ref + (int64_t)items.q * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
             const int64_t sc = a.ref_stride[1];
             {
                 float f[2][8];
@@ -539,7 +541,7 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
                 const int i = lane;
                 const bool ok = i >= g0 && i < g0 + gn && pix_ok(i);
                 float *ob = a.out + (int64_t)n * a.out_stride[0] + (int64_t)pix_y(i) * a.out_stride[2] + (int64_t)pix_x(i) * a.out_stride[3];
-                const float *rb = a.feat_ref + (int64_t)(n % a.n_ref) * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
+                const float *rb = a.feat_ref + (int64_t)items.q * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
                 if (ok)
                     for (int ch = warp; ch < C; ch += NWARP) {
                         float o = o_tile[i * OS + ch];
@@ -551,7 +553,7 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
                 for (int i = g0 + warp; i < g0 + gn; i += NWARP) {
                     if (!pix_ok(i)) continue;
                     float *ob = a.out + (int64_t)n * a.out_stride[0] + (int64_t)pix_y(i) * a.out_stride[2] + (int64_t)pix_x(i) * a.out_stride[3];
-                    const float *rb = a.feat_ref + (int64_t)(n % a.n_ref) * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
+                    const float *rb = a.feat_ref + (int64_t)items.q * a.ref_stride[0] + (int64_t)pix_y(i) * a.ref_stride[2] + (int64_t)pix_x(i) * a.ref_stride[3];
                     for (int ch = lane; ch < C; ch += 32) {
                         float o = o_tile[i * OS + ch];
                         if (a.add_ref) o += __ldg(rb + ch * a.ref_stride[1]);
@@ -605,14 +607,15 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
 // of (16-bit angle key << 14 | pixel index) in shared memory — unique keys, hence a deterministic order.
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) sector_order_kernel(const float *__restrict__ P_ref, const float *__restrict__ P_src,
-                                                            uint16_t *__restrict__ order, int n_ref, const GeomCfg gc) {
+                                                            uint16_t *__restrict__ order, int n_ref, int n_views, const GeomCfg gc) {
     extern __shared__ uint32_t keys[];
     __shared__ float s_e[4];          // ex, ey, a0, parallel-flag
     const int n = blockIdx.x, HW = gc.H * gc.W, W = gc.W;
     int npad = 1;
     while (npad < HW) npad <<= 1;
     if (threadIdx.x == 0) {
-        const float *P1 = P_ref + 12 * (n % n_ref), *P2 = P_src + 12 * n;
+        const PairItems items = pair_items(n, n_ref, n_views);
+        const float *P1 = P_ref + 12 * items.q, *P2 = P_src + 12 * items.s;
         double a[9], t1[3], b[9], t2[3], bi[9], cs[3], e[3];
         cam_load(P2, b, t2);
         cam_inverse(b, bi);
@@ -667,14 +670,15 @@ __global__ void __launch_bounds__(1024) sector_order_kernel(const float *__restr
     for (int i = threadIdx.x; i < HW; i += blockDim.x) order[(size_t)n * HW + i] = (uint16_t)(keys[i] & 0x3FFFu);
 }
 
-cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, const GeomCfg &gc, cudaStream_t st) {
+cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, int n_views, const GeomCfg &gc,
+                                cudaStream_t st) {
     const int HW = gc.H * gc.W;
     int npad = 1;
     while (npad < HW) npad <<= 1;
     const size_t smem = (size_t)npad * 4;
     cudaError_t e = cudaFuncSetAttribute(sector_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    sector_order_kernel<<<N, 1024, smem, st>>>(P_ref, P_src, order, n_ref, gc);
+    sector_order_kernel<<<N, 1024, smem, st>>>(P_ref, P_src, order, n_ref, n_views, gc);
     return cudaGetLastError();
 }
 

@@ -47,8 +47,9 @@ epi_fusion_warp_kernel(const FusionArgs a) {
     float *a_tile = smem + (size_t)C * 33;                   // [K][33]  attention weights
     __shared__ PairGeom s_geom;
 
-    const int nr = n % a.n_ref;                              // the pair's reference item
-    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * nr, a.P_src + 12 * n, s_geom);
+    const PairItems it = pair_items(n, a.n_ref, a.n_views);  // the pair's query and source items
+    const int nr = it.q;
+    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * nr, a.P_src + 12 * it.s, s_geom);
 
     // ---- stage the query tile: coalesced along whichever of (pixel, channel) is contiguous ----
     {
@@ -74,7 +75,7 @@ epi_fusion_warp_kernel(const FusionArgs a) {
 
     const PairGeom g = s_geom;
     const GeomCfg gc = a.geom;
-    const float *src = a.src_nhwc + (size_t)n * HW * C;
+    const float *src = a.src_nhwc + (size_t)it.s * HW * C;
     // exp(x*scale - m) as exp2(x*scale*log2e - m*log2e)
     const float sl2 = a.softmax_scale * 1.4426950408889634f;
 

@@ -1,6 +1,6 @@
 // epi_stage.cu — the ONE operand-staging launch in front of the fused attention kernel (epi_fusion_pipe.cu):
 //
-//   blocks [0, N)      per (ref, src) pair (pair n: reference item n % n_ref, source item n): fp64 pair constants (camera centre, epipole, infinite homography;
+//   blocks [0, N)      per (ref, src) pair (pair n: items pair_items(n, n_ref, n_views), epi_common.cuh): fp64 pair constants (camera centre, epipole, infinite homography;
 //                      /root/reference/vision/multiview.py:16-21, modeling/layers/epipolar.py:336-348) and the list of
 //                      reference pixels sorted by epipolar angle (counting sort on a 12-bit angle key, ties by pixel index
 //                      => deterministic).  Pixels on one epipolar line of the reference view share one epipolar line in
@@ -9,7 +9,9 @@
 //                      x ≈ hi + lo, for BOTH feature maps (reference -> planes 0,1; source -> planes 2,3 of one buffer), 64 x 64
 //                      tiles through shared memory: coalesced 4-pixel vector reads along pixels, 16-byte writes along channels.
 //                      The reference map has n_ref items and the source map N (several source views per reference item:
-//                      N = S·n_ref), so a reference tile is staged once however many sources it is fused with.
+//                      N = S·n_ref), so a reference tile is staged once however many sources it is fused with.  In the views
+//                      form (n_views = V) the reference map holds the V·n_ref view items and is the only map: each view is
+//                      staged once and serves as the query of V−1 pairs and the source of V−1 others.
 //                      fp16 values are split exactly like fp32 ones (hi + lo holds them exactly); a bf16 value is its own hi
 //                      part, so bf16 maps write hi planes only (reference -> plane 0, source -> plane 1).
 // Also zeroes the fused kernel's tile counter and error word.
@@ -70,8 +72,8 @@ struct StageArgs {
     int w_add_identity;               // ZRESIDUAL folded into the weight: planes hold Wf + I
     __nv_bfloat16 *w_planes;
     int N, C, H, W;
-    int n_ref;                        // reference items; pair n reads reference item n % n_ref
-    int ref_tiles;                    // layout tiles of the reference map (n_ref items); the source map has N items
+    int n_ref, n_views;               // pair n reads items pair_items(n, n_ref, n_views)
+    int ref_tiles;                    // layout tiles of the reference map (n_ref items, or n_views·n_ref); the source map has N items
     size_t ref_elems;                 // elements of one reference plane
     size_t src_plane0;                // offset of the source hi plane in `planes`
     int do_ref, do_src, do_order;
@@ -80,7 +82,7 @@ struct StageArgs {
 };
 
 // (min 5 blocks per SM: the layout-staging blocks need few registers; the rare order blocks may spill a little)
-// MULTI: several source views per reference item (n_ref < N).  The one-source instantiation keeps the single-map-size indexing,
+// MULTI: several source views per reference item (n_ref < N), or the views form.  The one-source instantiation keeps the single-map-size indexing,
 // so its code (and its register allocation, tight at 48 registers) does not pay for the general mapping.
 template <typename T, bool MULTI>
 __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T> s) {
@@ -108,12 +110,13 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
 #ifdef EPI_PIPE_TIMERS
         long long st_prev = clock64();
 #endif
-        const int n = blockIdx.x, nr = MULTI ? n % s.n_ref : n;         // pair, its reference item
+        const int n = blockIdx.x;                                        // pair
+        const PairItems pi = MULTI ? pair_items(n, s.n_ref, s.n_views) : PairItems{n, n};
         // cached order: the key is (P_ref, P_src, geometry configuration); an unchanged camera pair costs 32 compares
         float my_key = 0.f;
         if (t < 32) {
-            if (t < 12) my_key = s.P_ref[12 * nr + t];
-            else if (t < 24) my_key = s.P_src[12 * n + t - 12];
+            if (t < 12) my_key = s.P_ref[12 * pi.q + t];
+            else if (t < 24) my_key = s.P_src[12 * pi.s + t - 12];
             else if (t == 24) my_key = (float)H;
             else if (t == 25) my_key = (float)W;
             else if (t == 26) my_key = s.gc.ds;
@@ -130,7 +133,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
         __syncthreads();
         if (s_e[7] != 0.f) return;                               // hit: order and pair constants are already in place
         if (t == 0) {
-            const float *P1 = s.P_ref + 12 * nr, *P2 = s.P_src + 12 * n;
+            const float *P1 = s.P_ref + 12 * pi.q, *P2 = s.P_src + 12 * pi.s;
             PairGeom g;
             pair_geom_from_krt(P1, P2, g);
             s.pair_geom[n] = g;
@@ -287,7 +290,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     // layout staging: 64 channels x 64 pixels per block
     // ----------------------------------------------------------------------------------------------------
     const int tiles_p = (HW + TPX - 1) / TPX, tiles_c = (C + TC - 1) / TC;
-    const int src_tiles = tiles_p * tiles_c * s.N, ref_tiles = MULTI ? s.ref_tiles : src_tiles;
+    const int src_tiles = MULTI && !s.do_src ? 0 : tiles_p * tiles_c * s.N, ref_tiles = MULTI ? s.ref_tiles : src_tiles;
     int lin = (int)blockIdx.x - nord;
     const int wblocks = (s.Wf && s.w_planes) ? (C * C / 8 + NT - 1) / NT : 0;
     // block roles after the order blocks: [tiles | weight blocks], or with streaming blocks [weight blocks | streaming blocks]
@@ -360,6 +363,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     // reference and source tiles alternate while both remain (see below); the source tiles of the further sources follow
     // (tile index l -> map, tile of that map)
     auto split_tile = [&](int &l) -> int {
+        if (MULTI && !s.do_src) return 0;                               // the views form: one map
         if (!MULTI || l < 2 * ref_tiles) { const int mp = l & 1; l >>= 1; return mp; }
         l -= ref_tiles;
         return 1;
@@ -430,23 +434,24 @@ template <typename T>
 static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], const T *src, const int64_t src_stride[4],
                                   __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                                   float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
-                                  int n_ref, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
+                                  int n_ref, int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
     StageArgs<T> s;
     s.ref = ref; s.src = src;
     for (int i = 0; i < 4; i++) { s.ref_stride[i] = ref_stride[i]; s.src_stride[i] = src_stride[i]; }
     s.planes = planes; s.P_ref = P_ref; s.P_src = P_src; s.pair_geom = pair_geom; s.order = order; s.order_key = order_key; s.Wf = Wf; s.w_planes = w_planes; s.w_add_identity = w_add_identity;
-    s.zero_words = zero_words; s.N = N; s.n_ref = n_ref; s.C = C; s.H = H; s.W = W; s.gc = gc;
-    s.do_ref = 1; s.do_src = 1; s.do_order = (P_ref && P_src && order) ? 1 : 0; s.persist = 0;
+    s.zero_words = zero_words; s.N = N; s.n_ref = n_ref; s.n_views = n_views; s.C = C; s.H = H; s.W = W; s.gc = gc;
+    s.do_ref = 1; s.do_src = n_views ? 0 : 1; s.do_order = (P_ref && P_src && order) ? 1 : 0; s.persist = 0;
     const int tiles_pc = ((H * W + stg::TPX - 1) / stg::TPX) * ((C + stg::TC - 1) / stg::TC);
-    const int tiles = tiles_pc * n_ref + tiles_pc * N;                       // reference tiles + source tiles
-    s.ref_tiles = tiles_pc * n_ref;
-    s.ref_elems = (size_t)n_ref * H * W * C;
+    const int ref_items = n_views ? n_views * n_ref : n_ref;
+    const int tiles = tiles_pc * ref_items + (n_views ? 0 : tiles_pc * N);   // reference tiles + source tiles
+    s.ref_tiles = tiles_pc * ref_items;
+    s.ref_elems = (size_t)ref_items * H * W * C;
     s.src_plane0 = (std::is_same<T, __nv_bfloat16>::value ? 1 : 2) * s.ref_elems;
     const int wblocks = (Wf && w_planes) ? (C * C / 8 + stg::NT - 1) / stg::NT : 0;        // C % 8 == 0
     // dynamic shared memory: the transposition tile, or (order blocks) 16 KB histogram + 2 B per pixel
     const size_t smem_tile = (size_t)stg::TC * stg::TPITCH * sizeof(float);
     const size_t smem_order = (size_t)stg::NBIN * 4 + (size_t)H * W * 2;
-    const bool multi = n_ref != N;
+    const bool multi = n_ref != N || n_views;
     void (*kern)(const StageArgs<T>) = multi ? epi_stage_kernel<T, true> : epi_stage_kernel<T, false>;
     static thread_local size_t smem_set[2] = {0, 0};
     auto ensure = [&](size_t smem) -> cudaError_t {
@@ -475,7 +480,7 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
         return sd[3] == 1 && sd[2] == W && sd[1] % 4 == 0 && sd[0] % 4 == 0 && sd[1] != 1 && (reinterpret_cast<uintptr_t>(b) & (4 * sizeof(T) - 1)) == 0;
     };
     s.persist = 0;
-    if ((H * W) % stg::TPX == 0 && C % stg::TC == 0 && whole(ref, ref_stride) && whole(src, src_stride)) {
+    if ((H * W) % stg::TPX == 0 && C % stg::TC == 0 && whole(ref, ref_stride) && (n_views || whole(src, src_stride))) {
         const int slots = 5 * sm_count();                      // 5 resident blocks per SM (__launch_bounds__)
         s.persist = tiles < slots ? tiles : slots;
     }
@@ -489,15 +494,15 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
-                         int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
+                         int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
     if (dtype == kBF16)
         return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
     if (dtype == kF16)
         return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
     return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
-                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, C, H, W, gc, st, launched);
+                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
 }
 
 }  // namespace epi

@@ -1,7 +1,7 @@
 // epi_zgemm.cu — z-projection epilogue on the tensor cores (TMA + warpgroup MMA).
 //
-//   y[n,o,p] = Σ_c Wf[o,c]·x[n,c,p] + bf[o]  (+ x[n,o,p] if ZRESIDUAL)  (+ feat_ref[n % n_ref,o,p] for the caller's residual, read
-//   in the map's own element type; n_ref < N when several source views share a reference item)
+//   y[n,o,p] = Σ_c Wf[o,c]·x[n,c,p] + bf[o]  (+ x[n,o,p] if ZRESIDUAL)  (+ feat_ref[q,o,p] for the caller's residual, read in
+//   the map's own element type; q = pair_items(n, n_ref, n_views).q, the pair's query item)
 // restates  finalout = bn(z(out)) [+ out]   /root/reference/modeling/layers/epipolar.py:249-253 (eval-mode BN folded
 // into Wf, bf by epi_fold_z_bn_f32) and  ret + feat   /root/reference/modeling/backbones/resnet.py:388.
 //
@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
             res[k] = make_float4(0.f, 0.f, 0.f, 0.f);
             bias[k] = ol < CO ? __ldg(z.bf + oc0 + ol) : 0.f;      // folded bias: written long before the staging launch
             if (addr && vec && p + 3 < HW && ol < CO) {
-                const int64_t i = (int64_t)(n % z.n_ref) * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p;     // the caller's map, in its type
+                const int64_t i = (int64_t)pair_items(n, z.n_ref, z.n_views).q * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p;     // the caller's map, in its type
                 res[k] = z.ref_dtype == kBF16 ? ld4_cs(static_cast<const __nv_bfloat16 *>(z.ref) + i)
                        : z.ref_dtype == kF16  ? ld4_cs(static_cast<const __half *>(z.ref) + i)
                                               : ld4_cs(static_cast<const float *>(z.ref) + i);
@@ -160,7 +160,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
                 for (int e = 0; e < 4 && p + e < HW; e++) {
                     const int py = (p + e) / W, px = (p + e) % W;
                     float val = y[e];
-                    if (addr) val += ld_feat(z.ref, (int64_t)(n % z.n_ref) * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
+                    if (addr) val += ld_feat(z.ref, (int64_t)pair_items(n, z.n_ref, z.n_views).q * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
                     z.y[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = val;
                 }
             }

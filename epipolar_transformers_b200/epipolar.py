@@ -166,26 +166,93 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
             None if attn is None else attn.unflatten(0, (S, N)), None if locs is None else locs.unflatten(1, (S, N)))
 
 
+def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax_scale=0.125, correct_normalize=False,
+                          align_corners=False, z_folded=None, z_residual=False, add_ref_residual=False, sample_locs_in=None,
+                          want_attn=True, want_corr=True, want_locs=False, variant="auto", out=None,
+                          state: Optional[FusionState] = None):
+    """Fuses every view of a frame with every other view in one call: the whole multi-view test of the reference
+    (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239), where each of the V views takes a turn as the reference.  Each view's
+    map is staged once and serves as the query of V−1 pairs and the source of V−1 others.
+
+    feats: [V,N,C,H,W], or a sequence of V [N,C,H,W] maps (stacked), V >= 2; P: [V,N,3,4]; sample_locs_in: optional
+    [K,V,V−1,N,H,W,2]; out: optional float32 [V,V−1,N,C,H,W].  Reference view v with its j-th other view u = j + (j >= v) (the
+    other views in increasing order) gives, bit for bit, what `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every
+    residual (add_ref_residual, also under z) adds feats[v][n].  Returns
+    (out [V,V−1,N,C,H,W], corr_pos [V,V−1,N,H,W,2] | None, attn [V,V−1,N,K,H,W] | None, sample_locs [K,V,V−1,N,H,W,2] | None).
+    Inference only: inputs that require grad under grad mode raise RuntimeError."""
+    lib = _lib.load()
+    if isinstance(feats, (list, tuple)):
+        if not all(isinstance(t, torch.Tensor) for t in feats):
+            raise ValueError("feats must be a [V,N,C,H,W] tensor or a sequence of V [N,C,H,W] tensors")
+        if len({(tuple(t.shape), t.dtype, t.device) for t in feats}) > 1:
+            raise ValueError("the maps in feats must share shape, dtype and device")
+        if len(feats) < 2:
+            raise ValueError("feats needs at least two views (got %d)" % len(feats))
+        feats = torch.stack(list(feats))
+    if not isinstance(feats, torch.Tensor) or feats.dim() != 5:
+        raise ValueError("feats must be a [V,N,C,H,W] tensor or a sequence of V [N,C,H,W] tensors")
+    V, N, C, H, W = feats.shape
+    if V < 2:
+        raise ValueError("feats needs at least two views (got %d)" % V)
+    feat = feats.flatten(0, 1)                                  # [V·N,C,H,W]: item v·N + n
+    if out is not None:
+        if not isinstance(out, torch.Tensor) or tuple(out.shape) != (V, V - 1, N, C, H, W):
+            raise ValueError("out must be a [V,V-1,N,C,H,W] tensor")
+        try:
+            out4 = out.view(V * (V - 1) * N, C, H, W)
+        except RuntimeError:
+            raise ValueError("out must be viewable as [V*(V-1)*N,C,H,W]") from None
+    else:
+        out4 = None
+    if sample_locs_in is None:
+        if not isinstance(P, torch.Tensor) or tuple(P.shape) != (V, N, 3, 4):
+            raise ValueError("P must be [V,N,3,4]")
+        P = P.reshape(V * N, 3, 4)
+    else:
+        if tuple(sample_locs_in.shape) != (K, V, V - 1, N, H, W, 2):
+            raise ValueError("sample_locs_in must be [K,V,V-1,N,H,W,2]")
+        sample_locs_in = sample_locs_in.reshape(K, V * (V - 1) * N, H, W, 2)
+    dcode = _check_feat_pair(feat, feat, out4)
+    if torch.is_grad_enabled() and feat.requires_grad:
+        raise RuntimeError("epipolar_fusion_views is inference only (the views form has no backward); run it under "
+                           "torch.no_grad(), or use epipolar_fusion (one pair per call) for gradients")
+    o, corr, attn, locs = _fusion(lib, dcode, 1, feat, None, P, None, K=K, downsample=downsample, img_scale=img_scale,
+                                  softmax_scale=softmax_scale, correct_normalize=correct_normalize,
+                                  align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
+                                  add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
+                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state, views=V)
+    pairs = (V, V - 1, N)
+    return (out if out is not None else o.unflatten(0, pairs), None if corr is None else corr.unflatten(0, pairs),
+            None if attn is None else attn.unflatten(0, pairs), None if locs is None else locs.unflatten(1, pairs))
+
+
 def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, img_scale, softmax_scale, correct_normalize,
             align_corners, z_folded, z_residual, add_ref_residual, sample_locs_in, want_attn, want_corr, want_locs, variant, out,
-            state):
+            state, views=0):
     """The forward of `epipolar_fusion` (S = 1) and `epipolar_fusion_multi`: feat_ref [N,C,H,W], feat_src / out [S·N,C,H,W],
-    P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n)."""
-    N, C, H, W = feat_ref.shape
-    NP = S * N
+    P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n).
+    views = V >= 2 (`epipolar_fusion_views`): feat_ref [V·N,C,H,W] and P_ref [V·N,3,4] hold the views, feat_src and P_src are
+    None, and the outputs have V·(V−1)·N items (pair p = (v·(V−1) + j)·N + n)."""
+    NR, C, H, W = feat_ref.shape
+    N = NR // views if views else NR
+    NP = views * (views - 1) * N if views else S * N
     dev = feat_ref.device
     if sample_locs_in is None:
         if P_ref.device != dev or P_ref.dtype != torch.float32 or not P_ref.is_contiguous():
             P_ref = P_ref.to(device=dev, dtype=torch.float32).contiguous()
-        if P_src.device != dev or P_src.dtype != torch.float32 or not P_src.is_contiguous():
+        if P_src is not None and (P_src.device != dev or P_src.dtype != torch.float32 or not P_src.is_contiguous()):
             P_src = P_src.to(device=dev, dtype=torch.float32).contiguous()
-        if tuple(P_ref.shape) != (N, 3, 4) or tuple(P_src.shape) != (NP, 3, 4):
+        if tuple(P_ref.shape) != (NR, 3, 4) or (not views and tuple(P_src.shape) != (NP, 3, 4)):
             raise ValueError("P_ref/P_src must be [N,3,4]" if S == 1 else "P_ref must be [N,3,4] and P_srcs [S,N,3,4]")
     else:
         sample_locs_in = _aligned_locs(sample_locs_in.to(device=dev, dtype=torch.float32))
         if tuple(sample_locs_in.shape) != (K, NP, H, W, 2):
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
-    if out is None:
+    if out is None and views:                                            # the layout of a single call's empty_like(feat_src)
+        cl = feat_ref.dim() == 4 and feat_ref.is_contiguous(memory_format=torch.channels_last) and not feat_ref.is_contiguous()
+        out = torch.empty((NP, C, H, W), device=dev, dtype=torch.float32,
+                          memory_format=torch.channels_last if cl else torch.contiguous_format)
+    elif out is None:
         out = torch.empty_like(feat_src, dtype=torch.float32)           # preserves NCHW / channels_last
     attn = torch.empty((NP, K, H, W), device=dev, dtype=torch.float32) if want_attn else None
     corr = torch.empty((NP, H, W, 2), device=dev, dtype=torch.float32) if want_corr else None
@@ -193,15 +260,18 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
 
     vcode = _lib.VARIANTS[variant] if isinstance(variant, str) else int(variant)
     # the plan (and so the workspace size) also depends on whether `out` and feat_src start on a 16-byte boundary
-    key = (dev, S, N, C, H, W, int(K), dcode, feat_ref.stride(), feat_src.stride(), out.stride(), out.data_ptr() % 16 == 0,
-           feat_src.data_ptr() % 16 == 0, z_folded is not None, vcode,
+    src_key = (feat_src.stride(), feat_src.data_ptr() % 16 == 0) if feat_src is not None else (feat_ref.data_ptr() % 16 == 0,)
+    key = (dev, S, views, N, C, H, W, int(K), dcode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
+           z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
     if state is not None and state.key == key:
         p = state.params
     else:
         p = _lib.EpiFusionParams()
-        p.ref_stride = _strides4(feat_ref); p.src_stride = _strides4(feat_src); p.out_stride = _strides4(out)
+        p.ref_stride = _strides4(feat_ref); p.out_stride = _strides4(out)
+        if feat_src is not None:
+            p.src_stride = _strides4(feat_src)
         p.N, p.C, p.H, p.W, p.K = N, C, H, W, int(K)
         p.downsample = float(downsample); p.img_scale = float(img_scale)
         p.eps = _EPSILON; p.softmax_scale = float(softmax_scale)
@@ -210,9 +280,10 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
         p.variant = vcode
         p.feat_dtype = dcode
         p.n_src = S if S > 1 else 0
-    p.feat_ref = feat_ref.data_ptr(); p.feat_src = feat_src.data_ptr()
+        p.n_views = views
+    p.feat_ref = feat_ref.data_ptr(); p.feat_src = feat_src.data_ptr() if feat_src is not None else None
     p.P_ref = P_ref.data_ptr() if sample_locs_in is None else None
-    p.P_src = P_src.data_ptr() if sample_locs_in is None else None
+    p.P_src = P_src.data_ptr() if sample_locs_in is None and P_src is not None else None
     p.sample_locs_in = sample_locs_in.data_ptr() if sample_locs_in is not None else None
     p.out = out.data_ptr()
     p.attn = attn.data_ptr() if attn is not None else None
@@ -517,6 +588,31 @@ class Epipolar(nn.Module):
             state=self._state_for(feat1, "multi"))
         return out, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
 
+    def forward_views(self, feats, P):
+        """`forward` of every view of a frame against every other view in one fused call (the whole MULTITEST path,
+        modeling/model.py:213-239).  feats [V,N,C,H,W] or a sequence of V [N,C,H,W] maps, P [V,N,3,4].  Returns what
+        `forward(feats[v], feats[u], P[v], P[u])` returns for reference view v and its j-th other view u = j + (j >= v),
+        stacked as (finalout [V,V−1,N,C,H,W], corr_pos [V,V−1,N,H,W,2] | None, attention [V,V−1,N,K,H,W] | None,
+        sample_locs [V,V−1,N,K,H,W,2] | None).  Inference only.  With the z projection the module must be in eval mode, for the
+        reason `forward_multi` gives."""
+        cfg = self.cfg
+        ep = cfg.EPIPOLAR
+        has_z = "z" in ep.PARAMETERIZED
+        if has_z and self.training:
+            raise RuntimeError("Epipolar.forward_views with the z projection needs eval mode: training-mode BatchNorm statistics "
+                               "over V*(V-1)*N items differ from separate forward calls")
+        want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+        first = feats[0] if isinstance(feats, (list, tuple)) and feats else feats
+        out, corr, attn, locs = epipolar_fusion_views(
+            feats, P, K=self.sample_size, downsample=self.downsample,
+            img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE,
+            softmax_scale=ep.SOFTMAXSCALE, correct_normalize=ep.USE_CORRECT_NORMALIZE,
+            align_corners=self.align_corners, z_folded=self._folded() if has_z else None,
+            z_residual=bool(ep.ZRESIDUAL) if has_z else False, add_ref_residual=self.fuse_ref_residual,
+            want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
+            state=self._state_for(first, "views"))
+        return out, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
+
 
 def fused_other_feat(feat, other_features, KRT, other_KRT, sampler: Epipolar, camera=None, other_camera=None):
     """Caller-side mirror of getOtherFeat (modeling/backbones/resnet.py:377-388):
@@ -546,3 +642,27 @@ def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma
         S, N = x.shape[0], x.shape[1]
         heat = tail(x.flatten(0, 1))
         return find_tensor_peak_best(heat.unflatten(0, (S, N)), sigma, downsample)
+
+
+def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample):
+    """The reference's multi-view test (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239) for every view of a frame at once:
+    each view v is the reference in turn, is fused with each of its V−1 other views, each fusion goes through the rest of the
+    network and the peak finder, and every joint keeps the location of the other view whose peak scores highest.  All
+    V·(V−1) fusions are one `Epipolar.forward_views` call and the selection is one launch of `find_tensor_peak_best`.
+
+    feats [V,N,C,H,W] or V [N,C,H,W] maps (the views' features at the merge point), KRT [V,N,3,4]; tail, sigma and downsample
+    as for `multitest`.  Returns per view (locs [V,N,J,2], scores [V,N,J], source view [V,N,J]): the source is the camera index
+    u of the winning view, not its position j among the other views."""
+    with torch.no_grad():
+        if isinstance(feats, (list, tuple)):
+            feats = torch.stack(list(feats))
+        ret, _, _, _ = sampler.forward_views(feats, KRT)
+        V, N = feats.shape[0], feats.shape[1]
+        x = ret if sampler.fuse_ref_residual else ret + feats[:, None]    # getOtherFeat's `ret + feat` of reference view v
+        heat = tail(x.flatten(0, 2))                                       # [V·(V−1)·N, J, h, w]
+        # [V−1, V·N, J, h, w]: source slot j of every (view, item)
+        heat = heat.unflatten(0, (V, V - 1, N)).transpose(0, 1).flatten(1, 2)
+        locs, scores, j = find_tensor_peak_best(heat, sigma, downsample)
+        j = j.unflatten(0, (V, N))
+        v = torch.arange(V, device=j.device).view(V, 1, 1)
+        return locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), j + (j >= v).long()

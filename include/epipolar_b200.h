@@ -100,7 +100,18 @@ typedef struct EpiFusionParams {
                                      Every residual (add_ref_residual, also under the z epilogue) reads feat_ref[n]; z_residual
                                      adds pair p's own fused feature.  The reference map is staged once for all S sources.
                                      The cfg.EPIPOLAR.MULTITEST path of the reference (modeling/model.py:213-239) in one call. */
-    int32_t reserved[1];
+    union {
+    int32_t reserved[1];          /* the name of this word before n_views (ABI v3 as first released) */
+    int32_t n_views;              /* 0: the forms above.  V >= 2 (the views form; only where epi_fusion_views() returns 1): every view
+                                     of a frame against every other, in one call.  feat_ref (ref_stride) is logical [V·N,C,H,W] and
+                                     P_ref [V·N,3,4]: item v·N + n is view v of batch item n.  feat_src and P_src must be NULL and
+                                     n_src 0 or 1; anything else (and n_views = 1 or < 0) is EPI_EINVAL.  Pair
+                                     p = (v·(V−1) + j)·N + n (0 <= j < V−1) fuses query item v·N + n with source item u·N + n,
+                                     u = j + (j >= v): the other views in increasing order.  out, attn, corr_pos have V·(V−1)·N items
+                                     and sample_locs_in / sample_locs_out are [K,V·(V−1)·N,H,W,2].  Every residual reads the pair's
+                                     query item.  Each pair's outputs are bit for bit those of a one-source call on (view v, view u);
+                                     each view's map is staged once, as the query of V−1 pairs and the source of V−1 others. */
+    };
     /* ---- optional persistent state (ABI v2) -------------------------------------------- */
     void *cache;                  /* device memory the caller keeps alive ACROSS calls and zero-fills once, or NULL.  Holds the
                                      per-pair constants and the epipolar pixel order keyed by (P_ref, P_src, H, W, downsample,
@@ -116,10 +127,11 @@ int epi_version(void);
 const char *epi_last_error(void);
 
 /* Bytes of scratch the forward needs for these shapes/strides/flags (0 is possible).  With n_src > 1 it covers N reference items
- * and S·N source items and pairs. */
+ * and S·N source items and pairs; with n_views = V, V·N view items and V·(V−1)·N pairs. */
 size_t epi_fusion_workspace_bytes(const EpiFusionParams *p);
 
-/* Bytes of the optional persistent cache for these shapes (0 when the selected kernel keeps no cross-call state); S·N pairs. */
+/* Bytes of the optional persistent cache for these shapes (0 when the selected kernel keeps no cross-call state); S·N pairs, or
+ * V·(V−1)·N with n_views = V. */
 size_t epi_fusion_cache_bytes(const EpiFusionParams *p);
 
 /* The fused forward: geometry + K bilinear taps + softmax(QK)·V (+ z/BN epilogue, + residuals).
@@ -166,6 +178,9 @@ size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p);
 int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream);
 /* 1: this library honours EpiFusionBwdParams.deterministic (a library built before the field read it as a reserved word). */
 int epi_fusion_backward_deterministic(void);
+/* 1: this library honours EpiFusionParams.n_views (a library built before the field read it as a reserved word and would run a
+ * one-source call). */
+int epi_fusion_views(void);
 
 /* Only the geometry: sample locations [K,N,H,W,2] for (P_ref,P_src)  (grid2sample_locs). */
 int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_locs_out, int32_t N,
