@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libepipolar_b200.so")
 
 EPI_ABI_VERSION = 3
 EPI_DTYPE_F32, EPI_DTYPE_BF16, EPI_DTYPE_F16 = 0, 1, 2
+EPI_VIEW_SOURCES_MAX = 256          # V·S entries of a source table (include/epipolar_b200.h)
 EPI_VARIANT_AUTO, EPI_VARIANT_WARP, EPI_VARIANT_TILE, EPI_VARIANT_SECTOR, EPI_VARIANT_PIPE = 0, 1, 2, 3, 4
 VARIANTS = {"auto": EPI_VARIANT_AUTO, "warp": EPI_VARIANT_WARP, "tile": EPI_VARIANT_TILE, "sector": EPI_VARIANT_SECTOR,
             "pipe": EPI_VARIANT_PIPE}
@@ -21,7 +22,12 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_fusion_backward_workspace_bytes", "epi_fusion_backward_f32", "epi_find_peaks_f32", "epi_find_peaks_best_f32",
            "epi_sample_locs_f32", "epi_fold_z_bn_f32", "epi_last_launch_count", "epi_umma_selftest",
            "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3",
-           "epi_fusion_backward_deterministic", "epi_fusion_views")
+           "epi_fusion_backward_deterministic", "epi_fusion_views", "epi_fusion_view_sources_forward_f32",
+           "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources")
+# The source-table entry points are new symbols, not a reinterpreted field, so a library without them still runs every other
+# form correctly: load() accepts it, and only a call with a source table needs them (`require_view_sources`).
+VIEW_SOURCES_EXPORTS = ("epi_fusion_view_sources_forward_f32", "epi_fusion_view_sources_workspace_bytes",
+                        "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources")
 
 _fp = ctypes.POINTER(ctypes.c_float)
 
@@ -87,7 +93,7 @@ def load():
             "epipolar_transformers_b200: CUDA library %s is missing. Build it with "
             "`python -m epipolar_transformers_b200.build` (needs nvcc). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    missing = [s for s in EXPORTS if not hasattr(lib, s)]
+    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS and not hasattr(lib, s)]
     if missing:
         # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
         # (a views call would silently run as a one-source call)
@@ -129,11 +135,28 @@ def load():
     lib.epi_kernel_timing_last3.argtypes = [ctypes.POINTER(ctypes.c_float)]
     lib.epi_fusion_backward_deterministic.restype = ctypes.c_int
     lib.epi_fusion_views.restype = ctypes.c_int
+    if all(hasattr(lib, s) for s in VIEW_SOURCES_EXPORTS):
+        table = [ctypes.POINTER(EpiFusionParams), ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]
+        lib.epi_fusion_view_sources_forward_f32.restype = ctypes.c_int
+        lib.epi_fusion_view_sources_forward_f32.argtypes = table + [ctypes.c_void_p]
+        lib.epi_fusion_view_sources_workspace_bytes.restype = ctypes.c_size_t
+        lib.epi_fusion_view_sources_workspace_bytes.argtypes = table
+        lib.epi_fusion_view_sources_cache_bytes.restype = ctypes.c_size_t
+        lib.epi_fusion_view_sources_cache_bytes.argtypes = table
+        lib.epi_fusion_view_sources.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))
     _lib = lib
     return lib
+
+
+def require_view_sources(lib):
+    """Raise unless `lib` has the source-table form of the views call (epi_fusion_view_sources())."""
+    missing = [s for s in VIEW_SOURCES_EXPORTS if not hasattr(lib, s)]
+    if missing or lib.epi_fusion_view_sources() != 1:
+        raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot fuse views with a source table; rebuild it with "
+                           "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_view_sources"]))
 
 
 def check(rc: int, what: str):

@@ -47,14 +47,20 @@ struct Launches {
 
 // source views per reference item (EpiFusionParams.n_src: 0 and 1 both mean one)
 inline int n_sources(const EpiFusionParams *p) { return p->n_src > 1 ? p->n_src : 1; }
-// (query, source) pairs = items of out, attn, corr_pos and the sample locations: S·N, or V·(V−1)·N in the views form
-inline int64_t n_pairs64(const EpiFusionParams *p) {
-    return p->n_views ? (int64_t)p->n_views * (p->n_views - 1) * p->N : (int64_t)n_sources(p) * p->N;
+// The views form's source table: every other view (S = 0) for epi_fusion_forward_f32, the caller's table for the
+// epi_fusion_view_sources_* entry points
+static_assert(EPI_VIEW_SOURCES_MAX == epi::kMaxViewSources, "the header's table limit is the kernels' by-value table size");
+const epi::ViewSources kAllOthers{};
+// sources per view in the views form: the table's width, or V−1
+inline int view_sources(const EpiFusionParams *p, const epi::ViewSources &vs) { return vs.S ? vs.S : p->n_views - 1; }
+// (query, source) pairs = items of out, attn, corr_pos and the sample locations: S·N, or V·S·N in the views form
+inline int64_t n_pairs64(const EpiFusionParams *p, const epi::ViewSources &vs) {
+    return p->n_views ? (int64_t)p->n_views * view_sources(p, vs) * p->N : (int64_t)n_sources(p) * p->N;
 }
-inline int n_pairs(const EpiFusionParams *p) { return (int)n_pairs64(p); }
+inline int n_pairs(const EpiFusionParams *p, const epi::ViewSources &vs) { return (int)n_pairs64(p, vs); }
 // The views form (n_views = V) has one map, feat_ref with its V·N view items, that is both the query and the source map.
 inline int n_ref_items(const EpiFusionParams *p) { return p->n_views ? p->n_views * p->N : p->N; }
-inline int n_src_items(const EpiFusionParams *p) { return p->n_views ? p->n_views * p->N : n_pairs(p); }
+inline int n_src_items(const EpiFusionParams *p) { return p->n_views ? p->n_views * p->N : n_sources(p) * p->N; }
 inline const void *src_map(const EpiFusionParams *p) { return p->n_views ? p->feat_ref : p->feat_src; }
 inline const int64_t *src_strides(const EpiFusionParams *p) { return p->n_views ? p->ref_stride : p->src_stride; }
 
@@ -106,11 +112,11 @@ bool want_tile(const EpiFusionParams *p) {
 // Sizes: `ref_map` is one fp32 copy of the N reference items, `map` one fp32 map of the S·N pairs (source items, fused features).
 // The reference planes are staged once however many sources they are fused with.  One bf16 plane of a map is half its fp32 bytes.
 // The views form stages its V·N items once (`ref_map`): they are both the query and the source planes, and `map` covers the
-// V·(V−1)·N pairs' fused features only.
-Plan make_plan(const EpiFusionParams *p) {
+// V·S·N pairs' fused features only.
+Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
     Plan pl;
     const bool views = p->n_views != 0;
-    const size_t NP = (size_t)n_pairs(p), px = (size_t)p->H * p->W;
+    const size_t NP = (size_t)n_pairs(p, vs), px = (size_t)p->H * p->W;
     const size_t ref_map = (size_t)n_ref_items(p) * p->C * px * sizeof(float), map = NP * p->C * px * sizeof(float);
     const size_t src_map_bytes = (size_t)n_src_items(p) * p->C * px * sizeof(float);
     const size_t order_bytes = NP * px * sizeof(uint16_t), geom_bytes = NP * sizeof(epi::PairGeom);
@@ -186,12 +192,31 @@ Plan make_plan(const EpiFusionParams *p) {
 inline bool aligned8(const void *q) { return reinterpret_cast<uintptr_t>(q) % 8 == 0; }
 
 // the size queries answer 0 for params no plan is made for
-bool plannable(const EpiFusionParams *p) {
+bool plannable(const EpiFusionParams *p, const epi::ViewSources &vs) {
     return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0 &&
-           (p->n_views == 0 || (p->n_views >= 2 && p->n_views <= 256 && p->n_src <= 1 && n_pairs64(p) <= 65535));
+           (p->n_views == 0 || (p->n_views >= 2 && p->n_views <= 256 && p->n_src <= 1 && n_pairs64(p, vs) <= 65535));
 }
 
-int validate(const EpiFusionParams *p) {
+// Reads the caller's [V][S] host table into `vs` (the kernels' by-value copy).  Returns null, or why the table is refused.
+const char *read_view_table(const EpiFusionParams *p, const int32_t *sources, int32_t S, epi::ViewSources &vs, char *msg, size_t len) {
+    if (!p) return "params is null";
+    if (!sources) return "sources_host is null";
+    if (S < 1) return "S (sources per view) must be >= 1";
+    const int V = p->n_views;
+    if (V < 2) return "the source-table form needs n_views >= 2 (the views of a frame)";
+    if ((int64_t)V * S > EPI_VIEW_SOURCES_MAX)
+        return "n_views * S must be <= EPI_VIEW_SOURCES_MAX (256): the table travels in the kernels' launch parameters";
+    vs.S = S;
+    for (int i = 0; i < V * S; i++) {
+        const int32_t u = sources[i];
+        if (u < 0 || u >= V) { snprintf(msg, len, "sources[%d][%d] = %d is not a view in [0, %d)", i / S, i % S, (int)u, V); return msg; }
+        if (u == i / S) { snprintf(msg, len, "sources[%d][%d] = %d pairs view %d with itself", i / S, i % S, (int)u, (int)u); return msg; }
+        vs.src[i] = (uint8_t)u;
+    }
+    return nullptr;
+}
+
+int validate(const EpiFusionParams *p, const epi::ViewSources &vs) {
     if (!p) return fail(EPI_EINVAL, "params is null");
     if (p->n_views < 0 || p->n_views == 1) return fail(EPI_EINVAL, "n_views must be 0 or >= 2 (every view against every other)");
     if (p->n_views) {
@@ -214,8 +239,8 @@ int validate(const EpiFusionParams *p) {
     if (p->n_src > 1 || p->n_views) {
         // the layout, transposition and z epilogue kernels put the item in the grid's z dimension; the pipelined kernel numbers
         // its per-pair work records, and the staging kernel its tiles, in 32-bit ints
-        const int64_t np = p->n_views > 256 ? INT64_MAX : n_pairs64(p), hw = (int64_t)p->H * p->W;
-        if (np > 65535) return fail(EPI_EINVAL, "pairs (n_src * N, or n_views * (n_views - 1) * N) must be <= 65535 (grid z dimension of the per-item kernels)");
+        const int64_t np = p->n_views > 256 ? INT64_MAX : n_pairs64(p, vs), hw = (int64_t)p->H * p->W;
+        if (np > 65535) return fail(EPI_EINVAL, "pairs (n_src * N, or n_views * S * N with S = n_views - 1 or the table's width) must be <= 65535 (grid z dimension of the per-item kernels)");
         if (np * ((hw + 31) / 32 + 1) + np / p->N * 256 > INT32_MAX || 2 * np * ((hw + 63) / 64) * ((p->C + 63) / 64) > INT32_MAX || np * hw > INT32_MAX)
             return fail(EPI_EINVAL, "pairs * H * W too large: per-pair work records and staging tiles are counted in int32");
     }
@@ -289,6 +314,8 @@ int epi_fusion_backward_deterministic(void) { return 1; }
 
 int epi_fusion_views(void) { return 1; }
 
+int epi_fusion_view_sources(void) { return 1; }
+
 int epi_kernel_timing_enable(int on) { g_timing = on ? 1 : 0; return EPI_OK; }
 
 // Not declared in the public header: forces the pipe kernel's 32-pixel work items on every shape (on = 1) or restores the
@@ -313,15 +340,21 @@ float epi_kernel_timing_last_ms(void) {
     return ms;
 }
 
-size_t epi_fusion_cache_bytes(const EpiFusionParams *p) { return plannable(p) ? make_plan(p).cache_bytes : 0; }
+size_t epi_fusion_cache_bytes(const EpiFusionParams *p) { return plannable(p, kAllOthers) ? make_plan(p, kAllOthers).cache_bytes : 0; }
 
-size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) { return plannable(p) ? make_plan(p).workspace_bytes : 0; }
+size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) {
+    return plannable(p, kAllOthers) ? make_plan(p, kAllOthers).workspace_bytes : 0;
+}
 
-int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
-    int rc = validate(p);
+}  // extern "C"
+
+namespace {
+
+int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) {
+    int rc = validate(p, vs);
     if (rc != EPI_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const Plan pl = make_plan(p);
+    const Plan pl = make_plan(p, vs);
     void *ws = p->workspace;
     if (pl.workspace_bytes > 0 && (!ws || p->workspace_bytes < pl.workspace_bytes)) return fail(EPI_EWORKSPACE, "workspace too small");
     if (pl.workspace_bytes > 0 && reinterpret_cast<uintptr_t>(ws) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
@@ -337,7 +370,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     }
 
     const int dt = p->feat_dtype;
-    const int NP = n_pairs(p);          // pairs: items of every output (and of feat_src unless n_views)
+    const int NP = n_pairs(p, vs);      // pairs: items of every output (and of feat_src unless n_views)
     const int NR = n_ref_items(p), V = p->n_views;
     const float *P_src = V ? p->P_ref : p->P_src;      // the views form takes both cameras of a pair from P_ref
     epi::FusionArgs a;
@@ -374,7 +407,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         int kernels = 0;
         const cudaError_t e = epi::launch_stage(p->feat_ref, p->ref_stride, p->feat_src, p->src_stride, dt, at<__nv_bfloat16>(ws, pl.ref_hi),
                                                 p->P_ref, P_src, pg, order, okey, w_hi ? p->z_weight_folded : nullptr, w_hi,
-                                                p->z_residual ? 1 : 0, words, NP, p->N, V, p->C, p->H, p->W, a.geom, st, kernels);
+                                                p->z_residual ? 1 : 0, words, NP, p->N, V, vs, p->C, p->H, p->W, a.geom, st, kernels);
         if ((rc = run("operand staging", e, kernels))) return rc;
         a.ref_hi = at<__nv_bfloat16>(ws, pl.ref_hi); a.ref_lo = at<__nv_bfloat16>(ws, pl.ref_lo);
         a.src_hi = V ? a.ref_hi : at<__nv_bfloat16>(ws, pl.src_hi); a.src_lo = V ? a.ref_lo : at<__nv_bfloat16>(ws, pl.src_lo);
@@ -391,7 +424,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
             uint16_t *order = at<uint16_t>(ws, pl.order);
             if (!V && (rc = run("reference staging", epi::launch_split_planes(a.feat_ref, a.ref_stride, rhi, rlo, p->N, p->C, p->H, p->W, nullptr, EPI_DTYPE_F32, st))))
                 return rc;
-            if ((rc = run("sector ordering", epi::launch_sector_order(p->P_ref, P_src, order, NP, p->N, V, a.geom, st)))) return rc;
+            if ((rc = run("sector ordering", epi::launch_sector_order(p->P_ref, P_src, order, NP, p->N, V, vs, a.geom, st)))) return rc;
             a.ref_hi = rhi; a.ref_lo = rlo; a.order = order;
         }
     } else if (pl.staging == Staging::Nhwc) {
@@ -416,8 +449,8 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
     }
 
     if (g_timing) cudaEventRecord(g_ev0, st);
-    const cudaError_t e = pl.kernel == Kernel::Pipe ? epi::launch_fusion_pipe(a, st)
-                        : pl.kernel == Kernel::Warp ? epi::launch_fusion_warp(a, st) : epi::launch_fusion_tile(a, st);
+    const cudaError_t e = pl.kernel == Kernel::Pipe ? epi::launch_fusion_pipe(a, vs, st)
+                        : pl.kernel == Kernel::Warp ? epi::launch_fusion_warp(a, vs, st) : epi::launch_fusion_tile(a, vs, st);
     if ((rc = run("fusion kernel", e))) return rc;
     if (g_timing) cudaEventRecord(g_ev1, st);
 
@@ -426,7 +459,7 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, NR, p->C, p->H, p->W, dt, st)))) return rc;
     if (pl.epilogue == Epilogue::Unstage) {
         if ((rc = run("output transposition", epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out,
-                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, V, p->C, p->H, p->W, st)))) return rc;
+                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, V, vs, p->C, p->H, p->W, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZGemm) {
         epi::ZGemmArgs z;
         memset(&z, 0, sizeof(z));
@@ -436,20 +469,45 @@ int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) {
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
         z.N = NP; z.n_ref = p->N; z.n_views = V; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
-        if ((rc = run("z GEMM", epi::launch_zgemm(z, st)))) return rc;
+        if ((rc = run("z GEMM", epi::launch_zgemm(z, vs, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZFp32) {
         epi::ZArgs z;
         memset(&z, 0, sizeof(z));
         z.x = a.out;
         for (int i = 0; i < 4; i++) { z.x_stride[i] = a.out_stride[i]; z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = ref32 ? cl_stride[i] : p->ref_stride[i]; }
         z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
-        z.N = NP; z.n_ref = p->N; z.n_views = V; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
+        z.N = NP; z.n_ref = p->N; z.n_views = V; z.vsrc = vs; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         if ((rc = run("z epilogue", epi::launch_z_epilogue(z, st)))) return rc;
     }
     if (g_timing) { cudaEventRecord(g_evB, st); g_timing_valid = 1; }
     g_launches = run.n;
     return EPI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int epi_fusion_forward_f32(const EpiFusionParams *p, void *stream) { return forward(p, kAllOthers, stream); }
+
+size_t epi_fusion_view_sources_workspace_bytes(const EpiFusionParams *p, const int32_t *sources_host, int32_t S) {
+    epi::ViewSources vs{};
+    char msg[128];
+    return !read_view_table(p, sources_host, S, vs, msg, sizeof(msg)) && plannable(p, vs) ? make_plan(p, vs).workspace_bytes : 0;
+}
+
+size_t epi_fusion_view_sources_cache_bytes(const EpiFusionParams *p, const int32_t *sources_host, int32_t S) {
+    epi::ViewSources vs{};
+    char msg[128];
+    return !read_view_table(p, sources_host, S, vs, msg, sizeof(msg)) && plannable(p, vs) ? make_plan(p, vs).cache_bytes : 0;
+}
+
+int epi_fusion_view_sources_forward_f32(const EpiFusionParams *p, const int32_t *sources_host, int32_t S, void *stream) {
+    epi::ViewSources vs{};
+    char msg[128];
+    if (const char *why = read_view_table(p, sources_host, S, vs, msg, sizeof(msg))) return fail(EPI_EINVAL, "%s", why);
+    return forward(p, vs, stream);
 }
 
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p) {
@@ -503,10 +561,10 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     }
     if (p->grad_src &&
         (rc = run("gradient transposition", epi::launch_unstage(dsrc, nullptr, EPI_DTYPE_F32, p->gsrc_stride, p->grad_src, dt, p->gsrc_stride,
-                                                                p->N, p->N, 0, p->C, p->H, p->W, st)))) return rc;
+                                                                p->N, p->N, 0, kAllOthers, p->C, p->H, p->W, st)))) return rc;
     if (p->grad_ref && lowp &&         // fp32 gradient of a low-precision reference map, rounded once to its type
         (rc = run("gradient transposition", epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride,
-                                                                p->N, p->N, 0, p->C, p->H, p->W, st)))) return rc;
+                                                                p->N, p->N, 0, kAllOthers, p->C, p->H, p->W, st)))) return rc;
     g_launches = run.n;
     return EPI_OK;
 }

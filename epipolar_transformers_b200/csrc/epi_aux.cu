@@ -80,11 +80,12 @@ cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_b
 template <typename TO, typename TR>
 __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ pm, const TR *__restrict__ ref, int64_t rn,
                                                       int64_t rc, int64_t rh, int64_t rw, TO *__restrict__ out, int64_t on,
-                                                      int64_t oc, int64_t oh, int64_t ow, int n_ref, int n_views, int C, int H, int W) {
+                                                      int64_t oc, int64_t oh, int64_t ow, int n_ref, int n_views, const ViewSources vs,
+                                                      int C, int H, int W) {
     __shared__ float tile[64][65];                              // [channel][pixel]
     const int HW = H * W, t = threadIdx.x;
     const int n = blockIdx.z, c0 = blockIdx.y * 64, p0 = blockIdx.x * 64;
-    const int64_t rofs = (int64_t)pair_items(n, n_ref, n_views).q * rn;      // the item's reference (several pairs may share one)
+    const int64_t rofs = (int64_t)pair_items(n, n_ref, n_views, vs).q * rn;      // the item's reference (several pairs may share one)
     {
         const int q = t & 15, pl = t >> 4;                      // 16 float4 per pixel row (64 channels), 16 pixels per pass
 #pragma unroll
@@ -129,21 +130,22 @@ __global__ void __launch_bounds__(256) unstage_kernel(const float *__restrict__ 
 
 template <typename TO, typename TR>
 static void unstage_t(dim3 grid, cudaStream_t st, const float *pm, const void *ref, const int64_t ref_stride[4], void *out,
-                      const int64_t out_stride[4], int n_ref, int n_views, int C, int H, int W) {
+                      const int64_t out_stride[4], int n_ref, int n_views, const ViewSources &vs, int C, int H, int W) {
     unstage_kernel<TO, TR><<<grid, 256, 0, st>>>(pm, static_cast<const TR *>(ref), ref ? ref_stride[0] : 0, ref ? ref_stride[1] : 0,
                                                  ref ? ref_stride[2] : 0, ref ? ref_stride[3] : 0, static_cast<TO *>(out), out_stride[0],
-                                                 out_stride[1], out_stride[2], out_stride[3], n_ref, n_views, C, H, W);
+                                                 out_stride[1], out_stride[2], out_stride[3], n_ref, n_views, vs, C, H, W);
 }
 
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
-                           const int64_t out_stride[4], int N, int n_ref, int n_views, int C, int H, int W, cudaStream_t st) {
+                           const int64_t out_stride[4], int N, int n_ref, int n_views, const ViewSources &vs, int C, int H, int W,
+                           cudaStream_t st) {
     dim3 grid((H * W + 63) / 64, (C + 63) / 64, N);
     if (out_dtype != kF32 && ref) return cudaErrorInvalidValue;           // a low-precision output is a gradient: no residual
-    if (out_dtype == kBF16) unstage_t<__nv_bfloat16, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, C, H, W);
-    else if (out_dtype == kF16) unstage_t<__half, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, C, H, W);
-    else if (ref_dtype == kBF16) unstage_t<float, __nv_bfloat16>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, C, H, W);
-    else if (ref_dtype == kF16) unstage_t<float, __half>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, C, H, W);
-    else unstage_t<float, float>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, C, H, W);
+    if (out_dtype == kBF16) unstage_t<__nv_bfloat16, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else if (out_dtype == kF16) unstage_t<__half, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else if (ref_dtype == kBF16) unstage_t<float, __nv_bfloat16>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else if (ref_dtype == kF16) unstage_t<float, __half>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else unstage_t<float, float>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
     return cudaGetLastError();
 }
 
@@ -196,7 +198,8 @@ cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, c
 // ------------------------------------------------------------------------------------------
 constexpr int ZT = 64, ZK = 16;
 
-__global__ void __launch_bounds__(256) z_epilogue_kernel(const ZArgs z) {
+// (min 5 blocks per SM: 48 registers.  Unbounded, ptxas spends 64 on the source-table branch of pair_items and a block fewer fits.)
+__global__ void __launch_bounds__(256, 5) z_epilogue_kernel(const ZArgs z) {
     __shared__ float Ws[ZK][ZT + 1];     // [k][o]
     __shared__ float Xs[ZK][ZT + 1];     // [k][p]
     const int n = blockIdx.z, o0 = blockIdx.y * ZT, p0 = blockIdx.x * ZT;
@@ -231,7 +234,7 @@ __global__ void __launch_bounds__(256) z_epilogue_kernel(const ZArgs z) {
         __syncthreads();
     }
     float *Y = z.y + (int64_t)n * z.y_stride[0];
-    const float *R = z.ref ? z.ref + (int64_t)pair_items(n, z.n_ref, z.n_views).q * z.ref_stride[0] : nullptr;
+    const float *R = z.ref ? z.ref + (int64_t)pair_items(n, z.n_ref, z.n_views, z.vsrc).q * z.ref_stride[0] : nullptr;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         int o = o0 + ty * 4 + i;

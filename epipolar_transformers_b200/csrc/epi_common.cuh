@@ -148,15 +148,30 @@ __device__ __forceinline__ void stage_planes_tile(float (*tile)[65], const T *s,
     }
 }
 
+// The source table of the views form (EPI_VIEW_SOURCES_MAX in the header): view v is fused with views src[v·S + j], j < S.
+// S = 0 is the all-others form (u = j + (j >= v), no table).  Kernels take it by value in their arguments, so a table reaches
+// them in the launch's parameter block: no copy to the device, no synchronisation.  Indexed reads compile to constant-bank loads.
+constexpr int kMaxViewSources = 256;
+struct ViewSources { int S; uint8_t src[kMaxViewSources]; };
+
 // The two map items a (query, source) pair reads: every kernel maps pair p through this one function.
 //   n_views == 0: p fuses reference item p % n_ref with source item p (n_src sources per reference item: p = s·n_ref + n).
-//   n_views == V >= 2 (every view against every other): one map holds the V·n_ref view items and is both the query and the
-//   source map; p = (v·(V−1) + j)·n_ref + n fuses item v·n_ref + n with item u·n_ref + n, u = j + (j >= v).
+//   n_views == V >= 2: one map holds the V·n_ref view items and is both the query and the source map; with S sources per view
+//   (vs.S, or V−1 for the all-others form), p = (v·S + j)·n_ref + n fuses item v·n_ref + n with item u·n_ref + n, where
+//   u = vs.src[v·S + j], or u = j + (j >= v) (the other views in increasing order) when vs.S == 0.
+// Without `vs`: the forms that have no table.  The staging, pipelined and z GEMM kernels take the table as a trailing parameter
+// pack (`const Tab... vs`) that is empty unless the call has a table, so the one-source, several-source and all-others forms
+// launch them with no table bytes and no table code; the other kernels take a ViewSources and test vs.S at run time.
 struct PairItems { int q, s; };
 __host__ __device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n_views) {
     if (n_views == 0) return {p % n_ref, p};
     const int vj = p / n_ref, n = p - vj * n_ref, v = vj / (n_views - 1), j = vj - v * (n_views - 1);
     return {v * n_ref + n, (j + (j >= v)) * n_ref + n};
+}
+__host__ __device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n_views, const ViewSources &vs) {
+    if (n_views == 0 || vs.S == 0) return pair_items(p, n_ref, n_views);
+    const int vj = p / n_ref, n = p - vj * n_ref;
+    return {vj / vs.S * n_ref + n, (int)vs.src[vj] * n_ref + n};
 }
 
 // Per-(ref,src)-pair constants: M = A2·A1^-1 (row-major 3x3) and the epipole e2/e2.z.

@@ -175,8 +175,9 @@ __device__ unsigned long long g_pipe_cta[256 * 4];     // per CTA: globaltimer a
 // on every ring stage (GEMM1: row half wg & 1 of the chunk against query half wg >> 1; GEMM2: channel block wg & 1 of the stage
 // for pixel half wg >> 1), and the softmax phase runs once per half with the 32-pixel code.  The host picks 64 for maps of at
 // most 64 pixels a side with C <= 256, whose 64-pixel unions stay within DMAX rows.
-template <int KPL, bool LO, int P>
-__global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const FusionArgs a) {
+// vs: the source table of a table call, else empty (pair_items)
+template <int KPL, bool LO, int P, typename... Tab>
+__global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const FusionArgs a, const Tab... vs) {
     using Desc = ItemDesc<P>;
     using L = Layout<P>;
     constexpr int NSTAGE = L::NSTAGE;
@@ -335,7 +336,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
                         } else {
                             const float ov[4] = {o.x, o.y, o.z, o.w};
                             float *ob = a.out + (int64_t)d.n * a.out_stride[0] + (int64_t)y * a.out_stride[2] + (int64_t)x * a.out_stride[3];
-                            const int64_t rb = (int64_t)pair_items(d.n, a.n_ref, a.n_views).q * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
+                            const int64_t rb = (int64_t)pair_items(d.n, a.n_ref, a.n_views, vs...).q * a.ref_stride[0] + (int64_t)y * a.ref_stride[2] + (int64_t)x * a.ref_stride[3];
 #pragma unroll
                             for (int e = 0; e < 4; e++) {
                                 float val = ov[e];
@@ -967,7 +968,7 @@ __global__ void __launch_bounds__(NT_ALL, 1) epi_fusion_pipe_kernel(const Fusion
             PT(15);
             const Desc &d = desc_at(j);
             const bool last = d.tile < 0;
-            const PairItems items = pair_items(d.n, a.n_ref, a.n_views);
+            const PairItems items = pair_items(d.n, a.n_ref, a.n_views, vs...);
             const __nv_bfloat16 *src = a.src_hi + (size_t)items.s * HW * C;
             if (!last && d.D > 0) {
                 // ---- per half of the query panels (one half unless C > 256): the item's query rows as stacked panels
@@ -1074,14 +1075,15 @@ bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in) {
 // (at most 232 at K = 128 on the benchmark's cameras; a larger one splits into its 32-pixel halves).
 int fusion_pipe_item_pixels(int C, int H, int W) { return (H > W ? H : W) <= 64 && C <= 256 ? 64 : 32; }
 
-template <int P>
-static cudaError_t launch_items(const FusionArgs &a, cudaStream_t st) {
+template <int P, typename... Tab>
+static cudaError_t launch_items(const FusionArgs &a, cudaStream_t st, const Tab &... vs) {
     const int HW = a.geom.H * a.geom.W;
     const int tiles = a.N * ((HW + P - 1) / P);
     const int kpl = (a.geom.K + 31) / 32;
     const bool lo = a.src_lo != nullptr;
-    void (*kern)(const FusionArgs) = lo ? (kpl <= 1 ? epi_fusion_pipe_kernel<1, true, P> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, true, P> : epi_fusion_pipe_kernel<4, true, P>))
-                                        : (kpl <= 1 ? epi_fusion_pipe_kernel<1, false, P> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, false, P> : epi_fusion_pipe_kernel<4, false, P>));
+    void (*kern)(const FusionArgs, const Tab...) =
+        lo ? (kpl <= 1 ? epi_fusion_pipe_kernel<1, true, P, Tab...> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, true, P, Tab...> : epi_fusion_pipe_kernel<4, true, P, Tab...>))
+           : (kpl <= 1 ? epi_fusion_pipe_kernel<1, false, P, Tab...> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, false, P, Tab...> : epi_fusion_pipe_kernel<4, false, P, Tab...>));
     static thread_local bool attr_set[6] = {false, false, false, false, false, false};
     const int ki = (kpl <= 1 ? 0 : (kpl <= 2 ? 1 : 2)) + (lo ? 0 : 3);
     if (!attr_set[ki]) {
@@ -1091,12 +1093,13 @@ static cudaError_t launch_items(const FusionArgs &a, cudaStream_t st) {
     }
     const int sms = sm_count();
     const int grid = tiles < sms ? tiles : sms;                    // one persistent CTA per SM
-    cudaError_t le = launch_pdl(kern, dim3((unsigned)grid), dim3(NT_ALL), (size_t)smem_alloc<P>(), st, a);
+    cudaError_t le = launch_pdl(kern, dim3((unsigned)grid), dim3(NT_ALL), (size_t)smem_alloc<P>(), st, a, vs...);
     if (le != cudaSuccess) return le;
     return cudaGetLastError();
 }
 
-cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st) {
+cudaError_t launch_fusion_pipe(const FusionArgs &a, const ViewSources &vs, cudaStream_t st) {
+    if (vs.S) return a.item_px == 64 ? launch_items<64>(a, st, vs) : launch_items<32>(a, st, vs);
     return a.item_px == 64 ? launch_items<64>(a, st) : launch_items<32>(a, st);
 }
 

@@ -72,7 +72,7 @@ __device__ unsigned long long g_tile_timers[16];
 #endif
 
 template <int KPL, bool SECTOR>
-__global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs a) {
+__global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs a, const ViewSources vs) {
     extern __shared__ uint8_t smem_raw[];
     // keep the shared address space visible to the compiler: offset arithmetic on the array, no integer casts
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(NT, 1) epi_fusion_tile_kernel(const FusionArgs
         } else {
             ty0 = (trem / tiles_x) * TH; tx0 = (trem % tiles_x) * TW;
         }
-        items = pair_items(n, a.n_ref, a.n_views);
+        items = pair_items(n, a.n_ref, a.n_views, vs);
         src_hi = a.src_hi + (size_t)items.s * HW * C; src_lo = a.src_lo + (size_t)items.s * HW * C;
     }
     if (tid == 32) {
@@ -584,19 +584,19 @@ bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in) {
     return single <= DMAX;
 }
 
-cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
+cudaError_t launch_fusion_tile(const FusionArgs &a, const ViewSources &vs, cudaStream_t st) {
     const bool sector = a.order != nullptr;
     const int HW = a.geom.H * a.geom.W;
     const int tiles = a.N * (sector ? (HW + TM - 1) / TM : ((a.geom.W + TW - 1) / TW) * ((a.geom.H + TH - 1) / TH));
     const int kpl = (a.geom.K + 31) / 32;
-    void (*kern)(const FusionArgs);
+    void (*kern)(const FusionArgs, const ViewSources);
     if (sector) kern = kpl <= 1 ? epi_fusion_tile_kernel<1, true> : (kpl <= 2 ? epi_fusion_tile_kernel<2, true> : epi_fusion_tile_kernel<4, true>);
     else        kern = kpl <= 1 ? epi_fusion_tile_kernel<1, false> : (kpl <= 2 ? epi_fusion_tile_kernel<2, false> : epi_fusion_tile_kernel<4, false>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_ALLOC);
     if (e != cudaSuccess) return e;
     const int sms = sm_count();
     const int grid = a.tile_counter ? (tiles < sms ? tiles : sms) : tiles;     // one persistent CTA per SM
-    kern<<<grid, NT, SMEM_ALLOC, st>>>(a);
+    kern<<<grid, NT, SMEM_ALLOC, st>>>(a, vs);
     return cudaGetLastError();
 }
 
@@ -607,14 +607,15 @@ cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st) {
 // of (16-bit angle key << 14 | pixel index) in shared memory — unique keys, hence a deterministic order.
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) sector_order_kernel(const float *__restrict__ P_ref, const float *__restrict__ P_src,
-                                                            uint16_t *__restrict__ order, int n_ref, int n_views, const GeomCfg gc) {
+                                                            uint16_t *__restrict__ order, int n_ref, int n_views, const ViewSources vs,
+                                                            const GeomCfg gc) {
     extern __shared__ uint32_t keys[];
     __shared__ float s_e[4];          // ex, ey, a0, parallel-flag
     const int n = blockIdx.x, HW = gc.H * gc.W, W = gc.W;
     int npad = 1;
     while (npad < HW) npad <<= 1;
     if (threadIdx.x == 0) {
-        const PairItems items = pair_items(n, n_ref, n_views);
+        const PairItems items = pair_items(n, n_ref, n_views, vs);
         const float *P1 = P_ref + 12 * items.q, *P2 = P_src + 12 * items.s;
         double a[9], t1[3], b[9], t2[3], bi[9], cs[3], e[3];
         cam_load(P2, b, t2);
@@ -670,15 +671,15 @@ __global__ void __launch_bounds__(1024) sector_order_kernel(const float *__restr
     for (int i = threadIdx.x; i < HW; i += blockDim.x) order[(size_t)n * HW + i] = (uint16_t)(keys[i] & 0x3FFFu);
 }
 
-cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, int n_views, const GeomCfg &gc,
-                                cudaStream_t st) {
+cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, int n_views,
+                                const ViewSources &vs, const GeomCfg &gc, cudaStream_t st) {
     const int HW = gc.H * gc.W;
     int npad = 1;
     while (npad < HW) npad <<= 1;
     const size_t smem = (size_t)npad * 4;
     cudaError_t e = cudaFuncSetAttribute(sector_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    sector_order_kernel<<<N, 1024, smem, st>>>(P_ref, P_src, order, n_ref, n_views, gc);
+    sector_order_kernel<<<N, 1024, smem, st>>>(P_ref, P_src, order, n_ref, n_views, vs, gc);
     return cudaGetLastError();
 }
 

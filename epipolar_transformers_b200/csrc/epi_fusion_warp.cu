@@ -34,7 +34,7 @@ __device__ __forceinline__ void ld_vec(const float *p, float *dst) {
 // VEC floats per lane per chunk, NV chunks: lane owns channels (j*32+lane)*VEC+v, C <= 32*VEC*NV.
 template <int VEC, int NV>
 __global__ void __launch_bounds__(kWarpTileWarps * 32)
-epi_fusion_warp_kernel(const FusionArgs a) {
+epi_fusion_warp_kernel(const FusionArgs a, const ViewSources vs) {
     extern __shared__ float smem[];
     const int C = a.C, K = a.geom.K, H = a.geom.H, W = a.geom.W, HW = H * W;
     const int tiles_per_item = (HW + kWarpTilePix - 1) / kWarpTilePix;
@@ -47,7 +47,7 @@ epi_fusion_warp_kernel(const FusionArgs a) {
     float *a_tile = smem + (size_t)C * 33;                   // [K][33]  attention weights
     __shared__ PairGeom s_geom;
 
-    const PairItems it = pair_items(n, a.n_ref, a.n_views);  // the pair's query and source items
+    const PairItems it = pair_items(n, a.n_ref, a.n_views, vs);  // the pair's query and source items
     const int nr = it.q;
     if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * nr, a.P_src + 12 * it.s, s_geom);
 
@@ -242,26 +242,26 @@ epi_fusion_warp_kernel(const FusionArgs a) {
 }
 
 template <int VEC, int NV>
-static cudaError_t launch_warp_t(const FusionArgs &a, cudaStream_t st) {
+static cudaError_t launch_warp_t(const FusionArgs &a, const ViewSources &vs, cudaStream_t st) {
     const int HW = a.geom.H * a.geom.W;
     const int tiles = (HW + kWarpTilePix - 1) / kWarpTilePix;
     const size_t smem = ((size_t)a.C * 33 + (size_t)a.geom.K * 33) * sizeof(float);
     auto kern = epi_fusion_warp_kernel<VEC, NV>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    kern<<<a.N * tiles, kWarpTileWarps * 32, smem, st>>>(a);
+    kern<<<a.N * tiles, kWarpTileWarps * 32, smem, st>>>(a, vs);
     return cudaGetLastError();
 }
 
-cudaError_t launch_fusion_warp(const FusionArgs &a, cudaStream_t st) {
+cudaError_t launch_fusion_warp(const FusionArgs &a, const ViewSources &vs, cudaStream_t st) {
     const int C = a.C;
-    if (C % 4 == 0 && C <= 128) return launch_warp_t<4, 1>(a, st);
-    if (C % 4 == 0 && C <= 256) return launch_warp_t<4, 2>(a, st);
-    if (C % 4 == 0 && C <= 512) return launch_warp_t<4, 4>(a, st);
-    if (C % 4 == 0 && C <= 1024) return launch_warp_t<4, 8>(a, st);
-    if (C <= 32) return launch_warp_t<1, 1>(a, st);
-    if (C <= 128) return launch_warp_t<1, 4>(a, st);
-    if (C <= 512) return launch_warp_t<1, 16>(a, st);
+    if (C % 4 == 0 && C <= 128) return launch_warp_t<4, 1>(a, vs, st);
+    if (C % 4 == 0 && C <= 256) return launch_warp_t<4, 2>(a, vs, st);
+    if (C % 4 == 0 && C <= 512) return launch_warp_t<4, 4>(a, vs, st);
+    if (C % 4 == 0 && C <= 1024) return launch_warp_t<4, 8>(a, vs, st);
+    if (C <= 32) return launch_warp_t<1, 1>(a, vs, st);
+    if (C <= 128) return launch_warp_t<1, 4>(a, vs, st);
+    if (C <= 512) return launch_warp_t<1, 16>(a, vs, st);
     return cudaErrorInvalidValue;
 }
 

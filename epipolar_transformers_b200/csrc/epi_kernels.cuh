@@ -32,8 +32,8 @@ struct FusionArgs {
     __nv_bfloat16 *out_hi, *out_lo;           // optional: fused feature as bf16 (hi, lo) planes [N,H,W,C] (feeds the z GEMM)
     float *attn, *corr_pos, *locs_out;
     int N, C;                                 // N: pairs (S·N of the ABI)
-    int n_ref, n_views;                       // pair n reads query item pair_items(n, n_ref, n_views).q (feat_ref, ref_hi/lo, P_ref) and
-                                              // source item .s (src planes / src_nhwc, P_src); n_views > 0: both are the V·n_ref view items
+    int n_ref, n_views;                       // pair n reads query item pair_items(n, n_ref, n_views[, vs]).q (feat_ref, ref_hi/lo, P_ref)
+                                              // and source item .s (src planes / src_nhwc, P_src); n_views > 0: both are the V·n_ref view items
     float softmax_scale;
     int add_ref;
     int *tile_counter;                        // zeroed by the staging kernel; dynamic tile scheduler of the tile kernel
@@ -75,11 +75,12 @@ cudaError_t launch_acc_to_f32(const long long *acc, const unsigned *pair_max, fl
 // z-projection epilogue:  y[n,o,p] = sum_c Wf[o,c]·x[n,c,p] + bf[o] (+x[n,o,p]) (+ref[n,o,p])
 struct ZArgs {
     const float *x;         int64_t x_stride[4];     // pre-z fused feature
-    const float *ref;       int64_t ref_stride[4];   // may be null; item n reads ref item pair_items(n, n_ref, n_views).q
+    const float *ref;       int64_t ref_stride[4];   // may be null; item n reads ref item pair_items(n, n_ref, n_views, vsrc).q
     float *y;               int64_t y_stride[4];
     const float *Wf, *bf;
     int N, C, HW, W, n_ref, n_views;
     int z_residual, add_ref;
+    ViewSources vsrc;
 };
 
 // tensor-core z-projection: x arrives as bf16 (hi, lo) planes [N,H,W,C] written by the tile kernel
@@ -90,42 +91,45 @@ struct ZGemmArgs {
     const void *ref;        int64_t ref_stride[4];   // element type ref_dtype
     int ref_dtype;
     float *y;               int64_t y_stride[4];
-    int N, C, HW, W, Npad, n_ref, n_views;    // item n reads ref item pair_items(n, n_ref, n_views).q
+    int N, C, HW, W, Npad, n_ref, n_views;    // item n reads ref item pair_items(n, n_ref, n_views, vs).q
     int z_residual, add_ref;
 };
 bool zgemm_supported(int C);
-cudaError_t launch_zgemm(const ZGemmArgs &z, cudaStream_t st);
+// vs: the views form's source table, the kernel's last parameter (behind the tensor maps)
+cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, cudaStream_t st);
 
-cudaError_t launch_fusion_warp(const FusionArgs &a, cudaStream_t st);
-cudaError_t launch_fusion_tile(const FusionArgs &a, cudaStream_t st);
-cudaError_t launch_fusion_pipe(const FusionArgs &a, cudaStream_t st);
+// vs: the views form's source table (vs.S = 0: none)
+cudaError_t launch_fusion_warp(const FusionArgs &a, const ViewSources &vs, cudaStream_t st);
+cudaError_t launch_fusion_tile(const FusionArgs &a, const ViewSources &vs, cudaStream_t st);
+cudaError_t launch_fusion_pipe(const FusionArgs &a, const ViewSources &vs, cudaStream_t st);
 bool fusion_pipe_shape_ok(int C, int H, int W, int K, bool has_locs_in);
 size_t fusion_pipe_plan_record_bytes();
 int fusion_pipe_item_pixels(int C, int H, int W);                  // 32 or 64
 int fusion_pipe_plan_records(int N, int n_ref, int H, int W);   // N pairs on n_ref reference items
 bool fusion_tile_shape_ok(int C, int H, int W, int K, bool has_locs_in);
-// pair n: the cameras of pair_items(n, n_ref, n_views)
-cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, int n_views, const GeomCfg &gc,
-                                cudaStream_t st);
+// pair n: the cameras of pair_items(n, n_ref, n_views, vs)
+cudaError_t launch_sector_order(const float *P_ref, const float *P_src, uint16_t *order, int N, int n_ref, int n_views,
+                                const ViewSources &vs, const GeomCfg &gc, cudaStream_t st);
 // `dtype` (kF32 / kBF16 / kF16): element type of the source map(s)
 cudaError_t launch_split_planes(const void *src, const int64_t stride[4], __nv_bfloat16 *hi, __nv_bfloat16 *lo, int N, int C,
                                 int H, int W, int *zero_me, int dtype, cudaStream_t st);
 
 // planes: [ref_hi | ref_lo | src_hi | src_lo] for fp32 / fp16 maps, [ref_hi | src_hi] for bf16 maps (their lo part is zero);
 // the reference planes hold n_ref items, the source planes (and the pair constants / orders) N pairs, pair n on reference n % n_ref;
-// n_views > 0: `src` is null and only the reference planes are written, holding the n_views·n_ref view items (pair_items);
+// n_views > 0: `src` is null and only the reference planes are written, holding the n_views·n_ref view items (pair_items with vs);
 // `launched`: kernels started on success (2 when a large map orders its pixels in a launch of its own)
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
-                         int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched);
+                         int n_views, const ViewSources &vs, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched);
 
 cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
                                 cudaStream_t st);
 cudaError_t launch_z_epilogue(const ZArgs &z, cudaStream_t st);
-// out_dtype != kF32 (a gradient rounded once) takes no residual; item n adds ref item pair_items(n, n_ref, n_views).q
+// out_dtype != kF32 (a gradient rounded once) takes no residual; item n adds ref item pair_items(n, n_ref, n_views, vs).q
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
-                           const int64_t out_stride[4], int N, int n_ref, int n_views, int C, int H, int W, cudaStream_t st);
+                           const int64_t out_stride[4], int N, int n_ref, int n_views, const ViewSources &vs, int C, int H, int W,
+                           cudaStream_t st);
 cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, const float *b, const float *mean,
                              const float *var, float eps, int C, float *wf, float *bf, cudaStream_t st);
 cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, int J, int H, int W, float radius, float downsample,

@@ -1,6 +1,6 @@
 // epi_stage.cu — the ONE operand-staging launch in front of the fused attention kernel (epi_fusion_pipe.cu):
 //
-//   blocks [0, N)      per (ref, src) pair (pair n: items pair_items(n, n_ref, n_views), epi_common.cuh): fp64 pair constants (camera centre, epipole, infinite homography;
+//   blocks [0, N)      per (ref, src) pair (pair n: items pair_items(n, n_ref, n_views, vs), epi_common.cuh): fp64 pair constants (camera centre, epipole, infinite homography;
 //                      /root/reference/vision/multiview.py:16-21, modeling/layers/epipolar.py:336-348) and the list of
 //                      reference pixels sorted by epipolar angle (counting sort on a 12-bit angle key, ties by pixel index
 //                      => deterministic).  Pixels on one epipolar line of the reference view share one epipolar line in
@@ -11,7 +11,8 @@
 //                      The reference map has n_ref items and the source map N (several source views per reference item:
 //                      N = S·n_ref), so a reference tile is staged once however many sources it is fused with.  In the views
 //                      form (n_views = V) the reference map holds the V·n_ref view items and is the only map: each view is
-//                      staged once and serves as the query of V−1 pairs and the source of V−1 others.
+//                      staged once and serves as the query of its S pairs (S = V−1, or the source table's width) and the
+//                      source of whichever pairs name it.
 //                      fp16 values are split exactly like fp32 ones (hi + lo holds them exactly); a bf16 value is its own hi
 //                      part, so bf16 maps write hi planes only (reference -> plane 0, source -> plane 1).
 // Also zeroes the fused kernel's tile counter and error word.
@@ -72,7 +73,7 @@ struct StageArgs {
     int w_add_identity;               // ZRESIDUAL folded into the weight: planes hold Wf + I
     __nv_bfloat16 *w_planes;
     int N, C, H, W;
-    int n_ref, n_views;               // pair n reads items pair_items(n, n_ref, n_views)
+    int n_ref, n_views;               // pair n reads items pair_items(n, n_ref, n_views[, vs])
     int ref_tiles;                    // layout tiles of the reference map (n_ref items, or n_views·n_ref); the source map has N items
     size_t ref_elems;                 // elements of one reference plane
     size_t src_plane0;                // offset of the source hi plane in `planes`
@@ -84,8 +85,9 @@ struct StageArgs {
 // (min 5 blocks per SM: the layout-staging blocks need few registers; the rare order blocks may spill a little)
 // MULTI: several source views per reference item (n_ref < N), or the views form.  The one-source instantiation keeps the single-map-size indexing,
 // so its code (and its register allocation, tight at 48 registers) does not pay for the general mapping.
-template <typename T, bool MULTI>
-__global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T> s) {
+// vs: the source table of a table call, else empty (pair_items)
+template <typename T, bool MULTI, typename... Tab>
+__global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T> s, const Tab... vs) {
     using namespace stg;
     constexpr bool LO = !std::is_same<T, __nv_bfloat16>::value;   // a bf16 value's lo part is zero: no lo planes
     constexpr int NPL = LO ? 2 : 1;                               // planes per map
@@ -111,7 +113,7 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
         long long st_prev = clock64();
 #endif
         const int n = blockIdx.x;                                        // pair
-        const PairItems pi = MULTI ? pair_items(n, s.n_ref, s.n_views) : PairItems{n, n};
+        const PairItems pi = MULTI ? pair_items(n, s.n_ref, s.n_views, vs...) : PairItems{n, n};
         // cached order: the key is (P_ref, P_src, geometry configuration); an unchanged camera pair costs 32 compares
         float my_key = 0.f;
         if (t < 32) {
@@ -430,11 +432,12 @@ __global__ void __launch_bounds__(stg::NT, 5) epi_stage_kernel(const StageArgs<T
     stage_planes_tile<T, LO>(tile, sp, sc, sh, sw, vec, hi, lo, n, c0, p0, C, H, W);
 }
 
-template <typename T>
+template <typename T, typename... Tab>
 static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], const T *src, const int64_t src_stride[4],
                                   __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                                   float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
-                                  int n_ref, int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
+                                  int n_ref, int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched,
+                                  const Tab &... vs) {
     StageArgs<T> s;
     s.ref = ref; s.src = src;
     for (int i = 0; i < 4; i++) { s.ref_stride[i] = ref_stride[i]; s.src_stride[i] = src_stride[i]; }
@@ -452,7 +455,7 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     const size_t smem_tile = (size_t)stg::TC * stg::TPITCH * sizeof(float);
     const size_t smem_order = (size_t)stg::NBIN * 4 + (size_t)H * W * 2;
     const bool multi = n_ref != N || n_views;
-    void (*kern)(const StageArgs<T>) = multi ? epi_stage_kernel<T, true> : epi_stage_kernel<T, false>;
+    void (*kern)(const StageArgs<T>, const Tab...) = multi ? epi_stage_kernel<T, true, Tab...> : epi_stage_kernel<T, false, Tab...>;
     static thread_local size_t smem_set[2] = {0, 0};
     auto ensure = [&](size_t smem) -> cudaError_t {
         if (smem + 1024 > 48 * 1024 && smem > smem_set[multi]) {        // (+ the kernel's small static arrays)
@@ -471,7 +474,7 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
         o.do_ref = 0; o.do_src = 0; o.Wf = nullptr; o.w_planes = nullptr; o.persist = 0;
         cudaError_t e = ensure(smem_order);
         if (e != cudaSuccess) return e;
-        e = launch_pdl(kern, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o);
+        e = launch_pdl(kern, dim3((unsigned)N), dim3(stg::NT), smem_order, st, o, vs...);
         if (e != cudaSuccess) return e;
         s.do_order = 0; s.zero_words = nullptr;                  // the order launch has zeroed the counters
     }
@@ -488,21 +491,34 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     const size_t smem = (s.do_order && smem_order > smem_tile) ? smem_order : smem_tile;
     cudaError_t e = ensure(smem);
     if (e != cudaSuccess) return e;
-    return launch_pdl(kern, dim3((unsigned)grid), dim3(stg::NT), smem, st, s);
+    return launch_pdl(kern, dim3((unsigned)grid), dim3(stg::NT), smem, st, s, vs...);
+}
+
+template <typename... Tab>
+static cudaError_t launch_stage_d(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
+                                  __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
+                                  float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N,
+                                  int n_ref, int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched,
+                                  const Tab &... vs) {
+    if (dtype == kBF16)
+        return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched, vs...);
+    if (dtype == kF16)
+        return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
+                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched, vs...);
+    return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
+                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched, vs...);
 }
 
 cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const void *src, const int64_t src_stride[4], int dtype,
                          __nv_bfloat16 *planes, const float *P_ref, const float *P_src, PairGeom *pair_geom, uint16_t *order,
                          float *order_key, const float *Wf, __nv_bfloat16 *w_planes, int w_add_identity, int *zero_words, int N, int n_ref,
-                         int n_views, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
-    if (dtype == kBF16)
-        return launch_stage_t(static_cast<const __nv_bfloat16 *>(ref), ref_stride, static_cast<const __nv_bfloat16 *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
-    if (dtype == kF16)
-        return launch_stage_t(static_cast<const __half *>(ref), ref_stride, static_cast<const __half *>(src), src_stride, planes,
-                              P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
-    return launch_stage_t(static_cast<const float *>(ref), ref_stride, static_cast<const float *>(src), src_stride, planes,
-                          P_ref, P_src, pair_geom, order, order_key, Wf, w_planes, w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
+                         int n_views, const ViewSources &vs, int C, int H, int W, const GeomCfg &gc, cudaStream_t st, int &launched) {
+    if (vs.S)
+        return launch_stage_d(ref, ref_stride, src, src_stride, dtype, planes, P_ref, P_src, pair_geom, order, order_key, Wf, w_planes,
+                              w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched, vs);
+    return launch_stage_d(ref, ref_stride, src, src_stride, dtype, planes, P_ref, P_src, pair_geom, order, order_key, Wf, w_planes,
+                          w_add_identity, zero_words, N, n_ref, n_views, C, H, W, gc, st, launched);
 }
 
 }  // namespace epi

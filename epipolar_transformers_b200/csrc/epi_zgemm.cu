@@ -1,7 +1,7 @@
 // epi_zgemm.cu — z-projection epilogue on the tensor cores (TMA + warpgroup MMA).
 //
 //   y[n,o,p] = Σ_c Wf[o,c]·x[n,c,p] + bf[o]  (+ x[n,o,p] if ZRESIDUAL)  (+ feat_ref[q,o,p] for the caller's residual, read in
-//   the map's own element type; q = pair_items(n, n_ref, n_views).q, the pair's query item)
+//   the map's own element type; q = pair_items(n, n_ref, n_views[, vs]).q, the pair's query item)
 // restates  finalout = bn(z(out)) [+ out]   /root/reference/modeling/layers/epipolar.py:249-253 (eval-mode BN folded
 // into Wf, bf by epi_fold_z_bn_f32) and  ret + feat   /root/reference/modeling/backbones/resnet.py:388.
 //
@@ -17,6 +17,8 @@
 #include <cuda_bf16.h>
 
 #include <cstring>
+
+#include <type_traits>
 
 #include "epi_kernels.cuh"
 #include "epi_umma.cuh"
@@ -44,10 +46,16 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *t
 }
 }  // namespace zg
 
+// TABLE: vs is the call's source table; else an empty struct (one byte, no table code): the z GEMM's parameters hold tensor
+// maps, which a trailing parameter pack cannot follow here
+struct NoTable {};
+__device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n_views, NoTable) { return pair_items(p, n_ref, n_views); }
+template <bool TABLE>
 __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z, const __grid_constant__ CUtensorMap tm_hi,
                                                               const __grid_constant__ CUtensorMap tm_lo,
                                                               const __grid_constant__ CUtensorMap tw_hi,
-                                                              const __grid_constant__ CUtensorMap tw_lo) {
+                                                              const __grid_constant__ CUtensorMap tw_lo,
+                                                              const std::conditional_t<TABLE, ViewSources, NoTable> vs) {
     using namespace zg;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -80,7 +88,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
             res[k] = make_float4(0.f, 0.f, 0.f, 0.f);
             bias[k] = ol < CO ? __ldg(z.bf + oc0 + ol) : 0.f;      // folded bias: written long before the staging launch
             if (addr && vec && p + 3 < HW && ol < CO) {
-                const int64_t i = (int64_t)pair_items(n, z.n_ref, z.n_views).q * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p;     // the caller's map, in its type
+                const int64_t i = (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p;     // the caller's map, in its type
                 res[k] = z.ref_dtype == kBF16 ? ld4_cs(static_cast<const __nv_bfloat16 *>(z.ref) + i)
                        : z.ref_dtype == kF16  ? ld4_cs(static_cast<const __half *>(z.ref) + i)
                                               : ld4_cs(static_cast<const float *>(z.ref) + i);
@@ -160,7 +168,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
                 for (int e = 0; e < 4 && p + e < HW; e++) {
                     const int py = (p + e) / W, px = (p + e) % W;
                     float val = y[e];
-                    if (addr) val += ld_feat(z.ref, (int64_t)pair_items(n, z.n_ref, z.n_views).q * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
+                    if (addr) val += ld_feat(z.ref, (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
                     z.y[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = val;
                 }
             }
@@ -198,11 +206,13 @@ bool make_plane_map(CUtensorMap *m, const __nv_bfloat16 *base, int rows, int C, 
 }
 }  // namespace
 
-cudaError_t launch_zgemm(const ZGemmArgs &z, cudaStream_t st) {
+template <bool TABLE>
+static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std::conditional_t<TABLE, ViewSources, NoTable> &vs) {
     const int tiles = (z.HW + 127) / 128;
+    const auto kern = epi_zgemm_kernel<TABLE>;
     static thread_local bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(epi_zgemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
@@ -216,7 +226,11 @@ cudaError_t launch_zgemm(const ZGemmArgs &z, cudaStream_t st) {
             return cudaErrorInvalidValue;
         mc.xh = z.x_hi; mc.wh = z.w_hi; mc.rows = z.N * z.HW; mc.C = z.C;
     }
-    return launch_pdl(epi_zgemm_kernel, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::NB - 1) / zg::NB)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3]);
+    return launch_pdl(kern, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::NB - 1) / zg::NB)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3], vs);
+}
+
+cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, cudaStream_t st) {
+    return vs.S ? launch_zgemm_t<true>(z, st, vs) : launch_zgemm_t<false>(z, st, NoTable{});
 }
 
 }  // namespace epi

@@ -15,15 +15,12 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from .multiview import neighbor_cameras
+from .multiview import nearest_view_table
 
 
 def source_view_table(KRT_all) -> np.ndarray:
     """src(v) for every view: nearest other camera centre.  KRT_all: [V,3,4] (numpy or tensor, any device)."""
-    K = KRT_all.detach().cpu().numpy() if isinstance(KRT_all, torch.Tensor) else np.asarray(KRT_all)
-    K = K.astype(np.float64)
-    centers = np.stack([-np.linalg.solve(P[:, :3], P[:, 3]) for P in K])
-    return neighbor_cameras(centers, topk=1)[:, 0]
+    return nearest_view_table(KRT_all, topk=1)[:, 0].astype(np.int64)
 
 
 class ViewParallelFusion:

@@ -13,12 +13,13 @@ from __future__ import annotations
 import ctypes
 from typing import Optional
 
+import numpy as np
 import torch
 from torch import nn
 
 from . import _lib
 from .config import get_global_cfg
-from .peaks import find_tensor_peak_best
+from .peaks import find_tensor_peak_batch, find_tensor_peak_best
 
 _EPSILON = 0.001          # epipolar.py:20
 
@@ -166,19 +167,49 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
             None if attn is None else attn.unflatten(0, (S, N)), None if locs is None else locs.unflatten(1, (S, N)))
 
 
+def view_source_table(sources, V):
+    """A caller's source table as the C ABI takes it: [V,S] int32 on the host, every entry a view in [0, V) other than its
+    row's own view (duplicates are allowed).  sources: a list of rows, a numpy array or a CPU integer tensor.  A CUDA tensor is
+    refused: reading it back would synchronise the stream.  Build the table once per camera rig (`multiview.nearest_view_table`)."""
+    if isinstance(sources, torch.Tensor):
+        if sources.is_cuda:
+            raise TypeError("sources must be on the host (a list, numpy array or CPU tensor): reading a CUDA table back would "
+                            "synchronise the stream")
+        if sources.dtype.is_floating_point or sources.dtype.is_complex or sources.dtype == torch.bool:
+            raise TypeError("sources must hold integers (got %s)" % sources.dtype)
+        sources = sources.numpy()
+    t = np.asarray(sources)
+    if t.ndim != 2 or t.shape[0] != V or t.shape[1] < 1:
+        raise ValueError("sources must be a [V,S] table with V = %d rows and S >= 1 (got shape %s)" % (V, tuple(t.shape)))
+    if t.dtype.kind not in "iu":
+        raise TypeError("sources must hold integer view indices (got %s)" % t.dtype)
+    if V * t.shape[1] > _lib.EPI_VIEW_SOURCES_MAX:
+        raise ValueError("sources has %d entries; a call takes at most %d (V*S)" % (V * t.shape[1], _lib.EPI_VIEW_SOURCES_MAX))
+    if (t < 0).any() or (t >= V).any():
+        raise ValueError("sources entries must be views in [0, %d)" % V)
+    own = np.nonzero(t == np.arange(V)[:, None])
+    if own[0].size:
+        raise ValueError("sources[%d] names view %d itself: a view is not fused with itself" % (own[0][0], own[0][0]))
+    return np.ascontiguousarray(t, dtype=np.int32)
+
+
 def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax_scale=0.125, correct_normalize=False,
                           align_corners=False, z_folded=None, z_residual=False, add_ref_residual=False, sample_locs_in=None,
                           want_attn=True, want_corr=True, want_locs=False, variant="auto", out=None,
-                          state: Optional[FusionState] = None):
-    """Fuses every view of a frame with every other view in one call: the whole multi-view test of the reference
-    (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239), where each of the V views takes a turn as the reference.  Each view's
-    map is staged once and serves as the query of V−1 pairs and the source of V−1 others.
+                          state: Optional[FusionState] = None, sources=None):
+    """Fuses each view of a frame with several other views in one call, staging each view's map once.
+
+    sources=None: every view with every other view, the whole multi-view test of the reference (cfg.EPIPOLAR.MULTITEST,
+    modeling/model.py:213-239), where each of the V views takes a turn as the reference; S = V−1 and view v's j-th source is
+    u = j + (j >= v) (the other views in increasing order).
+    sources=[V,S] table (list, numpy array or CPU integer tensor; see `view_source_table`): view v's j-th source is
+    u = sources[v][j].  With the nearest camera per view (S = 1, `multiview.nearest_view_table`) this is the reference's
+    standard test (modeling/model.py:240-247) from one backbone pass.
 
     feats: [V,N,C,H,W], or a sequence of V [N,C,H,W] maps (stacked), V >= 2; P: [V,N,3,4]; sample_locs_in: optional
-    [K,V,V−1,N,H,W,2]; out: optional float32 [V,V−1,N,C,H,W].  Reference view v with its j-th other view u = j + (j >= v) (the
-    other views in increasing order) gives, bit for bit, what `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every
-    residual (add_ref_residual, also under z) adds feats[v][n].  Returns
-    (out [V,V−1,N,C,H,W], corr_pos [V,V−1,N,H,W,2] | None, attn [V,V−1,N,K,H,W] | None, sample_locs [K,V,V−1,N,H,W,2] | None).
+    [K,V,S,N,H,W,2]; out: optional float32 [V,S,N,C,H,W].  Reference view v with its j-th source u gives, bit for bit, what
+    `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every residual (add_ref_residual, also under z) adds feats[v][n].
+    Returns (out [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attn [V,S,N,K,H,W] | None, sample_locs [K,V,S,N,H,W,2] | None).
     Inference only: inputs that require grad under grad mode raise RuntimeError."""
     lib = _lib.load()
     if isinstance(feats, (list, tuple)):
@@ -194,14 +225,19 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
     V, N, C, H, W = feats.shape
     if V < 2:
         raise ValueError("feats needs at least two views (got %d)" % V)
+    table = None if sources is None else view_source_table(sources, V)
+    if table is not None:
+        _lib.require_view_sources(lib)
+    S = V - 1 if table is None else table.shape[1]
+    Sn = "V-1" if table is None else "S"                        # the sources dimension, as the messages name it
     feat = feats.flatten(0, 1)                                  # [V·N,C,H,W]: item v·N + n
     if out is not None:
-        if not isinstance(out, torch.Tensor) or tuple(out.shape) != (V, V - 1, N, C, H, W):
-            raise ValueError("out must be a [V,V-1,N,C,H,W] tensor")
+        if not isinstance(out, torch.Tensor) or tuple(out.shape) != (V, S, N, C, H, W):
+            raise ValueError("out must be a [V,%s,N,C,H,W] tensor" % Sn)
         try:
-            out4 = out.view(V * (V - 1) * N, C, H, W)
+            out4 = out.view(V * S * N, C, H, W)
         except RuntimeError:
-            raise ValueError("out must be viewable as [V*(V-1)*N,C,H,W]") from None
+            raise ValueError("out must be viewable as [V*(%s)*N,C,H,W]" % Sn) from None
     else:
         out4 = None
     if sample_locs_in is None:
@@ -209,9 +245,9 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
             raise ValueError("P must be [V,N,3,4]")
         P = P.reshape(V * N, 3, 4)
     else:
-        if tuple(sample_locs_in.shape) != (K, V, V - 1, N, H, W, 2):
-            raise ValueError("sample_locs_in must be [K,V,V-1,N,H,W,2]")
-        sample_locs_in = sample_locs_in.reshape(K, V * (V - 1) * N, H, W, 2)
+        if tuple(sample_locs_in.shape) != (K, V, S, N, H, W, 2):
+            raise ValueError("sample_locs_in must be [K,V,%s,N,H,W,2]" % Sn)
+        sample_locs_in = sample_locs_in.reshape(K, V * S * N, H, W, 2)
     dcode = _check_feat_pair(feat, feat, out4)
     if torch.is_grad_enabled() and feat.requires_grad:
         raise RuntimeError("epipolar_fusion_views is inference only (the views form has no backward); run it under "
@@ -220,22 +256,24 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
                                   softmax_scale=softmax_scale, correct_normalize=correct_normalize,
                                   align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
                                   add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
-                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state, views=V)
-    pairs = (V, V - 1, N)
+                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state, views=V,
+                                  table=table)
+    pairs = (V, S, N)
     return (out if out is not None else o.unflatten(0, pairs), None if corr is None else corr.unflatten(0, pairs),
             None if attn is None else attn.unflatten(0, pairs), None if locs is None else locs.unflatten(1, pairs))
 
 
 def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, img_scale, softmax_scale, correct_normalize,
             align_corners, z_folded, z_residual, add_ref_residual, sample_locs_in, want_attn, want_corr, want_locs, variant, out,
-            state, views=0):
+            state, views=0, table=None):
     """The forward of `epipolar_fusion` (S = 1) and `epipolar_fusion_multi`: feat_ref [N,C,H,W], feat_src / out [S·N,C,H,W],
     P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n).
     views = V >= 2 (`epipolar_fusion_views`): feat_ref [V·N,C,H,W] and P_ref [V·N,3,4] hold the views, feat_src and P_src are
-    None, and the outputs have V·(V−1)·N items (pair p = (v·(V−1) + j)·N + n)."""
+    None, and the outputs have V·S·N items (pair p = (v·S + j)·N + n), S = V−1, or the width of `table` ([V,S] int32 host
+    array from `view_source_table`, which selects the source-table entry points)."""
     NR, C, H, W = feat_ref.shape
     N = NR // views if views else NR
-    NP = views * (views - 1) * N if views else S * N
+    NP = views * (views - 1 if table is None else table.shape[1]) * N if views else S * N
     dev = feat_ref.device
     if sample_locs_in is None:
         if P_ref.device != dev or P_ref.dtype != torch.float32 or not P_ref.is_contiguous():
@@ -261,7 +299,8 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     vcode = _lib.VARIANTS[variant] if isinstance(variant, str) else int(variant)
     # the plan (and so the workspace size) also depends on whether `out` and feat_src start on a 16-byte boundary
     src_key = (feat_src.stride(), feat_src.data_ptr() % 16 == 0) if feat_src is not None else (feat_ref.data_ptr() % 16 == 0,)
-    key = (dev, S, views, N, C, H, W, int(K), dcode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
+    tkey = None if table is None else (table.shape, table.tobytes())
+    key = (dev, S, views, tkey, N, C, H, W, int(K), dcode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
            z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
@@ -292,16 +331,24 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     if z_folded is not None:
         wf, bf = z_folded
         p.z_weight_folded = wf.data_ptr(); p.z_bias_folded = bf.data_ptr()
+    if table is None:
+        cache_bytes, workspace_bytes = lib.epi_fusion_cache_bytes, lib.epi_fusion_workspace_bytes
+        forward = lib.epi_fusion_forward_f32
+    else:                                                          # the [V,S] host table goes with every call
+        targs = (table.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), table.shape[1])
+        cache_bytes = lambda q: lib.epi_fusion_view_sources_cache_bytes(q, *targs)
+        workspace_bytes = lambda q: lib.epi_fusion_view_sources_workspace_bytes(q, *targs)
+        forward = lambda q, st: lib.epi_fusion_view_sources_forward_f32(q, *targs, st)
     ws = None
     if state is not None and state.key == key:
         pass                                                       # workspace / cache pointers already in the block
     else:
         if state is not None:
-            cbytes = lib.epi_fusion_cache_bytes(ctypes.byref(p))
+            cbytes = cache_bytes(ctypes.byref(p))
             state.cache = torch.zeros(cbytes, device=dev, dtype=torch.uint8) if cbytes else None
             p.cache = state.cache.data_ptr() if cbytes else None
             p.cache_bytes = cbytes
-        nbytes = lib.epi_fusion_workspace_bytes(ctypes.byref(p))
+        nbytes = workspace_bytes(ctypes.byref(p))
         if nbytes:
             ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)      # caching allocator: stream-ordered, 512-B aligned
             p.workspace = ws.data_ptr(); p.workspace_bytes = nbytes
@@ -309,7 +356,8 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
             state.ws = ws; state.params = p; state.key = key
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.epi_fusion_forward_f32(ctypes.byref(p), ctypes.c_void_p(stream)), "epi_fusion_forward_f32")
+        _lib.check(forward(ctypes.byref(p), ctypes.c_void_p(stream)),
+                   "epi_fusion_forward_f32" if table is None else "epi_fusion_view_sources_forward_f32")
     return out, corr, attn, locs
 
 
@@ -588,12 +636,13 @@ class Epipolar(nn.Module):
             state=self._state_for(feat1, "multi"))
         return out, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
 
-    def forward_views(self, feats, P):
-        """`forward` of every view of a frame against every other view in one fused call (the whole MULTITEST path,
-        modeling/model.py:213-239).  feats [V,N,C,H,W] or a sequence of V [N,C,H,W] maps, P [V,N,3,4].  Returns what
-        `forward(feats[v], feats[u], P[v], P[u])` returns for reference view v and its j-th other view u = j + (j >= v),
-        stacked as (finalout [V,V−1,N,C,H,W], corr_pos [V,V−1,N,H,W,2] | None, attention [V,V−1,N,K,H,W] | None,
-        sample_locs [V,V−1,N,K,H,W,2] | None).  Inference only.  With the z projection the module must be in eval mode, for the
+    def forward_views(self, feats, P, sources=None):
+        """`forward` of every view of a frame against several other views in one fused call.  feats [V,N,C,H,W] or a
+        sequence of V [N,C,H,W] maps, P [V,N,3,4].  sources=None: every other view (the whole MULTITEST path,
+        modeling/model.py:213-239), S = V−1 and u = j + (j >= v); a [V,S] host table (see `epipolar_fusion_views`): u =
+        sources[v][j].  Returns what `forward(feats[v], feats[u], P[v], P[u])` returns for reference view v and its j-th source
+        u, stacked as (finalout [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attention [V,S,N,K,H,W] | None,
+        sample_locs [V,S,N,K,H,W,2] | None).  Inference only.  With the z projection the module must be in eval mode, for the
         reason `forward_multi` gives."""
         cfg = self.cfg
         ep = cfg.EPIPOLAR
@@ -610,7 +659,7 @@ class Epipolar(nn.Module):
             align_corners=self.align_corners, z_folded=self._folded() if has_z else None,
             z_residual=bool(ep.ZRESIDUAL) if has_z else False, add_ref_residual=self.fuse_ref_residual,
             want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
-            state=self._state_for(first, "views"))
+            state=self._state_for(first, "views"), sources=sources)
         return out, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
 
 
@@ -644,25 +693,66 @@ def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma
         return find_tensor_peak_best(heat.unflatten(0, (S, N)), sigma, downsample)
 
 
-def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample):
+_device_tables = {}          # (device, shape, bytes) -> the [V,S] source table as an int64 device tensor
+
+
+def _table_on(table, dev):
+    """The source table on `dev`, copied once per (table, device): the per-step path makes no host-to-device copy."""
+    key = (str(dev), table.shape, table.tobytes())
+    t = _device_tables.get(key)
+    if t is None:
+        t = _device_tables[key] = torch.from_numpy(table.astype(np.int64)).to(dev)
+    return t
+
+
+def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample, sources=None):
     """The reference's multi-view test (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239) for every view of a frame at once:
-    each view v is the reference in turn, is fused with each of its V−1 other views, each fusion goes through the rest of the
-    network and the peak finder, and every joint keeps the location of the other view whose peak scores highest.  All
-    V·(V−1) fusions are one `Epipolar.forward_views` call and the selection is one launch of `find_tensor_peak_best`.
+    each view v is the reference in turn, is fused with each of its sources, each fusion goes through the rest of the
+    network and the peak finder, and every joint keeps the location of the source whose peak scores highest.  All V·S
+    fusions are one `Epipolar.forward_views` call and the selection is one launch of `find_tensor_peak_best`.
 
     feats [V,N,C,H,W] or V [N,C,H,W] maps (the views' features at the merge point), KRT [V,N,3,4]; tail, sigma and downsample
-    as for `multitest`.  Returns per view (locs [V,N,J,2], scores [V,N,J], source view [V,N,J]): the source is the camera index
-    u of the winning view, not its position j among the other views."""
+    as for `multitest`.  sources=None: every other view (S = V−1); a [V,S] host table (e.g. `multiview.nearest_view_table`
+    with topk = S): the sources it names, a cheaper test over each view's S nearest cameras.  Returns per view
+    (locs [V,N,J,2], scores [V,N,J], source view [V,N,J]): the source is the camera index u of the winning view, not its
+    position j among the view's sources."""
     with torch.no_grad():
         if isinstance(feats, (list, tuple)):
             feats = torch.stack(list(feats))
-        ret, _, _, _ = sampler.forward_views(feats, KRT)
-        V, N = feats.shape[0], feats.shape[1]
+        ret, _, _, _ = sampler.forward_views(feats, KRT, sources=sources)
+        V, S, N = ret.shape[0], ret.shape[1], ret.shape[2]
         x = ret if sampler.fuse_ref_residual else ret + feats[:, None]    # getOtherFeat's `ret + feat` of reference view v
-        heat = tail(x.flatten(0, 2))                                       # [V·(V−1)·N, J, h, w]
-        # [V−1, V·N, J, h, w]: source slot j of every (view, item)
-        heat = heat.unflatten(0, (V, V - 1, N)).transpose(0, 1).flatten(1, 2)
+        heat = tail(x.flatten(0, 2))                                       # [V·S·N, J, h, w]
+        # [S, V·N, J, h, w]: source slot j of every (view, item)
+        heat = heat.unflatten(0, (V, S, N)).transpose(0, 1).flatten(1, 2)
         locs, scores, j = find_tensor_peak_best(heat, sigma, downsample)
         j = j.unflatten(0, (V, N))
-        v = torch.arange(V, device=j.device).view(V, 1, 1)
-        return locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), j + (j >= v).long()
+        if sources is None:
+            v = torch.arange(V, device=j.device).view(V, 1, 1)
+            return locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), j + (j >= v).long()
+        table = _table_on(view_source_table(sources, V), j.device)        # [V,S]
+        return locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), table.gather(1, j.flatten(1)).view_as(j)
+
+
+def standard_views_test(sampler: Epipolar, tail, feats, KRT, sources, sigma, downsample):
+    """The reference's standard (non-MULTITEST) test from one backbone pass: each view v is the reference once, fused with
+    the one source view sources[v][0] (its nearest camera, data/datasets/multiview_h36m.py:231-238), and the fusion goes
+    through getOtherFeat's residual (modeling/backbones/resnet.py:377-388), the rest of the network and the peak finder
+    (resnet.py:423-430).  The reference runs the backbone a second time on the permuted views (modeling/model.py:240-247);
+    here the other view's map is the same backbone output, so the V fusions are one `Epipolar.forward_views` call.
+
+    sampler: the Epipolar layer; tail: everything after the merge point ([B,C,H,W] -> heat-maps [B,J,h,w]); feats
+    [V,N,C,H,W] or V [N,C,H,W] maps (the views' features at the merge point); KRT [V,N,3,4]; sources: a [V,1] host table
+    (`multiview.nearest_view_table(..., topk=1)`); sigma = cfg.KEYPOINT.SIGMA, downsample as for find_tensor_peak_batch.
+    Returns per view (locs [V,N,J,2], scores [V,N,J], corr_pos [V,N,H,W,2] | None, attention [V,N,K,H,W] | None)."""
+    with torch.no_grad():
+        if isinstance(feats, (list, tuple)):
+            feats = torch.stack(list(feats))
+        V, N = feats.shape[0], feats.shape[1]
+        if view_source_table(sources, V).shape[1] != 1:
+            raise ValueError("the standard test fuses each view with one source: sources must be [V,1]")
+        ret, corr, attn, _ = sampler.forward_views(feats, KRT, sources=sources)
+        x = ret[:, 0] if sampler.fuse_ref_residual else ret[:, 0] + feats     # getOtherFeat's `ret + feat`
+        locs, scores = find_tensor_peak_batch(tail(x.flatten(0, 1)), sigma, downsample)
+        return (locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), None if corr is None else corr[:, 0],
+                None if attn is None else attn[:, 0])

@@ -64,3 +64,16 @@ def neighbor_cameras(centers, topk=1):
     d = np.linalg.norm(C[:, None] - C[None], axis=-1)
     np.fill_diagonal(d, np.inf)
     return np.argsort(d, axis=1, kind="stable")[:, :topk]
+
+
+def nearest_view_table(KRT_all, topk=1) -> np.ndarray:
+    """The [V,topk] source table of `epipolar_fusion_views(..., sources=)`: for each view of a rig its `topk` nearest other
+    cameras by centre distance, nearest first (`neighbor_cameras`; topk=1 is the pairing of the reference's standard test,
+    data/datasets/multiview_h36m.py:231-238).  KRT_all: [V,3,4] (numpy or tensor, any device).  The cameras are constants of
+    a rig, so compute the table once: reading a device tensor here synchronises."""
+    K = KRT_all.detach().cpu().numpy() if isinstance(KRT_all, torch.Tensor) else np.asarray(KRT_all)
+    K = K.astype(np.float64)
+    if K.ndim != 3 or K.shape[1:] != (3, 4) or not 1 <= topk <= max(K.shape[0] - 1, 1):
+        raise ValueError("need KRT_all [V,3,4] and 1 <= topk <= V-1 (got %s, topk=%d)" % (K.shape, topk))
+    centers = np.stack([-np.linalg.solve(P[:, :3], P[:, 3]) for P in K])
+    return neighbor_cameras(centers, topk=topk).astype(np.int32)

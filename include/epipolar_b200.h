@@ -182,6 +182,28 @@ int epi_fusion_backward_deterministic(void);
  * one-source call). */
 int epi_fusion_views(void);
 
+/* ---- the views form with a caller's source table --------------------------------------------------------------------------
+ * The views form (n_views = V >= 2, see EpiFusionParams.n_views) with the sources chosen by the caller instead of every other
+ * view: view v of item n is fused with views sources_host[v·S + j], 0 <= j < S.  sources_host is a [V][S] int32 table in HOST
+ * memory, read and checked during the call (the caller may reuse it once the call returns).  It reaches the kernels inside their
+ * launch parameters, so the call neither synchronises nor copies from pageable memory; that bounds the table to
+ * V·S <= EPI_VIEW_SOURCES_MAX entries.  Every other field of p means what it means in the views form (feat_src and P_src NULL,
+ * n_src 0 or 1).  Pair p = (v·S + j)·N + n fuses query item v·N + n with source item sources_host[v·S + j]·N + n.  out, attn and
+ * corr_pos have V·S·N items, sample_locs_in / sample_locs_out are [K,V·S·N,H,W,2], and every residual reads the pair's query
+ * item.  Each pair's outputs (every output and epilogue, every variant and feat_dtype, injected locations, with or without the
+ * cache) are bit for bit those of a one-source call on (view v, view u) at item n; each view's map is staged once.  The cache
+ * stays keyed per pair by that pair's cameras, so a changed table on the same cache gives fresh-call results.
+ * Duplicate entries are allowed.  EPI_EINVAL (with a message) for a NULL table, S < 1, n_views < 2, V·S > EPI_VIEW_SOURCES_MAX,
+ * an entry outside [0, V), an entry equal to its own view (a self-pair), V·S·N > 65535 pairs, and every refusal of the views form.
+ * No backward: the views forms are inference only. */
+#define EPI_VIEW_SOURCES_MAX 256
+int epi_fusion_view_sources_forward_f32(const EpiFusionParams *p, const int32_t *sources_host, int32_t S, void *stream);
+/* Workspace / cache bytes of that call: V·N staged view items and V·S·N pairs.  0 when the table or params cannot be planned. */
+size_t epi_fusion_view_sources_workspace_bytes(const EpiFusionParams *p, const int32_t *sources_host, int32_t S);
+size_t epi_fusion_view_sources_cache_bytes(const EpiFusionParams *p, const int32_t *sources_host, int32_t S);
+/* 1: this library has the source-table entry points above (a library built before them lacks this symbol). */
+int epi_fusion_view_sources(void);
+
 /* Only the geometry: sample locations [K,N,H,W,2] for (P_ref,P_src)  (grid2sample_locs). */
 int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_locs_out, int32_t N,
                         int32_t H, int32_t W, int32_t K, float downsample, float img_scale, float eps,
