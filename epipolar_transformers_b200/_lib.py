@@ -23,11 +23,14 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_sample_locs_f32", "epi_fold_z_bn_f32", "epi_last_launch_count", "epi_umma_selftest",
            "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3",
            "epi_fusion_backward_deterministic", "epi_fusion_views", "epi_fusion_view_sources_forward_f32",
-           "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources")
+           "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources",
+           "epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward")
 # The source-table entry points are new symbols, not a reinterpreted field, so a library without them still runs every other
 # form correctly: load() accepts it, and only a call with a source table needs them (`require_view_sources`).
 VIEW_SOURCES_EXPORTS = ("epi_fusion_view_sources_forward_f32", "epi_fusion_view_sources_workspace_bytes",
                         "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources")
+# The backward of the views form is optional in the same way: only a views-backward call needs it (`require_views_backward`).
+VIEWS_BACKWARD_EXPORTS = ("epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward")
 
 _fp = ctypes.POINTER(ctypes.c_float)
 
@@ -93,7 +96,7 @@ def load():
             "epipolar_transformers_b200: CUDA library %s is missing. Build it with "
             "`python -m epipolar_transformers_b200.build` (needs nvcc). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS and not hasattr(lib, s)]
+    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS and not hasattr(lib, s)]
     if missing:
         # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
         # (a views call would silently run as a one-source call)
@@ -144,6 +147,13 @@ def load():
         lib.epi_fusion_view_sources_cache_bytes.restype = ctypes.c_size_t
         lib.epi_fusion_view_sources_cache_bytes.argtypes = table
         lib.epi_fusion_view_sources.restype = ctypes.c_int
+    if all(hasattr(lib, s) for s in VIEWS_BACKWARD_EXPORTS):
+        views = [ctypes.POINTER(EpiFusionBwdParams), ctypes.c_int32, ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]
+        lib.epi_fusion_views_backward_f32.restype = ctypes.c_int
+        lib.epi_fusion_views_backward_f32.argtypes = views + [ctypes.c_void_p]
+        lib.epi_fusion_views_backward_workspace_bytes.restype = ctypes.c_size_t
+        lib.epi_fusion_views_backward_workspace_bytes.argtypes = views
+        lib.epi_fusion_views_backward.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))
@@ -157,6 +167,14 @@ def require_view_sources(lib):
     if missing or lib.epi_fusion_view_sources() != 1:
         raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot fuse views with a source table; rebuild it with "
                            "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_view_sources"]))
+
+
+def require_views_backward(lib):
+    """Raise unless `lib` has the backward of the views form (epi_fusion_views_backward())."""
+    missing = [s for s in VIEWS_BACKWARD_EXPORTS if not hasattr(lib, s)]
+    if missing or lib.epi_fusion_views_backward() != 1:
+        raise RuntimeError("libepipolar_b200.so does not export %s, so it has no backward for the views form; rebuild it with "
+                           "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_views_backward"]))
 
 
 def check(rc: int, what: str):

@@ -197,12 +197,11 @@ bool plannable(const EpiFusionParams *p, const epi::ViewSources &vs) {
            (p->n_views == 0 || (p->n_views >= 2 && p->n_views <= 256 && p->n_src <= 1 && n_pairs64(p, vs) <= 65535));
 }
 
-// Reads the caller's [V][S] host table into `vs` (the kernels' by-value copy).  Returns null, or why the table is refused.
-const char *read_view_table(const EpiFusionParams *p, const int32_t *sources, int32_t S, epi::ViewSources &vs, char *msg, size_t len) {
-    if (!p) return "params is null";
+// Reads the caller's [V][S] host table of V = n_views views into `vs` (the kernels' by-value copy).  Returns null, or why the
+// table is refused.
+const char *read_table(int V, const int32_t *sources, int32_t S, epi::ViewSources &vs, char *msg, size_t len) {
     if (!sources) return "sources_host is null";
     if (S < 1) return "S (sources per view) must be >= 1";
-    const int V = p->n_views;
     if (V < 2) return "the source-table form needs n_views >= 2 (the views of a frame)";
     if ((int64_t)V * S > EPI_VIEW_SOURCES_MAX)
         return "n_views * S must be <= EPI_VIEW_SOURCES_MAX (256): the table travels in the kernels' launch parameters";
@@ -214,6 +213,10 @@ const char *read_view_table(const EpiFusionParams *p, const int32_t *sources, in
         vs.src[i] = (uint8_t)u;
     }
     return nullptr;
+}
+
+const char *read_view_table(const EpiFusionParams *p, const int32_t *sources, int32_t S, epi::ViewSources &vs, char *msg, size_t len) {
+    return p ? read_table(p->n_views, sources, S, vs, msg, len) : "params is null";
 }
 
 int validate(const EpiFusionParams *p, const epi::ViewSources &vs) {
@@ -286,6 +289,46 @@ BwdPlan make_bwd_plan(const EpiFusionBwdParams *p) {
     return pl;
 }
 
+// Views form of the backward (epi_fusion_views_backward_f32), V·N view items and NP = V·S·N pairs: a pixel-major fp32 copy of
+// the view maps (the query and the source map of every pair), the per-item sums (float accumulator of the source terms, then
+// dL/dfeats in fp32), one pixel-major fp32 query term per pair; deterministic: + the int64 fixed-point accumulator per item, one
+// bound word per item and the [NP,K,H·W] float2 coefficients (accumulator and words adjacent, so that one memset zeroes both)
+struct ViewsBwdPlan { size_t items, nhwc, gsum, gq, acc = NONE, words = NONE, coef = NONE, workspace_bytes; };
+
+ViewsBwdPlan make_views_bwd_plan(const EpiFusionBwdParams *p, int V, int S) {
+    ViewsBwdPlan pl;
+    Regions ws;
+    const size_t px = (size_t)p->H * p->W, item = (size_t)p->C * px * sizeof(float), NI = (size_t)V * p->N, NP = NI * S;
+    pl.items = NI * item;
+    pl.nhwc = ws.take(pl.items); pl.gsum = ws.take(pl.items); pl.gq = ws.take(NP * item);
+    if (p->deterministic == 1) {
+        pl.acc = ws.take(2 * pl.items);
+        pl.words = ws.take(NI * sizeof(uint32_t));
+        pl.coef = ws.take(NP * px * p->K * sizeof(float2));
+    }
+    pl.workspace_bytes = ws.end;
+    return pl;
+}
+
+// The table (or the all-others form: sources NULL and S = 0) and the params of a views backward.  Returns null, or why they are
+// refused; on success `vs` holds the table and `S` the sources per view.
+const char *read_views_bwd(const EpiFusionBwdParams *p, int32_t V, const int32_t *sources, int32_t &S, epi::ViewSources &vs,
+                           char *msg, size_t len) {
+    if (!p) return "params is null";
+    if (V < 2) return "n_views must be >= 2 (the views of a frame)";
+    if (sources || S != 0) {
+        if (const char *why = read_table(V, sources, S, vs, msg, len)) return why;
+    } else {
+        if (V > 256) return "n_views must be <= 256";
+        S = V - 1;
+    }
+    if (p->N <= 0 || p->H <= 0 || p->W <= 0) return "bad shape";
+    const int64_t np = (int64_t)V * S * p->N;
+    if (np > 65535) return "pairs (n_views * S * N, S = n_views - 1 or the table's width) must be <= 65535";
+    if (np * (((int64_t)p->H * p->W + 31) / 32) > INT32_MAX) return "pairs * H * W too large: the backward's tiles are counted in int32";
+    return nullptr;
+}
+
 epi::GeomCfg make_geom(int H, int W, int K, float ds, float r, float eps, int correct, int align) {
     epi::GeomCfg g;
     g.ds = ds; g.r = r; g.eps = eps;
@@ -315,6 +358,8 @@ int epi_fusion_backward_deterministic(void) { return 1; }
 int epi_fusion_views(void) { return 1; }
 
 int epi_fusion_view_sources(void) { return 1; }
+
+int epi_fusion_views_backward(void) { return 1; }
 
 int epi_kernel_timing_enable(int on) { g_timing = on ? 1 : 0; return EPI_OK; }
 
@@ -565,6 +610,65 @@ int epi_fusion_backward_f32(const EpiFusionBwdParams *p, void *stream) {
     if (p->grad_ref && lowp &&         // fp32 gradient of a low-precision reference map, rounded once to its type
         (rc = run("gradient transposition", epi::launch_unstage(gref32, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride,
                                                                 p->N, p->N, 0, kAllOthers, p->C, p->H, p->W, st)))) return rc;
+    g_launches = run.n;
+    return EPI_OK;
+}
+
+size_t epi_fusion_views_backward_workspace_bytes(const EpiFusionBwdParams *p, int32_t n_views, const int32_t *sources_host, int32_t S) {
+    epi::ViewSources vs{};
+    char msg[128];
+    if (read_views_bwd(p, n_views, sources_host, S, vs, msg, sizeof(msg)) || p->C <= 0) return 0;
+    return make_views_bwd_plan(p, n_views, S).workspace_bytes;
+}
+
+int epi_fusion_views_backward_f32(const EpiFusionBwdParams *p, int32_t n_views, const int32_t *sources_host, int32_t S, void *stream) {
+    epi::ViewSources vs{};
+    char msg[128];
+    if (const char *why = read_views_bwd(p, n_views, sources_host, S, vs, msg, sizeof(msg))) return fail(EPI_EINVAL, "%s", why);
+    if (p->feat_src || p->P_src || p->grad_src)
+        return fail(EPI_EINVAL, "views backward: feat_src, P_src and grad_src must be null (feat_ref / P_ref / grad_ref hold the views)");
+    // every check of the one-pair backward, with the view maps in both roles
+    EpiFusionBwdParams q = *p;
+    q.feat_src = p->feat_ref; q.P_src = p->P_ref;
+    int rc = validate_bwd(&q);
+    if (rc != EPI_OK) return rc;
+    if (!p->grad_ref) return EPI_OK;
+    const ViewsBwdPlan pl = make_views_bwd_plan(p, n_views, S);
+    void *ws = p->workspace;
+    if (!ws || p->workspace_bytes < pl.workspace_bytes) return fail(EPI_EWORKSPACE, "workspace too small");
+    if (reinterpret_cast<uintptr_t>(ws) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int dt = p->feat_dtype, NI = n_views * p->N, NP = NI * S, HW = p->H * p->W;
+    const bool has_src = p->grad_keys || p->grad_vals;
+    const bool det = p->deterministic == 1 && has_src;          // the query terms alone are the same launch on both paths
+    float *nhwc = at<float>(ws, pl.nhwc), *gsum = at<float>(ws, pl.gsum), *gq = at<float>(ws, pl.gq);
+    const int64_t pm_stride[4] = {(int64_t)p->C * HW, 1, (int64_t)p->W * p->C, p->C};      // pixel-major / channels-last
+    const epi::BwdViews vw{p->N, n_views, vs};
+    Launches run;
+    // the view maps staged once: the query of the pairs of a view and the source of the pairs that name it
+    if ((rc = run("layout staging", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, nhwc, NI, p->C, p->H, p->W, dt, st)))) return rc;
+    if (has_src) {
+        const cudaError_t e = det ? cudaMemsetAsync(at<char>(ws, pl.acc), 0, pl.words + NI * sizeof(uint32_t) - pl.acc, st)
+                                  : cudaMemsetAsync(gsum, 0, pl.items, st);
+        if (e != cudaSuccess) return fail(EPI_ECUDA, "memset failed: %s", cudaGetErrorString(e));
+    }
+    epi::BwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.feat_ref = nhwc; a.src_nhwc = nhwc; a.P_ref = p->P_ref; a.P_src = p->P_ref;
+    a.locs_in = p->sample_locs_in; a.attn = p->attn; a.grad_out = p->grad_out; a.grad_attn = p->grad_attn;
+    a.grad_ref = gq;
+    a.dsrc_nhwc = has_src && !det ? gsum : nullptr;
+    for (int i = 0; i < 4; i++) { a.ref_stride[i] = pm_stride[i]; a.gout_stride[i] = p->gout_stride[i]; a.gref_stride[i] = pm_stride[i]; }
+    a.N = NP; a.C = p->C; a.softmax_scale = p->softmax_scale; a.grad_keys = p->grad_keys; a.grad_vals = p->grad_vals;
+    a.geom = make_geom(p->H, p->W, p->K, p->downsample, p->img_scale, p->eps, p->correct_normalize, p->align_corners);
+    if (det) { a.coef = at<float2>(ws, pl.coef); a.pair_max = at<unsigned>(ws, pl.words); a.acc = at<long long>(ws, pl.acc); }
+    int kernels = 0;
+    const cudaError_t e = epi::launch_fusion_bwd_views(a, vw, st, det, kernels);
+    if ((rc = run(det ? "deterministic backward kernels" : "backward kernel", e, kernels))) return rc;
+    if ((rc = run("gradient sum", epi::launch_views_grad_sum(gq, a.dsrc_nhwc, det ? a.acc : nullptr, det ? a.pair_max : nullptr, gsum,
+                                                               vw, HW, p->C, st)))) return rc;
+    if ((rc = run("gradient transposition", epi::launch_unstage(gsum, nullptr, EPI_DTYPE_F32, p->gref_stride, p->grad_ref, dt, p->gref_stride,
+                                                                NI, NI, 0, kAllOthers, p->C, p->H, p->W, st)))) return rc;
     g_launches = run.n;
     return EPI_OK;
 }

@@ -174,6 +174,43 @@ cudaError_t launch_acc_to_f32(const long long *acc, const unsigned *pair_max, fl
 }
 
 // ------------------------------------------------------------------------------------------
+// Views form of the backward: one pass per view item sums its query terms (one pixel-major fp32 plane per pair, order-fixed) in
+// the order of its pairs and adds its source term, float sums or fixed-point sums converted with the item's scale (NaN for an
+// item one of whose pairs has a non-finite bound, zero for a zero bound).  Each element is read and written by one thread, so
+// `g` may be `dsrc`.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) views_grad_sum_kernel(const float *__restrict__ gq, const float *dsrc, const long long *__restrict__ acc,
+                                                             const unsigned *__restrict__ item_max, float *g, const BwdViews vw,
+                                                             int HW, int C) {
+    const int i = blockIdx.y, v = i / vw.n_ref, n = i - v * vw.n_ref;
+    const int S = vw.vs.S ? vw.vs.S : vw.n_views - 1;
+    const size_t len = (size_t)HW * C, base = (size_t)i * len;
+    int s = 0;
+    bool scaled = false;
+    float fill = 0.f;
+    if (acc) {
+        const unsigned word = __ldg(item_max + i);
+        scaled = det_item_scale(word, HW, view_source_count(v, vw.n_views, vw.vs), s);
+        fill = __uint_as_float(word) == 0.f ? 0.f : __int_as_float(0x7fffffff);
+    }
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < len; e += (size_t)gridDim.x * blockDim.x) {
+        float sum = __ldg(gq + (size_t)(v * S * vw.n_ref + n) * len + e);
+        for (int j = 1; j < S; j++) sum += __ldg(gq + (size_t)((v * S + j) * vw.n_ref + n) * len + e);
+        if (dsrc) sum += dsrc[base + e];
+        else if (acc) sum += scaled ? (float)ldexp((double)__ldg(acc + base + e), -s) : fill;
+        g[base + e] = sum;
+    }
+}
+
+cudaError_t launch_views_grad_sum(const float *gq, const float *dsrc, const long long *acc, const unsigned *item_max, float *g,
+                                  const BwdViews &vw, int HW, int C, cudaStream_t st) {
+    const size_t len = (size_t)HW * C;
+    const int blocks = (int)((len + 255) / 256 < 1024 ? (len + 255) / 256 : 1024);
+    views_grad_sum_kernel<<<dim3(blocks, vw.n_views * vw.n_ref), 256, 0, st>>>(gq, dsrc, acc, item_max, g, vw, HW, C);
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
 // Fold conv1x1 z + eval BN (epipolar.py:250-251, BN.py:79 with training=False) into Wf, bf.
 // ------------------------------------------------------------------------------------------
 __global__ void fold_z_bn_kernel(const float *__restrict__ zw, const float *__restrict__ zb,

@@ -174,6 +174,14 @@ __host__ __device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n
     return {vj / vs.S * n_ref + n, (int)vs.src[vj] * n_ref + n};
 }
 
+// Number of pairs whose source is view u: V−1 in the all-others form, else the table entries that name u.
+__host__ __device__ __forceinline__ int view_source_count(int u, int n_views, const ViewSources &vs) {
+    if (vs.S == 0) return n_views - 1;
+    int c = 0;
+    for (int i = 0; i < n_views * vs.S; i++) c += vs.src[i] == u;
+    return c;
+}
+
 // Per-(ref,src)-pair constants: M = A2·A1^-1 (row-major 3x3) and the epipole e2/e2.z.
 struct PairGeom {
     float M[9];
@@ -332,6 +340,15 @@ __device__ __forceinline__ bool det_scale(unsigned word, int HW, int &s) {
     int e;
     frexpf(m, &e);
     s = 61 - (32 - __clz(HW - 1)) - e;
+    return true;
+}
+
+// The same for one view item of the views form's backward, into which `pairs` pairs of its frame scatter: `word` holds the largest
+// of their bounds, so their sums stay below pairs·HW·M_max·2^s, and s is lowered by ceil(log2(pairs)) to keep that under 2^61.
+// Only the frame's own pairs enter the scale, and one non-finite bound among them makes the item's sums NaN.
+__device__ __forceinline__ bool det_item_scale(unsigned word, int HW, int pairs, int &s) {
+    if (!det_scale(word, HW, s)) return false;
+    s -= 32 - __clz(pairs - 1);
     return true;
 }
 

@@ -13,9 +13,22 @@
 // caller's layout afterwards.  The attention weights saved by the forward are reused, so no softmax is recomputed.
 // The deterministic backward (EpiFusionBwdParams.deterministic) runs the same kernel as a coefficient pass that stores
 // (cv_k, ck_k) and a per-pair bound instead of scattering, then a fixed-point scatter with int64 atomics (DESIGN.md §3.5, §5).
+// The views form (epi_fusion_views_backward_f32) launches the same kernels with a trailing BwdViews parameter: pair n then reads
+// its query item and its source item of one staged map through pair_items, and the source terms of every pair that names an item
+// land in that item's accumulator.  Without the parameter the pack is empty and both items are n.
 #include "epi_kernels.cuh"
 
 namespace epi {
+
+// (query item, source item) of pair n: n itself in the one-pair form, pair_items in the views form
+__device__ __forceinline__ PairItems bwd_items(int n) { return {n, n}; }
+__device__ __forceinline__ PairItems bwd_items(int n, const BwdViews &vw) { return pair_items(n, vw.n_ref, vw.n_views, vw.vs); }
+// fixed-point scale of source item `item`: the pair's own bound word in the one-pair form; in the views form the item's word (the
+// largest bound of the pairs that scatter into it) and their number (det_item_scale)
+__device__ __forceinline__ bool bwd_scale(unsigned word, int HW, int item, int &s) { return det_scale(word, HW, s); }
+__device__ __forceinline__ bool bwd_scale(unsigned word, int HW, int item, int &s, const BwdViews &vw) {
+    return det_item_scale(word, HW, view_source_count(item / vw.n_ref, vw.n_views, vw.vs), s);
+}
 
 namespace bwd {
 constexpr int TILE_PIX = 32;
@@ -42,21 +55,22 @@ __device__ __forceinline__ void stage_bwd_tile(float *tile, const float *base, c
 // DET = false: the default kernel, which scatters dL/dfeat_src with float atomics.  DET = true: the coefficient pass of the
 // deterministic backward, the same operations up to the scatter, which it replaces by storing each sample's coefficients and
 // folding the pixel's bound on its contributions into the pair's bound word.  (The switch is a parameter of the kernel itself:
-// an inlined body function would allocate the default kernel's registers differently.)
-template <int VEC, int NV, bool DET>
-__global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_kernel(const BwdArgs a) {
+// an inlined body function would allocate the default kernel's registers differently.)  vw: the views form, else empty.
+template <int VEC, int NV, bool DET, typename... Views>
+__global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_kernel(const BwdArgs a, const Views... vw) {
     using namespace bwd;
     extern __shared__ float smem[];
     const int C = a.C, K = a.geom.K, H = a.geom.H, W = a.geom.W, HW = H * W;
     const int tiles_per_item = (HW + TILE_PIX - 1) / TILE_PIX;
-    const int n = blockIdx.x / tiles_per_item;
+    const int n = blockIdx.x / tiles_per_item;               // pair
+    const PairItems it = bwd_items(n, vw...);                // its query and source items
     const int p0 = (blockIdx.x % tiles_per_item) * TILE_PIX;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int npix = min(TILE_PIX, HW - p0);
     float *q_tile = smem;                                    // [C][33]  query in, dL/dq out
     float *g_tile = smem + (size_t)C * 33;                   // [C][33]  dL/dout
     __shared__ PairGeom s_geom;
-    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * n, a.P_src + 12 * n, s_geom);
+    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * it.q, a.P_src + 12 * it.s, s_geom);
 
     auto stage_tile = [&](float *tile, const float *base, const int64_t *st) {
         const int64_t sc = st[1], sh = st[2], sw = st[3];
@@ -72,14 +86,14 @@ __global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_kernel(const B
             }
         }
     };
-    stage_tile(q_tile, a.feat_ref + (int64_t)n * a.ref_stride[0], a.ref_stride);
+    stage_tile(q_tile, a.feat_ref + (int64_t)it.q * a.ref_stride[0], a.ref_stride);
     stage_tile(g_tile, a.grad_out + (int64_t)n * a.gout_stride[0], a.gout_stride);
     __syncthreads();
 
     const PairGeom g = s_geom;
     const GeomCfg gc = a.geom;
-    const float *src = a.src_nhwc + (size_t)n * HW * C;
-    float *dsrc = a.dsrc_nhwc ? a.dsrc_nhwc + (size_t)n * HW * C : nullptr;
+    const float *src = a.src_nhwc + (size_t)it.s * HW * C;
+    float *dsrc = a.dsrc_nhwc ? a.dsrc_nhwc + (size_t)it.s * HW * C : nullptr;
 
     unsigned warp_bound = 0u;                        // DET: bits of the largest M_i of the warp's pixels
     for (int pi = 0; pi < TILE_PIX / WARPS; pi++) {
@@ -239,7 +253,7 @@ __global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_kernel(const B
                 if (c < C) q_tile[c * 33 + pp] = dq[j * VEC + v];
             }
     }
-    if (DET && lane == 0 && warp_bound != 0u) atomicMax(a.pair_max + n, warp_bound);   // max of non-negative floats: their bits' max
+    if (DET && lane == 0 && warp_bound != 0u) atomicMax(a.pair_max + it.s, warp_bound);   // max of non-negative floats: their bits' max
     __syncthreads();
     if (a.grad_ref) {
         float *obase = a.grad_ref + (int64_t)n * a.gref_stride[0];
@@ -262,30 +276,31 @@ __global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_kernel(const B
 // each sample's taps as pass 1 does (from locs_in or the cameras, with the same functions), forms every contribution in fp32 as the
 // default scatter does, and adds round(v·2^s) to the int64 accumulator.  Integer addition is associative, so the sums do not
 // depend on the order the warps' atomics land in.  A pair with a zero or non-finite bound adds nothing.
-template <int VEC, int NV>
-__global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_scatter_kernel(const BwdArgs a) {
+template <int VEC, int NV, typename... Views>
+__global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_scatter_kernel(const BwdArgs a, const Views... vw) {
     using namespace bwd;
     extern __shared__ float smem[];
     const int C = a.C, K = a.geom.K, H = a.geom.H, W = a.geom.W, HW = H * W;
     const int tiles_per_item = (HW + TILE_PIX - 1) / TILE_PIX;
-    const int n = blockIdx.x / tiles_per_item;
+    const int n = blockIdx.x / tiles_per_item;                       // pair
+    const PairItems it = bwd_items(n, vw...);                        // its query and source items
     const int p0 = (blockIdx.x % tiles_per_item) * TILE_PIX;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int npix = min(TILE_PIX, HW - p0);
     int s;
-    if (!det_scale(__ldg(a.pair_max + n), HW, s)) return;          // block-uniform
+    if (!bwd_scale(__ldg(a.pair_max + it.s), HW, it.s, s, vw...)) return;    // block-uniform
     const double scale = ldexp(1.0, s);                              // exact in fp64 for every s a float bound can give
     float *q_tile = smem;                                            // [C][33]  query
     float *g_tile = smem + (size_t)C * 33;                           // [C][33]  dL/dout
     __shared__ PairGeom s_geom;
-    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * n, a.P_src + 12 * n, s_geom);
-    stage_bwd_tile(q_tile, a.feat_ref + (int64_t)n * a.ref_stride[0], a.ref_stride, C, W, p0, npix);
+    if (tid == 0 && a.locs_in == nullptr) pair_geom_from_krt(a.P_ref + 12 * it.q, a.P_src + 12 * it.s, s_geom);
+    stage_bwd_tile(q_tile, a.feat_ref + (int64_t)it.q * a.ref_stride[0], a.ref_stride, C, W, p0, npix);
     stage_bwd_tile(g_tile, a.grad_out + (int64_t)n * a.gout_stride[0], a.gout_stride, C, W, p0, npix);
     __syncthreads();
 
     const PairGeom g = s_geom;
     const GeomCfg gc = a.geom;
-    unsigned long long *acc = reinterpret_cast<unsigned long long *>(a.acc) + (size_t)n * HW * C;   // two's complement sums
+    unsigned long long *acc = reinterpret_cast<unsigned long long *>(a.acc) + (size_t)it.s * HW * C;   // two's complement sums
     for (int pi = 0; pi < TILE_PIX / WARPS; pi++) {
         const int pp = warp * (TILE_PIX / WARPS) + pi;
         if (pp >= npix) break;                       // warp-uniform
@@ -346,29 +361,31 @@ __global__ void __launch_bounds__(bwd::WARPS * 32) epi_fusion_bwd_scatter_kernel
     }
 }
 
-template <int VEC, int NV>
-static cudaError_t launch_bwd_t(const BwdArgs &a, cudaStream_t st, bool det) {
+template <int VEC, int NV, typename... Views>
+static cudaError_t launch_bwd_t(const BwdArgs &a, cudaStream_t st, bool det, const Views &...vw) {
     const int HW = a.geom.H * a.geom.W;
     const int tiles = (HW + bwd::TILE_PIX - 1) / bwd::TILE_PIX;
     const size_t smem = (size_t)a.C * 33 * 2 * sizeof(float);
-    void (*const kernels[2])(BwdArgs) = {det ? epi_fusion_bwd_kernel<VEC, NV, true> : epi_fusion_bwd_kernel<VEC, NV, false>,
-                                         epi_fusion_bwd_scatter_kernel<VEC, NV>};
+    // (each entry a conditional: a kernel template with a trailing parameter pack converts to a pointer only once it is resolved)
+    void (*const kernels[2])(const BwdArgs, const Views...) = {det ? epi_fusion_bwd_kernel<VEC, NV, true, Views...> : epi_fusion_bwd_kernel<VEC, NV, false, Views...>,
+                                                               det ? epi_fusion_bwd_scatter_kernel<VEC, NV, Views...> : nullptr};
     for (int i = 0; i < (det ? 2 : 1); i++) {
         cudaError_t e = cudaFuncSetAttribute(kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        kernels[i]<<<a.N * tiles, bwd::WARPS * 32, smem, st>>>(a);
+        kernels[i]<<<a.N * tiles, bwd::WARPS * 32, smem, st>>>(a, vw...);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     return cudaSuccess;
 }
 
-static cudaError_t launch_bwd(const BwdArgs &a, cudaStream_t st, bool det) {
+template <typename... Views>
+static cudaError_t launch_bwd(const BwdArgs &a, cudaStream_t st, bool det, const Views &...vw) {
     const int C = a.C;
-    if (C % 4 == 0 && C <= 128) return launch_bwd_t<4, 1>(a, st, det);
-    if (C % 4 == 0 && C <= 256) return launch_bwd_t<4, 2>(a, st, det);
-    if (C % 4 == 0 && C <= 512) return launch_bwd_t<4, 4>(a, st, det);
-    if (C <= 32) return launch_bwd_t<1, 1>(a, st, det);
-    if (C <= 128) return launch_bwd_t<1, 4>(a, st, det);
+    if (C % 4 == 0 && C <= 128) return launch_bwd_t<4, 1>(a, st, det, vw...);
+    if (C % 4 == 0 && C <= 256) return launch_bwd_t<4, 2>(a, st, det, vw...);
+    if (C % 4 == 0 && C <= 512) return launch_bwd_t<4, 4>(a, st, det, vw...);
+    if (C <= 32) return launch_bwd_t<1, 1>(a, st, det, vw...);
+    if (C <= 128) return launch_bwd_t<1, 4>(a, st, det, vw...);
     return cudaErrorInvalidValue;
 }
 
@@ -377,6 +394,12 @@ cudaError_t launch_fusion_bwd(const BwdArgs &a, cudaStream_t st) { return launch
 cudaError_t launch_fusion_bwd_det(const BwdArgs &a, cudaStream_t st, int &launched) {
     const cudaError_t e = launch_bwd(a, st, true);
     launched = e == cudaSuccess ? 2 : 0;
+    return e;
+}
+
+cudaError_t launch_fusion_bwd_views(const BwdArgs &a, const BwdViews &vw, cudaStream_t st, bool det, int &launched) {
+    const cudaError_t e = launch_bwd(a, st, det, vw);
+    launched = e == cudaSuccess ? (det ? 2 : 1) : 0;
     return e;
 }
 

@@ -71,6 +71,17 @@ cudaError_t launch_fusion_bwd(const BwdArgs &a, cudaStream_t st);
 cudaError_t launch_fusion_bwd_det(const BwdArgs &a, cudaStream_t st, int &launched);
 // fixed-point accumulator [N,HW,C] + per-pair bound words -> pixel-major fp32 dsrc (NaN for a pair whose bound is not finite)
 cudaError_t launch_acc_to_f32(const long long *acc, const unsigned *pair_max, float *dsrc, int N, int HW, int C, cudaStream_t st);
+// The views form of the backward: BwdArgs then describes a.N = V·S·N pairs on the V·n_ref items of one staged map.  Pair n reads
+// feat_ref at its query item and src_nhwc at its source item (pair_items(n, n_ref, n_views, vs)), P_ref / P_src at the same
+// items, and attn, grad_out, grad_attn and locs_in at n; grad_ref receives the pair's query term at n.  dsrc_nhwc, acc and
+// pair_max are per source item (pair_max: the largest bound of the pairs that scatter into the item, det_item_scale).
+struct BwdViews { int n_ref, n_views; ViewSources vs; };
+cudaError_t launch_fusion_bwd_views(const BwdArgs &a, const BwdViews &vw, cudaStream_t st, bool det, int &launched);
+// dL/dfeats of the views form, pixel-major fp32 [V·n_ref,HW,C]: for item i = v·n_ref + n, the query terms gq of its pairs
+// (v·S + j)·n_ref + n summed in the order of j, plus its source term: dsrc[i] (float sums), or the fixed-point sums acc[i] with
+// the item's bound word item_max[i], or nothing when both are null.  `g` may be `dsrc`.
+cudaError_t launch_views_grad_sum(const float *gq, const float *dsrc, const long long *acc, const unsigned *item_max, float *g,
+                                  const BwdViews &vw, int HW, int C, cudaStream_t st);
 
 // z-projection epilogue:  y[n,o,p] = sum_c Wf[o,c]·x[n,c,p] + bf[o] (+x[n,o,p]) (+ref[n,o,p])
 struct ZArgs {

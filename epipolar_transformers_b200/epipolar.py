@@ -210,7 +210,8 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
     [K,V,S,N,H,W,2]; out: optional float32 [V,S,N,C,H,W].  Reference view v with its j-th source u gives, bit for bit, what
     `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every residual (add_ref_residual, also under z) adds feats[v][n].
     Returns (out [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attn [V,S,N,K,H,W] | None, sample_locs [K,V,S,N,H,W,2] | None).
-    Inference only: inputs that require grad under grad mode raise RuntimeError."""
+    Inference only: inputs that require grad under grad mode raise RuntimeError.  `epipolar_fusion_views_backward` is its
+    backward, and `Epipolar.forward_views_train` the differentiable form."""
     lib = _lib.load()
     if isinstance(feats, (list, tuple)):
         if not all(isinstance(t, torch.Tensor) for t in feats):
@@ -250,8 +251,8 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
         sample_locs_in = sample_locs_in.reshape(K, V * S * N, H, W, 2)
     dcode = _check_feat_pair(feat, feat, out4)
     if torch.is_grad_enabled() and feat.requires_grad:
-        raise RuntimeError("epipolar_fusion_views is inference only (the views form has no backward); run it under "
-                           "torch.no_grad(), or use epipolar_fusion (one pair per call) for gradients")
+        raise RuntimeError("epipolar_fusion_views is inference only; run it under torch.no_grad(), or use "
+                           "Epipolar.forward_views_train (backward: epipolar_fusion_views_backward) for gradients")
     o, corr, attn, locs = _fusion(lib, dcode, 1, feat, None, P, None, K=K, downsample=downsample, img_scale=img_scale,
                                   softmax_scale=softmax_scale, correct_normalize=correct_normalize,
                                   align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
@@ -421,6 +422,85 @@ def epipolar_fusion_backward(feat_ref, feat_src, P_ref, P_src, attn, grad_out, *
     return g_ref, g_src
 
 
+def epipolar_fusion_views_backward(feats, P, attn, grad_out, *, K, downsample=4.0, img_scale=1.0, softmax_scale=0.125,
+                                   correct_normalize=False, align_corners=False, sources=None, grad_attn=None, sample_locs_in=None,
+                                   grad_keys=True, grad_vals=True, deterministic=None):
+    """Backward of `epipolar_fusion_views` without the z epilogue: dL/dfeats [V,N,C,H,W] in the maps' dtype (float32 sums,
+    rounded once).  Each view item gets the dL/dfeat_ref terms of the pairs it is the query of and, as grad_keys / grad_vals
+    ('other1' / 'other2' in cfg.EPIPOLAR.OTHER_GRAD) select, the dL/dfeat_src terms of the pairs that name it as their source;
+    every term is what `epipolar_fusion_backward` computes for that pair.  A view that is nobody's source gets query terms only.
+
+    feats: [V,N,C,H,W] (or V [N,C,H,W] maps); P: [V,N,3,4] (unused with sample_locs_in); attn, grad_attn: [V,S,N,K,H,W];
+    grad_out: [V,S,N,C,H,W]; sample_locs_in: optional [K,V,S,N,H,W,2], the locations the forward sampled; sources: None (every
+    other view) or a [V,S] host table, as in `epipolar_fusion_views`.  Each view map is staged once.
+    deterministic: None follows torch.are_deterministic_algorithms_enabled(); True sums the source terms in per-item int64 fixed
+    point, whose scale depends on the item's own frame only, so the bits do not depend on the rest of the batch or the layouts.
+    An item one of whose source pairs has a NaN or inf in its maps or gradients comes out all NaN on that path."""
+    if deterministic is None:
+        deterministic = torch.are_deterministic_algorithms_enabled()
+    elif not isinstance(deterministic, bool):
+        raise TypeError("deterministic must be None or a bool (got %s)" % type(deterministic).__name__)
+    lib = _lib.load()
+    if isinstance(feats, (list, tuple)):
+        if len({(tuple(t.shape), t.dtype, t.device) for t in feats if isinstance(t, torch.Tensor)}) != 1 or \
+                not all(isinstance(t, torch.Tensor) for t in feats):
+            raise ValueError("the maps in feats must be tensors sharing shape, dtype and device")
+        feats = torch.stack(list(feats))
+    if not isinstance(feats, torch.Tensor) or feats.dim() != 5:
+        raise ValueError("feats must be a [V,N,C,H,W] tensor or a sequence of V [N,C,H,W] tensors")
+    V, N, C, H, W = feats.shape
+    if V < 2:
+        raise ValueError("feats needs at least two views (got %d)" % V)
+    table = None if sources is None else view_source_table(sources, V)
+    _lib.require_views_backward(lib)
+    S = V - 1 if table is None else table.shape[1]
+    Sn = "V-1" if table is None else "S"
+    for name, t, shape in (("attn", attn, (V, S, N, K, H, W)), ("grad_out", grad_out, (V, S, N, C, H, W)),
+                           ("grad_attn", grad_attn, (V, S, N, K, H, W))):
+        if t is not None and (not isinstance(t, torch.Tensor) or tuple(t.shape) != shape):
+            raise ValueError("%s must be a [V,%s,N,%s,H,W] tensor" % (name, Sn, "K" if name != "grad_out" else "C"))
+    feat = feats.flatten(0, 1)                                  # [V·N,C,H,W]: item v·N + n
+    dcode = _check_feat_pair(feat, feat)
+    dev = feat.device
+    NP = V * S * N
+    grad_out = grad_out.reshape(NP, C, H, W)
+    grad_out = grad_out if grad_out.dtype == torch.float32 else grad_out.float()
+    attn = attn.reshape(NP, K, H, W).to(dtype=torch.float32).contiguous()
+    g = torch.empty_like(feat)
+    p = _lib.EpiFusionBwdParams()
+    p.feat_ref = feat.data_ptr(); p.ref_stride = _strides4(feat)
+    if sample_locs_in is None:
+        if not isinstance(P, torch.Tensor) or tuple(P.shape) != (V, N, 3, 4):
+            raise ValueError("P must be [V,N,3,4]")
+        P = P.reshape(V * N, 3, 4).to(device=dev, dtype=torch.float32).contiguous()
+        p.P_ref = P.data_ptr()
+    else:
+        if tuple(sample_locs_in.shape) != (K, V, S, N, H, W, 2):
+            raise ValueError("sample_locs_in must be [K,V,%s,N,H,W,2]" % Sn)
+        sample_locs_in = _aligned_locs(sample_locs_in.reshape(K, NP, H, W, 2).to(device=dev, dtype=torch.float32))
+        p.sample_locs_in = sample_locs_in.data_ptr()
+    p.attn = attn.data_ptr()
+    p.grad_out = grad_out.data_ptr(); p.gout_stride = _strides4(grad_out)
+    if grad_attn is not None:
+        grad_attn = grad_attn.reshape(NP, K, H, W).to(dtype=torch.float32).contiguous()
+        p.grad_attn = grad_attn.data_ptr()
+    p.grad_ref = g.data_ptr(); p.gref_stride = _strides4(g)
+    p.N, p.C, p.H, p.W, p.K = N, C, H, W, int(K)
+    p.downsample = float(downsample); p.img_scale = float(img_scale); p.eps = _EPSILON; p.softmax_scale = float(softmax_scale)
+    p.align_corners = int(bool(align_corners)); p.correct_normalize = int(bool(correct_normalize))
+    p.grad_keys = int(bool(grad_keys)); p.grad_vals = int(bool(grad_vals))
+    p.feat_dtype = dcode
+    p.deterministic = int(deterministic)
+    targs = (V, None if table is None else table.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), 0 if table is None else S)
+    nbytes = lib.epi_fusion_views_backward_workspace_bytes(ctypes.byref(p), *targs)
+    ws = torch.empty(max(nbytes, 1), device=dev, dtype=torch.uint8)
+    p.workspace = ws.data_ptr(); p.workspace_bytes = nbytes
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(lib.epi_fusion_views_backward_f32(ctypes.byref(p), *targs, ctypes.c_void_p(stream)), "epi_fusion_views_backward_f32")
+    return g.unflatten(0, (V, N))
+
+
 class _FusionFn(torch.autograd.Function):
     """The fused attention under autograd (no z epilogue: conv/BN stay in PyTorch when gradients are needed).
     The gradients of bfloat16 / float16 maps come back in their dtype.
@@ -458,6 +538,42 @@ class _FusionFn(torch.autograd.Function):
         if ctx.needs_input_grad[1] and g_src is None:
             g_src = torch.zeros_like(feat_src)
         return g_ref, g_src, None, None, None
+
+
+class _ViewsFusionFn(torch.autograd.Function):
+    """The views form under autograd (no z epilogue), for the reason and in the way of `_FusionFn`: the forward saves the
+    attention and the locations it sampled, and the backward (`epipolar_fusion_views_backward`) samples there.  feats
+    [V,N,C,H,W] gets one gradient per view item, summed over the pairs it is the query or the source of."""
+
+    @staticmethod
+    def forward(ctx, feats, P, sources, opts):
+        with torch.no_grad():
+            out, corr, attn, locs = epipolar_fusion_views(feats, P, want_attn=True, sources=sources,
+                                                          **dict(opts["fwd"], want_locs=True))
+        ctx.save_for_backward(feats, attn, locs)
+        ctx.opts, ctx.sources = opts, sources
+        if not opts["fwd"].get("want_locs", False):
+            locs = None
+        nd = [t for t in (corr, locs) if t is not None]
+        if nd:
+            ctx.mark_non_differentiable(*nd)
+        return out, corr, attn, locs
+
+    @staticmethod
+    def backward(ctx, g_out, g_corr, g_attn, g_locs):
+        feats, attn, locs = ctx.saved_tensors
+        o = ctx.opts
+        f = o["fwd"]
+        if not ctx.needs_input_grad[0]:
+            return None, None, None, None
+        if g_out is None:
+            g_out = torch.zeros(attn.shape[:3] + feats.shape[2:], device=feats.device, dtype=torch.float32)
+        g = epipolar_fusion_views_backward(
+            feats, None, attn, g_out, K=f["K"], downsample=f["downsample"], img_scale=f["img_scale"],
+            softmax_scale=f["softmax_scale"], correct_normalize=f["correct_normalize"], align_corners=f["align_corners"],
+            sources=ctx.sources, grad_attn=g_attn, sample_locs_in=locs, grad_keys=o["grad_keys"], grad_vals=o["grad_vals"],
+            deterministic=None)          # read torch's flag now, as PyTorch's own ops do in their backward
+        return g, None, None, None
 
 
 def fold_z_bn(z: nn.Conv2d, bn: nn.BatchNorm2d):
@@ -661,6 +777,40 @@ class Epipolar(nn.Module):
             want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
             state=self._state_for(first, "views"), sources=sources)
         return out, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
+
+    def forward_views_train(self, feats, P, sources=None):
+        """The differentiable counterpart of `forward_views`, for training from one backbone pass: every view of a frame is
+        fused with its sources (sources=None: every other view; a [V,S] host table, e.g. `multiview.nearest_view_table` with
+        topk=1: the views it names), and gradients reach `feats` (honouring cfg.EPIPOLAR.OTHER_GRAD) and z / bn.
+        feats [V,N,C,H,W] or V [N,C,H,W] maps, P [V,N,3,4].  Returns what `forward(feats[q], feats[u], P[q], P[u])` returns on
+        the gathered batch of V·S·N pairs in pair order ((v·S + j)·N + n: query view v, source u = its j-th source), shaped
+        (finalout [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attention [V,S,N,K,H,W] | None,
+        sample_locs [V,S,N,K,H,W,2] | None).  The z conv and BatchNorm stay PyTorch's, over the V·S·N pair items, in training and
+        eval mode; fuse_ref_residual adds feats[v] in PyTorch, as `forward` does under autograd."""
+        cfg = self.cfg
+        ep = cfg.EPIPOLAR
+        has_z = "z" in ep.PARAMETERIZED
+        want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+        if isinstance(feats, (list, tuple)):
+            feats = torch.stack(list(feats))
+        opts = dict(fwd=dict(K=self.sample_size, downsample=self.downsample,
+                             img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE,
+                             softmax_scale=ep.SOFTMAXSCALE, correct_normalize=ep.USE_CORRECT_NORMALIZE,
+                             align_corners=self.align_corners, want_corr=self.emit_corr, want_locs=want_locs,
+                             variant=self.variant),
+                    grad_keys="other1" in ep.OTHER_GRAD, grad_vals="other2" in ep.OTHER_GRAD)
+        out, corr, attn, locs = _ViewsFusionFn.apply(feats, P, sources, opts)
+        if not self.emit_attn:
+            attn = None
+        finalout = out
+        if has_z:
+            pairs = out.shape[:3]
+            finalout = self.bn(self.z(out.flatten(0, 2))).unflatten(0, pairs)
+            if ep.ZRESIDUAL:
+                finalout = finalout + out
+        if self.fuse_ref_residual:
+            finalout = finalout + feats[:, None]             # the pair's query view feats[v], over its S sources
+        return finalout, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
 
 
 def fused_other_feat(feat, other_features, KRT, other_KRT, sampler: Epipolar, camera=None, other_camera=None):

@@ -195,7 +195,7 @@ int epi_fusion_views(void);
  * stays keyed per pair by that pair's cameras, so a changed table on the same cache gives fresh-call results.
  * Duplicate entries are allowed.  EPI_EINVAL (with a message) for a NULL table, S < 1, n_views < 2, V·S > EPI_VIEW_SOURCES_MAX,
  * an entry outside [0, V), an entry equal to its own view (a self-pair), V·S·N > 65535 pairs, and every refusal of the views form.
- * No backward: the views forms are inference only. */
+ * Its backward is epi_fusion_views_backward_f32 below. */
 #define EPI_VIEW_SOURCES_MAX 256
 int epi_fusion_view_sources_forward_f32(const EpiFusionParams *p, const int32_t *sources_host, int32_t S, void *stream);
 /* Workspace / cache bytes of that call: V·N staged view items and V·S·N pairs.  0 when the table or params cannot be planned. */
@@ -203,6 +203,30 @@ size_t epi_fusion_view_sources_workspace_bytes(const EpiFusionParams *p, const i
 size_t epi_fusion_view_sources_cache_bytes(const EpiFusionParams *p, const int32_t *sources_host, int32_t S);
 /* 1: this library has the source-table entry points above (a library built before them lacks this symbol). */
 int epi_fusion_view_sources(void);
+
+/* ---- backward of the views form ---------------------------------------------------------------------------------------------
+ * The gradient of every view item of a frame, for the pairs of the views form (n_views = V, sources_host a [V][S] host table
+ * read as in epi_fusion_view_sources_forward_f32, or NULL with S = 0 for every other view, S = V−1).  Pair p = (v·S + j)·N + n
+ * fuses query item v·N + n with source item u·N + n, u = sources_host[v·S + j] (or j + (j >= v)).  Fields of p:
+ *   N                          items per view;
+ *   feat_ref / ref_stride      the V·N view maps [V·N,C,H,W] (feat_dtype), P_ref [V·N,3,4] (or sample_locs_in);
+ *   attn, grad_out, grad_attn, sample_locs_in    per pair: [V·S·N,K,H,W], [V·S·N,C,H,W], [V·S·N,K,H,W], [K,V·S·N,H,W,2];
+ *   grad_ref / gref_stride     out [V·N,C,H,W] (feat_dtype, the caller's strides), overwritten with
+ *                              dL/dfeats[i] = Σ over pairs p with query item i of dL/dfeat_ref(p)
+ *                                           + Σ over pairs p with source item i of dL/dfeat_src(p)   (grad_keys / grad_vals select
+ *                              the source terms, as in epi_fusion_backward_f32; with both 0 only the query terms remain);
+ *   feat_src, P_src, grad_src  must be NULL.
+ * Every term is what epi_fusion_backward_f32 computes for pair p; the sums are formed in fp32 and rounded once.  Each view map is
+ * staged once.  deterministic = 1: bit-reproducible, the source terms summed in int64 fixed point per item, with a scale set by
+ * the bounds of that item's pairs (so by its frame alone); an item one of whose pairs has a non-finite bound gets all NaN.  The
+ * query terms are summed in pair order on both paths.  EPI_EINVAL (with a message) for every refusal of epi_fusion_backward_f32,
+ * every table refusal of epi_fusion_view_sources_forward_f32, n_views < 2, more than 65535 pairs and a non-NULL
+ * feat_src / P_src / grad_src. */
+int epi_fusion_views_backward_f32(const EpiFusionBwdParams *p, int32_t n_views, const int32_t *sources_host, int32_t S, void *stream);
+/* Workspace bytes of that call (0 when the table or params cannot be planned). */
+size_t epi_fusion_views_backward_workspace_bytes(const EpiFusionBwdParams *p, int32_t n_views, const int32_t *sources_host, int32_t S);
+/* 1: this library has the views backward above (a library built before it lacks this symbol). */
+int epi_fusion_views_backward(void);
 
 /* Only the geometry: sample locations [K,N,H,W,2] for (P_ref,P_src)  (grid2sample_locs). */
 int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_locs_out, int32_t N,
@@ -244,7 +268,7 @@ float epi_kernel_timing_last_ms(void);
 /* same, per launch group: ms3[0] operand staging, ms3[1] fused attention kernel, ms3[2] epilogue pass */
 int epi_kernel_timing_last3(float *ms3);
 
-/* Number of kernels the last successful epi_fusion_forward_f32 or epi_fusion_backward_f32 on this thread launched. */
+/* Number of kernels the last successful forward or backward call on this thread launched. */
 int epi_last_launch_count(void);
 
 #ifdef __cplusplus
