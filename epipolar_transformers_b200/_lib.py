@@ -13,6 +13,13 @@ LIB_PATH = os.path.join(_HERE, "libepipolar_b200.so")
 
 EPI_ABI_VERSION = 3
 EPI_DTYPE_F32, EPI_DTYPE_BF16, EPI_DTYPE_F16 = 0, 1, 2
+
+
+def EPI_OUT_DTYPE(d):
+    """`out`'s element type in bits 8-15 of EpiFusionParams.feat_dtype (include/epipolar_b200.h): maps | EPI_OUT_DTYPE(out)"""
+    return d << 8
+
+
 EPI_VIEW_SOURCES_MAX = 256          # V·S entries of a source table (include/epipolar_b200.h)
 EPI_VARIANT_AUTO, EPI_VARIANT_WARP, EPI_VARIANT_TILE, EPI_VARIANT_SECTOR, EPI_VARIANT_PIPE = 0, 1, 2, 3, 4
 VARIANTS = {"auto": EPI_VARIANT_AUTO, "warp": EPI_VARIANT_WARP, "tile": EPI_VARIANT_TILE, "sector": EPI_VARIANT_SECTOR,

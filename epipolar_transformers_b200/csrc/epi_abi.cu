@@ -45,6 +45,11 @@ struct Launches {
     }
 };
 
+// EpiFusionParams.feat_dtype: the maps' element type in bits 0-7, `out`'s in bits 8-15 (EPI_OUT_DTYPE; 0 = float32)
+inline int map_dtype(const EpiFusionParams *p) { return p->feat_dtype & 0xff; }
+inline int out_dtype(const EpiFusionParams *p) { return (p->feat_dtype >> 8) & 0xff; }
+inline bool out_dtype_ok(const EpiFusionParams *p) { return (p->feat_dtype & ~0xffff) == 0 && out_dtype(p) <= EPI_DTYPE_F16; }
+
 // source views per reference item (EpiFusionParams.n_src: 0 and 1 both mean one)
 inline int n_sources(const EpiFusionParams *p) { return p->n_src > 1 ? p->n_src : 1; }
 // The views form's source table: every other view (S = 0) for epi_fusion_forward_f32, the caller's table for the
@@ -120,7 +125,9 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
     const size_t ref_map = (size_t)n_ref_items(p) * p->C * px * sizeof(float), map = NP * p->C * px * sizeof(float);
     const size_t src_map_bytes = (size_t)n_src_items(p) * p->C * px * sizeof(float);
     const size_t order_bytes = NP * px * sizeof(uint16_t), geom_bytes = NP * sizeof(epi::PairGeom);
-    const bool lowp = p->feat_dtype != EPI_DTYPE_F32, has_z = p->z_weight_folded != nullptr;
+    const bool lowp = map_dtype(p) != EPI_DTYPE_F32, has_z = p->z_weight_folded != nullptr;
+    // a 16-bit `out` is rounded by an epilogue pass from an fp32 plane: the fused kernels store fp32 only
+    const bool out16 = out_dtype(p) != EPI_DTYPE_F32;
     // sector tiles (pixels grouped by epipolar angle) need the fused geometry; injected locations and an explicit
     // EPI_VARIANT_TILE request use the 4x8 block tiles
     if (want_pipe(p)) pl.kernel = Kernel::Pipe;
@@ -137,12 +144,13 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         const bool out_direct = p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0 &&
                                 reinterpret_cast<uintptr_t>(p->out) % 16 == 0;
         pl.staging = Staging::Pipe;
-        pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32) : (out_direct ? Epilogue::Direct : Epilogue::Unstage);
+        pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32)
+                            : (out_direct && !out16 ? Epilogue::Direct : Epilogue::Unstage);
         if (lowp && pl.epilogue == Epilogue::ZFp32 && p->add_ref_residual) pl.ref_copy = RefCopy::After;   // the fp32 z epilogue's residual
         pl.cached = p->cache != nullptr;
         pl.item_px = g_items32 ? 32 : epi::fusion_pipe_item_pixels(p->C, p->H, p->W);
         // [ref_hi | ref_lo | src_hi | src_lo] bf16 planes; bf16 maps have no lo part: [ref_hi | src_hi]
-        const bool lo = p->feat_dtype != EPI_DTYPE_BF16;
+        const bool lo = map_dtype(p) != EPI_DTYPE_BF16;
         pl.ref_hi = ws.part(ref_map / 2);
         if (lo) pl.ref_lo = ws.part(ref_map / 2);
         if (!views) {
@@ -169,7 +177,7 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         // the tile kernel reads bf16 (hi, lo) planes; the warp kernel reads a channels-last fp32 source in place
         const bool tiles = pl.kernel != Kernel::Warp;
         pl.staging = tiles ? Staging::Planes : (!src_is_channels_last(p) || lowp ? Staging::Nhwc : Staging::InPlace);
-        pl.epilogue = has_z ? Epilogue::ZFp32 : Epilogue::Direct;
+        pl.epilogue = has_z ? Epilogue::ZFp32 : out16 ? Epilogue::Unstage : Epilogue::Direct;
         pl.ref_copy = lowp ? RefCopy::Before : RefCopy::None;        // these kernels read the query (and the residual) as fp32
         // views form: a low-precision map's fp32 copy is the warp kernel's source as it stands, and the sector tiles query the
         // source planes
@@ -177,7 +185,7 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         if (lowp) pl.ref32 = ws.take(ref_map);
         if (tiles) { pl.src_hi = ws.part(src_map_bytes / 2); pl.src_lo = ws.take(src_map_bytes / 2); }
         else if (pl.staging == Staging::Nhwc) pl.src_nhwc = ws.take(src_map_bytes);
-        if (has_z) pl.fused = ws.take(map);
+        if (pl.epilogue != Epilogue::Direct) pl.fused = ws.take(map);      // NCHW for the z epilogue, pixel-major for the transposition
         if (tiles) pl.counter = ws.take(256);
         if (pl.kernel == Kernel::Sector) {
             if (!views) { pl.ref_hi = ws.part(ref_map / 2); pl.ref_lo = ws.take(ref_map / 2); }
@@ -193,7 +201,7 @@ inline bool aligned8(const void *q) { return reinterpret_cast<uintptr_t>(q) % 8 
 
 // the size queries answer 0 for params no plan is made for
 bool plannable(const EpiFusionParams *p, const epi::ViewSources &vs) {
-    return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0 &&
+    return p && p->N > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->n_src >= 0 && out_dtype_ok(p) &&
            (p->n_views == 0 || (p->n_views >= 2 && p->n_views <= 256 && p->n_src <= 1 && n_pairs64(p, vs) <= 65535));
 }
 
@@ -237,7 +245,9 @@ int validate(const EpiFusionParams *p, const epi::ViewSources &vs) {
     if (!(p->downsample > 0.f) || !(p->img_scale > 0.f)) return fail(EPI_EINVAL, "downsample and img_scale must be positive");
     if (p->z_weight_folded && !p->z_bias_folded) return fail(EPI_EINVAL, "z_bias_folded required with z_weight_folded");
     if (p->variant < EPI_VARIANT_AUTO || p->variant > EPI_VARIANT_PIPE) return fail(EPI_EINVAL, "unknown variant");
-    if (p->feat_dtype < EPI_DTYPE_F32 || p->feat_dtype > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    if (p->feat_dtype & ~0xffff) return fail(EPI_EINVAL, "unknown feat_dtype: bits above 15 must be zero (bits 0-7: the maps' EPI_DTYPE_*, bits 8-15: EPI_OUT_DTYPE of out)");
+    if (map_dtype(p) > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown feat_dtype");
+    if (out_dtype(p) > EPI_DTYPE_F16) return fail(EPI_EINVAL, "unknown output dtype in feat_dtype bits 8-15 (EPI_OUT_DTYPE of EPI_DTYPE_F32, _BF16 or _F16)");
     if (p->n_src < 0) return fail(EPI_EINVAL, "n_src must be >= 0 (0 or 1: one source view per reference item)");
     if (p->n_src > 1 || p->n_views) {
         // the layout, transposition and z epilogue kernels put the item in the grid's z dimension; the pipelined kernel numbers
@@ -414,7 +424,7 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
         if (reinterpret_cast<uintptr_t>(p->cache) % 256 != 0) return fail(EPI_EINVAL, "cache must be 256-byte aligned");
     }
 
-    const int dt = p->feat_dtype;
+    const int dt = map_dtype(p), od = out_dtype(p);
     const int NP = n_pairs(p, vs);      // pairs: items of every output (and of feat_src unless n_views)
     const int NR = n_ref_items(p), V = p->n_views;
     const float *P_src = V ? p->P_ref : p->P_src;      // the views form takes both cameras of a pair from P_ref
@@ -504,7 +514,7 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
         (rc = run("reference conversion", epi::launch_nchw_to_nhwc(p->feat_ref, p->ref_stride, ref32, NR, p->C, p->H, p->W, dt, st)))) return rc;
     if (pl.epilogue == Epilogue::Unstage) {
         if ((rc = run("output transposition", epi::launch_unstage(a.out, p->add_ref_residual ? p->feat_ref : nullptr, dt, p->ref_stride, p->out,
-                                                                  EPI_DTYPE_F32, p->out_stride, NP, p->N, V, vs, p->C, p->H, p->W, st)))) return rc;
+                                                                  od, p->out_stride, NP, p->N, V, vs, p->C, p->H, p->W, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZGemm) {
         epi::ZGemmArgs z;
         memset(&z, 0, sizeof(z));
@@ -514,7 +524,7 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
         for (int i = 0; i < 4; i++) { z.y_stride[i] = p->out_stride[i]; z.ref_stride[i] = p->ref_stride[i]; }
         z.N = NP; z.n_ref = p->N; z.n_views = V; z.C = p->C; z.HW = p->H * p->W; z.W = p->W; z.Npad = p->C;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
-        if ((rc = run("z GEMM", epi::launch_zgemm(z, vs, st)))) return rc;
+        if ((rc = run("z GEMM", epi::launch_zgemm(z, vs, od, st)))) return rc;
     } else if (pl.epilogue == Epilogue::ZFp32) {
         epi::ZArgs z;
         memset(&z, 0, sizeof(z));
@@ -523,7 +533,7 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
         z.ref = ref32 ? ref32 : static_cast<const float *>(p->feat_ref); z.y = p->out; z.Wf = p->z_weight_folded; z.bf = p->z_bias_folded;
         z.N = NP; z.n_ref = p->N; z.n_views = V; z.vsrc = vs; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
-        if ((rc = run("z epilogue", epi::launch_z_epilogue(z, st)))) return rc;
+        if ((rc = run("z epilogue", epi::launch_z_epilogue(z, od, st)))) return rc;
     }
     if (g_timing) { cudaEventRecord(g_evB, st); g_timing_valid = 1; }
     g_launches = run.n;

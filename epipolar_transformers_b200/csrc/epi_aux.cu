@@ -136,16 +136,22 @@ static void unstage_t(dim3 grid, cudaStream_t st, const float *pm, const void *r
                                                  out_stride[1], out_stride[2], out_stride[3], n_ref, n_views, vs, C, H, W);
 }
 
+// without a residual TR is float and never read
+template <typename TO>
+static void unstage_out(dim3 grid, cudaStream_t st, const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out,
+                        const int64_t out_stride[4], int n_ref, int n_views, const ViewSources &vs, int C, int H, int W) {
+    if (ref && ref_dtype == kBF16) unstage_t<TO, __nv_bfloat16>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else if (ref && ref_dtype == kF16) unstage_t<TO, __half>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else unstage_t<TO, float>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+}
+
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
                            const int64_t out_stride[4], int N, int n_ref, int n_views, const ViewSources &vs, int C, int H, int W,
                            cudaStream_t st) {
     dim3 grid((H * W + 63) / 64, (C + 63) / 64, N);
-    if (out_dtype != kF32 && ref) return cudaErrorInvalidValue;           // a low-precision output is a gradient: no residual
-    if (out_dtype == kBF16) unstage_t<__nv_bfloat16, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
-    else if (out_dtype == kF16) unstage_t<__half, float>(grid, st, pm, nullptr, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
-    else if (ref_dtype == kBF16) unstage_t<float, __nv_bfloat16>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
-    else if (ref_dtype == kF16) unstage_t<float, __half>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
-    else unstage_t<float, float>(grid, st, pm, ref, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    if (out_dtype == kBF16) unstage_out<__nv_bfloat16>(grid, st, pm, ref, ref_dtype, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else if (out_dtype == kF16) unstage_out<__half>(grid, st, pm, ref, ref_dtype, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
+    else unstage_out<float>(grid, st, pm, ref, ref_dtype, ref_stride, out, out_stride, n_ref, n_views, vs, C, H, W);
     return cudaGetLastError();
 }
 
@@ -236,6 +242,8 @@ cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, c
 constexpr int ZT = 64, ZK = 16;
 
 // (min 5 blocks per SM: 48 registers.  Unbounded, ptxas spends 64 on the source-table branch of pair_items and a block fewer fits.)
+// TO: element type of y, the fp32 result rounded once
+template <typename TO>
 __global__ void __launch_bounds__(256, 5) z_epilogue_kernel(const ZArgs z) {
     __shared__ float Ws[ZK][ZT + 1];     // [k][o]
     __shared__ float Xs[ZK][ZT + 1];     // [k][p]
@@ -270,7 +278,7 @@ __global__ void __launch_bounds__(256, 5) z_epilogue_kernel(const ZArgs z) {
         }
         __syncthreads();
     }
-    float *Y = z.y + (int64_t)n * z.y_stride[0];
+    TO *Y = static_cast<TO *>(z.y) + (int64_t)n * z.y_stride[0];
     const float *R = z.ref ? z.ref + (int64_t)pair_items(n, z.n_ref, z.n_views, z.vsrc).q * z.ref_stride[0] : nullptr;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
@@ -285,14 +293,16 @@ __global__ void __launch_bounds__(256, 5) z_epilogue_kernel(const ZArgs z) {
             float v = acc[i][j] + b;
             if (z.z_residual) v += __ldg(X + o * z.x_stride[1] + yy * z.x_stride[2] + xx * z.x_stride[3]);
             if (z.add_ref && R) v += __ldg(R + o * z.ref_stride[1] + yy * z.ref_stride[2] + xx * z.ref_stride[3]);
-            Y[o * z.y_stride[1] + yy * z.y_stride[2] + xx * z.y_stride[3]] = v;
+            Y[o * z.y_stride[1] + yy * z.y_stride[2] + xx * z.y_stride[3]] = from_f32<TO>(v);
         }
     }
 }
 
-cudaError_t launch_z_epilogue(const ZArgs &z, cudaStream_t st) {
+cudaError_t launch_z_epilogue(const ZArgs &z, int y_dtype, cudaStream_t st) {
     dim3 grid((z.HW + ZT - 1) / ZT, (z.C + ZT - 1) / ZT, z.N);
-    z_epilogue_kernel<<<grid, 256, 0, st>>>(z);
+    if (y_dtype == kBF16) z_epilogue_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(z);
+    else if (y_dtype == kF16) z_epilogue_kernel<__half><<<grid, 256, 0, st>>>(z);
+    else z_epilogue_kernel<float><<<grid, 256, 0, st>>>(z);
     return cudaGetLastError();
 }
 

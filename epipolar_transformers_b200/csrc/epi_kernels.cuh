@@ -87,7 +87,7 @@ cudaError_t launch_views_grad_sum(const float *gq, const float *dsrc, const long
 struct ZArgs {
     const float *x;         int64_t x_stride[4];     // pre-z fused feature
     const float *ref;       int64_t ref_stride[4];   // may be null; item n reads ref item pair_items(n, n_ref, n_views, vsrc).q
-    float *y;               int64_t y_stride[4];
+    void *y;                int64_t y_stride[4];     // element type: launch_z_epilogue's y_dtype
     const float *Wf, *bf;
     int N, C, HW, W, n_ref, n_views;
     int z_residual, add_ref;
@@ -101,13 +101,14 @@ struct ZGemmArgs {
     const float *Wf, *bf;
     const void *ref;        int64_t ref_stride[4];   // element type ref_dtype
     int ref_dtype;
-    float *y;               int64_t y_stride[4];
+    void *y;                int64_t y_stride[4];     // element type: launch_zgemm's y_dtype
     int N, C, HW, W, Npad, n_ref, n_views;    // item n reads ref item pair_items(n, n_ref, n_views, vs).q
     int z_residual, add_ref;
 };
 bool zgemm_supported(int C);
-// vs: the views form's source table, the kernel's last parameter (behind the tensor maps)
-cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, cudaStream_t st);
+// vs: the views form's source table, the kernel's last parameter (behind the tensor maps); y_dtype (kF32 / kBF16 / kF16): element
+// type of y, the fp32 result rounded once
+cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, int y_dtype, cudaStream_t st);
 
 // vs: the views form's source table (vs.S = 0: none)
 cudaError_t launch_fusion_warp(const FusionArgs &a, const ViewSources &vs, cudaStream_t st);
@@ -136,8 +137,10 @@ cudaError_t launch_stage(const void *ref, const int64_t ref_stride[4], const voi
 
 cudaError_t launch_nchw_to_nhwc(const void *src, const int64_t stride[4], float *dst, int N, int C, int H, int W, int dtype,
                                 cudaStream_t st);
-cudaError_t launch_z_epilogue(const ZArgs &z, cudaStream_t st);
-// out_dtype != kF32 (a gradient rounded once) takes no residual; item n adds ref item pair_items(n, n_ref, n_views, vs).q
+// y_dtype (kF32 / kBF16 / kF16): element type of z.y, the fp32 result rounded once
+cudaError_t launch_z_epilogue(const ZArgs &z, int y_dtype, cudaStream_t st);
+// out_dtype (kF32 / kBF16 / kF16): fp32 sums rounded once (a gradient, or a 16-bit `out`); item n adds ref item
+// pair_items(n, n_ref, n_views, vs).q of element type ref_dtype when ref is not null
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
                            const int64_t out_stride[4], int N, int n_ref, int n_views, const ViewSources &vs, int C, int H, int W,
                            cudaStream_t st);

@@ -11,8 +11,9 @@
 // (hi, lo) planes [N·HW, C] (K-major rows) and Wf split to (hi, lo) while it is staged.  Three MMAs per
 // product (hi·hi + hi·lo + lo·hi), fp32 accumulation in registers (two warpgroups of M=64, N=128), K streamed in 64-channel
 // panels — the X and W panels arrive by TMA (cp.async.bulk.tensor.2d with the 128-byte swizzle the wgmma descriptors expect,
-// completion on an mbarrier); the epilogue adds bias/residuals and writes NCHW (a warp's lanes are 32 consecutive pixels, so
-// every store instruction is one 128-byte line per channel).
+// completion on an mbarrier); the epilogue adds bias/residuals and writes NCHW in y's type, fp32 or the fp32 result rounded once
+// to bf16 / fp16 (a warp's lanes are 32 consecutive pixels, so every store instruction is one 128-byte line per channel, 64
+// bytes for a 16-bit y).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -50,7 +51,21 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *t
 // maps, which a trailing parameter pack cannot follow here
 struct NoTable {};
 __device__ __forceinline__ PairItems pair_items(int p, int n_ref, int n_views, NoTable) { return pair_items(p, n_ref, n_views); }
-template <bool TABLE>
+
+// four consecutive fp32 results rounded once to TO, one streaming store (16 bytes for fp32, 8 for bf16 / fp16); p is aligned
+// to 4 elements
+__device__ __forceinline__ void st4_cs(float *p, float4 v) { __stcs(reinterpret_cast<float4 *>(p), v); }
+__device__ __forceinline__ void st4_cs(__nv_bfloat16 *p, float4 v) {
+    const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    __stcs(reinterpret_cast<uint2 *>(p), make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b)));
+}
+__device__ __forceinline__ void st4_cs(__half *p, float4 v) {
+    const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+    __stcs(reinterpret_cast<uint2 *>(p), make_uint2(*reinterpret_cast<const uint32_t *>(&a), *reinterpret_cast<const uint32_t *>(&b)));
+}
+
+// TO: element type of y (the fp32 result rounded once)
+template <bool TABLE, typename TO>
 __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z, const __grid_constant__ CUtensorMap tm_hi,
                                                               const __grid_constant__ CUtensorMap tm_lo,
                                                               const __grid_constant__ CUtensorMap tw_hi,
@@ -74,7 +89,7 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
     // output row of the epilogue (16 dependent round trips per warp).
     const bool addr = z.ref && z.add_ref;
     const bool vec = (z.y_stride[3] == 1) && (z.y_stride[2] == W) && (HW % 4 == 0) && (z.y_stride[1] % 4 == 0) && (z.y_stride[0] % 4 == 0) &&
-                     ((reinterpret_cast<uintptr_t>(z.y) & 15) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(z.y) & (4 * sizeof(TO) - 1)) == 0) &&
                      (!addr || ((z.ref_stride[3] == 1) && (z.ref_stride[2] == W) && (z.ref_stride[1] % 4 == 0) && (z.ref_stride[0] % 4 == 0) &&
                                 ((reinterpret_cast<uintptr_t>(z.ref) & (4 * feat_esize(z.ref_dtype) - 1)) == 0)));
     constexpr int ROWS = NB / (NT / 32);              // output rows per warp
@@ -162,14 +177,14 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
             const float b = bias[k];
             float y[4] = {t.x + b, t.y + b, t.z + b, t.w + b};
             if (vec && p + 3 < HW) {
-                __stcs(reinterpret_cast<float4 *>(z.y + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + p),     // written once, read by
-                       make_float4(y[0] + res[k].x, y[1] + res[k].y, y[2] + res[k].z, y[3] + res[k].w));               // nobody here: streaming
+                st4_cs(static_cast<TO *>(z.y) + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + p,     // written once, read by
+                       make_float4(y[0] + res[k].x, y[1] + res[k].y, y[2] + res[k].z, y[3] + res[k].w));       // nobody here: streaming
             } else {
                 for (int e = 0; e < 4 && p + e < HW; e++) {
                     const int py = (p + e) / W, px = (p + e) % W;
                     float val = y[e];
                     if (addr) val += ld_feat(z.ref, (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
-                    z.y[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = val;
+                    static_cast<TO *>(z.y)[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = from_f32<TO>(val);
                 }
             }
         }
@@ -206,10 +221,10 @@ bool make_plane_map(CUtensorMap *m, const __nv_bfloat16 *base, int rows, int C, 
 }
 }  // namespace
 
-template <bool TABLE>
+template <bool TABLE, typename TO>
 static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std::conditional_t<TABLE, ViewSources, NoTable> &vs) {
     const int tiles = (z.HW + 127) / 128;
-    const auto kern = epi_zgemm_kernel<TABLE>;
+    const auto kern = epi_zgemm_kernel<TABLE, TO>;
     static thread_local bool attr_set = false;
     if (!attr_set) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
@@ -229,8 +244,14 @@ static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std
     return launch_pdl(kern, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::NB - 1) / zg::NB)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3], vs);
 }
 
-cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, cudaStream_t st) {
-    return vs.S ? launch_zgemm_t<true>(z, st, vs) : launch_zgemm_t<false>(z, st, NoTable{});
+template <typename TO>
+static cudaError_t launch_zgemm_out(const ZGemmArgs &z, const ViewSources &vs, cudaStream_t st) {
+    return vs.S ? launch_zgemm_t<true, TO>(z, st, vs) : launch_zgemm_t<false, TO>(z, st, NoTable{});
+}
+
+cudaError_t launch_zgemm(const ZGemmArgs &z, const ViewSources &vs, int y_dtype, cudaStream_t st) {
+    return y_dtype == kBF16 ? launch_zgemm_out<__nv_bfloat16>(z, vs, st)
+         : y_dtype == kF16  ? launch_zgemm_out<__half>(z, vs, st) : launch_zgemm_out<float>(z, vs, st);
 }
 
 }  // namespace epi

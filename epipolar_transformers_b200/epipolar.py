@@ -48,10 +48,14 @@ def _aligned_locs(t: torch.Tensor) -> torch.Tensor:
 
 # element types the kernels read natively (EPI_DTYPE_*); bf16 / fp16 maps give the fp32 result of their exact values
 FEAT_DTYPES = {torch.float32: _lib.EPI_DTYPE_F32, torch.bfloat16: _lib.EPI_DTYPE_BF16, torch.float16: _lib.EPI_DTYPE_F16}
+_DTYPE_NAMES = {torch.float32: "float32", torch.bfloat16: "bfloat16", torch.float16: "float16"}
 
 
-def _check_feat_pair(feat_ref, feat_src, out=None):
-    """Both maps: 4-D, one supported dtype, on the GPU (a caller-supplied `out` must be float32).  -> EPI_DTYPE_* code."""
+def _check_feat_pair(feat_ref, feat_src, out=None, out_dtype=torch.float32):
+    """Both maps: 4-D, one supported dtype, on the GPU; `out_dtype` float32, bfloat16 or float16, and a caller-supplied `out` of
+    that dtype.  -> EPI_DTYPE_* code of the maps."""
+    if out_dtype not in FEAT_DTYPES:
+        raise TypeError("out_dtype must be torch.float32, torch.bfloat16 or torch.float16 (got %r)" % (out_dtype,))
     for name, t in (("feat_ref", feat_ref), ("feat_src", feat_src)):
         if not isinstance(t, torch.Tensor) or t.dim() != 4:
             raise ValueError("%s must be a 4-D tensor [N,C,H,W]" % name)
@@ -59,8 +63,11 @@ def _check_feat_pair(feat_ref, feat_src, out=None):
             raise TypeError("%s must be float32, bfloat16 or float16 (got %s)" % (name, t.dtype))
     if feat_ref.dtype != feat_src.dtype:
         raise TypeError("feat_ref and feat_src must have the same dtype (got %s and %s)" % (feat_ref.dtype, feat_src.dtype))
-    if out is not None and out.dtype != torch.float32:
-        raise TypeError("out must be float32 (got %s): the fused feature is computed and stored in float32" % out.dtype)
+    if out is not None and out.dtype != out_dtype:
+        if out_dtype == torch.float32:
+            raise TypeError("out must be float32 (got %s): the fused feature is computed and stored in float32, unless "
+                            "out_dtype asks for bfloat16 or float16" % out.dtype)
+        raise TypeError("out must be %s (got %s): out_dtype=%s" % (_DTYPE_NAMES[out_dtype], out.dtype, out_dtype))
     for name, t in (("feat_ref", feat_ref), ("feat_src", feat_src)):
         if not t.is_cuda:
             raise RuntimeError("%s is on %s: the CUDA epipolar path has no CPU implementation" % (name, t.device))
@@ -86,39 +93,42 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
                     softmax_scale=0.125, correct_normalize=False, align_corners=False,
                     z_folded=None, z_residual=False, add_ref_residual=False,
                     sample_locs_in=None, want_attn=True, want_corr=True, want_locs=False,
-                    variant="auto", out=None, state: Optional[FusionState] = None):
+                    variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32):
     """Functional form of the fused forward.  Returns (out, corr_pos|None, attn|None, sample_locs|None).
 
     feat_ref/feat_src: CUDA [N,C,H,W] (NCHW or channels_last strides), both float32, both bfloat16 or both float16 (what a
-      backbone under torch.autocast produces).  The result is the float32 computation on the exact input values, and every
-      output (including a caller-supplied `out`) is float32.
+      backbone under torch.autocast produces).  The result is the float32 computation on the exact input values.
+    out_dtype: dtype of `out` (and of a caller-supplied `out`): float32, or bfloat16 / float16, the float32 result rounded
+      once to nearest even (for a model cast to half precision).  corr_pos, attn and sample_locs are float32.
     P_ref/P_src: [N,3,4] (cast to float32 like modeling/model.py:183-195).
     z_folded: optional (Wf [C,C], bf [C]) from `fold_z_bn` (eval-mode epilogue, epipolar.py:249-253).
     sample_locs_in: optional [K,N,H,W,2] normalised locations replacing the fused geometry.
     state: optional FusionState (persistent workspace + camera-keyed cache); without it scratch is allocated per call.
     """
     lib = _lib.load()
-    dcode = _check_feat_pair(feat_ref, feat_src, out)
+    dcode = _check_feat_pair(feat_ref, feat_src, out, out_dtype)
     if feat_ref.shape != feat_src.shape or feat_ref.device != feat_src.device:
         raise ValueError("feat_ref and feat_src must have the same shape and device")
     return _fusion(lib, dcode, 1, feat_ref, feat_src, P_ref, P_src, K=K, downsample=downsample, img_scale=img_scale,
                    softmax_scale=softmax_scale, correct_normalize=correct_normalize, align_corners=align_corners,
                    z_folded=z_folded, z_residual=z_residual, add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in,
-                   want_attn=want_attn, want_corr=want_corr, want_locs=want_locs, variant=variant, out=out, state=state)
+                   want_attn=want_attn, want_corr=want_corr, want_locs=want_locs, variant=variant, out=out, state=state,
+                   out_dtype=out_dtype)
 
 
 def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4.0, img_scale=1.0,
                           softmax_scale=0.125, correct_normalize=False, align_corners=False,
                           z_folded=None, z_residual=False, add_ref_residual=False,
                           sample_locs_in=None, want_attn=True, want_corr=True, want_locs=False,
-                          variant="auto", out=None, state: Optional[FusionState] = None):
+                          variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32):
     """Fuses every reference item with S source views in one call: the multi-view test path of the reference
     (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239), where each reference batch is fused against every other view.
     Source s of item n gives exactly what `epipolar_fusion(feat_ref, feat_srcs[s], P_ref, P_srcs[s])` gives, but the
     reference map is staged once and the S pairs share one launch chain.
 
     feat_ref: [N,C,H,W] as in `epipolar_fusion`; feat_srcs: [S,N,C,H,W], or a sequence of S [N,C,H,W] maps (stacked);
-    P_ref: [N,3,4]; P_srcs: [S,N,3,4]; sample_locs_in: optional [K,S,N,H,W,2]; out: optional float32 [S,N,C,H,W].
+    P_ref: [N,3,4]; P_srcs: [S,N,3,4]; sample_locs_in: optional [K,S,N,H,W,2]; out: optional [S,N,C,H,W] of dtype out_dtype
+    (float32, or bfloat16 / float16 as in `epipolar_fusion`).
     Every residual (add_ref_residual, also under z) adds feat_ref[n].  Returns
     (out [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attn [S,N,K,H,W] | None, sample_locs [K,S,N,H,W,2] | None).
     Inference only (no backward for several sources): inputs that require grad under grad mode raise RuntimeError."""
@@ -154,7 +164,7 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
         if tuple(sample_locs_in.shape) != (K, S, N, H, W, 2):
             raise ValueError("sample_locs_in must be [K,S,N,H,W,2]")
         sample_locs_in = sample_locs_in.reshape(K, S * N, H, W, 2)
-    dcode = _check_feat_pair(feat_ref, feat_src, out4)
+    dcode = _check_feat_pair(feat_ref, feat_src, out4, out_dtype)
     if torch.is_grad_enabled() and (feat_ref.requires_grad or feat_src.requires_grad):
         raise RuntimeError("epipolar_fusion_multi is inference only (several sources have no backward); run it under "
                            "torch.no_grad(), or use epipolar_fusion (one source per call) for gradients")
@@ -162,7 +172,8 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
                                   img_scale=img_scale, softmax_scale=softmax_scale, correct_normalize=correct_normalize,
                                   align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
                                   add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
-                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state)
+                                  want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state,
+                                  out_dtype=out_dtype)
     return (out if out is not None else o.unflatten(0, (S, N)), None if corr is None else corr.unflatten(0, (S, N)),
             None if attn is None else attn.unflatten(0, (S, N)), None if locs is None else locs.unflatten(1, (S, N)))
 
@@ -196,7 +207,7 @@ def view_source_table(sources, V):
 def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax_scale=0.125, correct_normalize=False,
                           align_corners=False, z_folded=None, z_residual=False, add_ref_residual=False, sample_locs_in=None,
                           want_attn=True, want_corr=True, want_locs=False, variant="auto", out=None,
-                          state: Optional[FusionState] = None, sources=None):
+                          state: Optional[FusionState] = None, sources=None, out_dtype=torch.float32):
     """Fuses each view of a frame with several other views in one call, staging each view's map once.
 
     sources=None: every view with every other view, the whole multi-view test of the reference (cfg.EPIPOLAR.MULTITEST,
@@ -207,7 +218,7 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
     standard test (modeling/model.py:240-247) from one backbone pass.
 
     feats: [V,N,C,H,W], or a sequence of V [N,C,H,W] maps (stacked), V >= 2; P: [V,N,3,4]; sample_locs_in: optional
-    [K,V,S,N,H,W,2]; out: optional float32 [V,S,N,C,H,W].  Reference view v with its j-th source u gives, bit for bit, what
+    [K,V,S,N,H,W,2]; out: optional [V,S,N,C,H,W] of dtype out_dtype (float32, or bfloat16 / float16 as in `epipolar_fusion`).  Reference view v with its j-th source u gives, bit for bit, what
     `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every residual (add_ref_residual, also under z) adds feats[v][n].
     Returns (out [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attn [V,S,N,K,H,W] | None, sample_locs [K,V,S,N,H,W,2] | None).
     Inference only: inputs that require grad under grad mode raise RuntimeError.  `epipolar_fusion_views_backward` is its
@@ -249,7 +260,7 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
         if tuple(sample_locs_in.shape) != (K, V, S, N, H, W, 2):
             raise ValueError("sample_locs_in must be [K,V,%s,N,H,W,2]" % Sn)
         sample_locs_in = sample_locs_in.reshape(K, V * S * N, H, W, 2)
-    dcode = _check_feat_pair(feat, feat, out4)
+    dcode = _check_feat_pair(feat, feat, out4, out_dtype)
     if torch.is_grad_enabled() and feat.requires_grad:
         raise RuntimeError("epipolar_fusion_views is inference only; run it under torch.no_grad(), or use "
                            "Epipolar.forward_views_train (backward: epipolar_fusion_views_backward) for gradients")
@@ -258,7 +269,7 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
                                   align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
                                   add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
                                   want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state, views=V,
-                                  table=table)
+                                  table=table, out_dtype=out_dtype)
     pairs = (V, S, N)
     return (out if out is not None else o.unflatten(0, pairs), None if corr is None else corr.unflatten(0, pairs),
             None if attn is None else attn.unflatten(0, pairs), None if locs is None else locs.unflatten(1, pairs))
@@ -266,13 +277,14 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
 
 def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, img_scale, softmax_scale, correct_normalize,
             align_corners, z_folded, z_residual, add_ref_residual, sample_locs_in, want_attn, want_corr, want_locs, variant, out,
-            state, views=0, table=None):
+            state, views=0, table=None, out_dtype=torch.float32):
     """The forward of `epipolar_fusion` (S = 1) and `epipolar_fusion_multi`: feat_ref [N,C,H,W], feat_src / out [S·N,C,H,W],
     P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n).
     views = V >= 2 (`epipolar_fusion_views`): feat_ref [V·N,C,H,W] and P_ref [V·N,3,4] hold the views, feat_src and P_src are
     None, and the outputs have V·S·N items (pair p = (v·S + j)·N + n), S = V−1, or the width of `table` ([V,S] int32 host
-    array from `view_source_table`, which selects the source-table entry points)."""
+    array from `view_source_table`, which selects the source-table entry points).  out has dtype out_dtype."""
     NR, C, H, W = feat_ref.shape
+    ocode = FEAT_DTYPES[out_dtype]
     N = NR // views if views else NR
     NP = views * (views - 1 if table is None else table.shape[1]) * N if views else S * N
     dev = feat_ref.device
@@ -289,10 +301,10 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
     if out is None and views:                                            # the layout of a single call's empty_like(feat_src)
         cl = feat_ref.dim() == 4 and feat_ref.is_contiguous(memory_format=torch.channels_last) and not feat_ref.is_contiguous()
-        out = torch.empty((NP, C, H, W), device=dev, dtype=torch.float32,
+        out = torch.empty((NP, C, H, W), device=dev, dtype=out_dtype,
                           memory_format=torch.channels_last if cl else torch.contiguous_format)
     elif out is None:
-        out = torch.empty_like(feat_src, dtype=torch.float32)           # preserves NCHW / channels_last
+        out = torch.empty_like(feat_src, dtype=out_dtype)               # preserves NCHW / channels_last
     attn = torch.empty((NP, K, H, W), device=dev, dtype=torch.float32) if want_attn else None
     corr = torch.empty((NP, H, W, 2), device=dev, dtype=torch.float32) if want_corr else None
     locs = torch.empty((K, NP, H, W, 2), device=dev, dtype=torch.float32) if want_locs else None
@@ -301,7 +313,7 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     # the plan (and so the workspace size) also depends on whether `out` and feat_src start on a 16-byte boundary
     src_key = (feat_src.stride(), feat_src.data_ptr() % 16 == 0) if feat_src is not None else (feat_ref.data_ptr() % 16 == 0,)
     tkey = None if table is None else (table.shape, table.tobytes())
-    key = (dev, S, views, tkey, N, C, H, W, int(K), dcode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
+    key = (dev, S, views, tkey, N, C, H, W, int(K), dcode, ocode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
            z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
            bool(align_corners), bool(z_residual), bool(add_ref_residual))
@@ -318,7 +330,7 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
         p.align_corners = int(bool(align_corners)); p.correct_normalize = int(bool(correct_normalize))
         p.z_residual = int(bool(z_residual)); p.add_ref_residual = int(bool(add_ref_residual))
         p.variant = vcode
-        p.feat_dtype = dcode
+        p.feat_dtype = dcode | _lib.EPI_OUT_DTYPE(ocode)
         p.n_src = S if S > 1 else 0
         p.n_views = views
     p.feat_ref = feat_ref.data_ptr(); p.feat_src = feat_src.data_ptr() if feat_src is not None else None
@@ -503,7 +515,8 @@ def epipolar_fusion_views_backward(feats, P, attn, grad_out, *, K, downsample=4.
 
 class _FusionFn(torch.autograd.Function):
     """The fused attention under autograd (no z epilogue: conv/BN stay in PyTorch when gradients are needed).
-    The gradients of bfloat16 / float16 maps come back in their dtype.
+    The gradients of bfloat16 / float16 maps come back in their dtype; `out` has opts["fwd"]["out_dtype"] (float32 by
+    default), and its gradient is upcast to float32 for the backward kernels.
     The backward samples at the locations the forward emitted rather than re-deriving them from the cameras: the forward
     kernels round the line geometry differently, and with ill-conditioned cameras a recomputation moves samples by
     thousandths of a feature pixel, enough to put the gradients ~1e-3 (relative) off the function the forward computed."""
@@ -577,17 +590,19 @@ class _ViewsFusionFn(torch.autograd.Function):
 
 
 def fold_z_bn(z: nn.Conv2d, bn: nn.BatchNorm2d):
-    """(Wf, bf) such that BN_eval(z(x)) == Wf·x + bf, computed on the device (no host sync)."""
+    """(Wf, bf) such that BN_eval(z(x)) == Wf·x + bf, computed on the device (no host sync), always float32.  Parameters of a
+    module cast to bfloat16 / float16 (or held in any other layout) are read as their exact contiguous float32 upcast."""
     lib = _lib.load()
     C = z.out_channels
     dev = z.weight.device
     wf = torch.empty((C, z.in_channels), device=dev, dtype=torch.float32)
     bf = torch.empty((C,), device=dev, dtype=torch.float32)
-    zb = z.bias.data_ptr() if z.bias is not None else None
+    f32 = lambda t: None if t is None else t.detach().to(dtype=torch.float32).contiguous()      # no copy when already so
+    zw, zb, g, b, mean, var = map(f32, (z.weight, z.bias, bn.weight, bn.bias, bn.running_mean, bn.running_var))
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.epi_fold_z_bn_f32(z.weight.data_ptr(), zb, bn.weight.data_ptr(), bn.bias.data_ptr(),
-                                         bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), C,
+        _lib.check(lib.epi_fold_z_bn_f32(zw.data_ptr(), zb.data_ptr() if zb is not None else None, g.data_ptr(), b.data_ptr(),
+                                         mean.data_ptr(), var.data_ptr(), float(bn.eps), C,
                                          wf.data_ptr(), bf.data_ptr(), ctypes.c_void_p(stream)), "epi_fold_z_bn_f32")
     return wf, bf
 
@@ -620,6 +635,11 @@ class Epipolar(nn.Module):
 
     Under torch.use_deterministic_algorithms(True) the training backward is bit-reproducible (see
     `epipolar_fusion_backward`); the flag is read when the backward runs.  The z conv and BatchNorm stay PyTorch's.
+
+    The module follows the dtype it is cast to (`.to(torch.bfloat16)`, `.half()`, `.bfloat16()`): a 16-bit module returns
+    its fused feature in that dtype, the float32 result rounded once (in eval the folded epilogue stores it directly; under
+    autograd z, BatchNorm and the residual adds then run in the module's dtype).  A float32 module returns float32, with or
+    without torch.autocast.
     """
 
     def __init__(self, debug=False, *, cfg=None, align_corners=False, fuse_ref_residual=False, variant="auto",
@@ -660,6 +680,14 @@ class Epipolar(nn.Module):
             self.bn = ZeroInitBN(nf)
         self._fold_cache = None
         self._states = {}            # device -> FusionState (persistent workspace + camera-keyed cache)
+        # carries the dtype the module is cast to, which `out` takes; no elements and not persistent, so the state_dict keys
+        # stay the reference's
+        self.register_buffer("_dtype_probe", torch.empty(0, dtype=torch.float32), persistent=False)
+
+    @property
+    def out_dtype(self):
+        """dtype of the fused feature this module returns: the dtype it was cast to (float32, bfloat16 or float16)"""
+        return self._dtype_probe.dtype
 
     # -- eval-mode folding of z + BN, cached on parameter versions -------------------------------
     def _folded(self):
@@ -700,7 +728,7 @@ class Epipolar(nn.Module):
                                  img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE,
                                  softmax_scale=ep.SOFTMAXSCALE, correct_normalize=ep.USE_CORRECT_NORMALIZE,
                                  align_corners=self.align_corners, want_corr=self.emit_corr, want_locs=want_locs,
-                                 variant=self.variant),
+                                 variant=self.variant, out_dtype=self.out_dtype),
                         grad_keys="other1" in ep.OTHER_GRAD, grad_vals="other2" in ep.OTHER_GRAD)
             out, corr, attn, locs = _FusionFn.apply(feat1, feat2, P1, P2, opts)
             if not self.emit_attn:
@@ -714,7 +742,7 @@ class Epipolar(nn.Module):
                 z_residual=bool(ep.ZRESIDUAL) if fold else False,
                 add_ref_residual=self.fuse_ref_residual and (fold or not has_z),
                 want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
-                state=self._state_for(feat1))
+                state=self._state_for(feat1), out_dtype=self.out_dtype)
         if has_z and not fold:
             # training-mode BN needs batch statistics (+ autograd to z/bn): keep conv/BN in PyTorch
             finalout = self.bn(self.z(out))
@@ -749,7 +777,7 @@ class Epipolar(nn.Module):
             align_corners=self.align_corners, z_folded=self._folded() if has_z else None,
             z_residual=bool(ep.ZRESIDUAL) if has_z else False, add_ref_residual=self.fuse_ref_residual,
             want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
-            state=self._state_for(feat1, "multi"))
+            state=self._state_for(feat1, "multi"), out_dtype=self.out_dtype)
         return out, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
 
     def forward_views(self, feats, P, sources=None):
@@ -775,7 +803,7 @@ class Epipolar(nn.Module):
             align_corners=self.align_corners, z_folded=self._folded() if has_z else None,
             z_residual=bool(ep.ZRESIDUAL) if has_z else False, add_ref_residual=self.fuse_ref_residual,
             want_attn=self.emit_attn, want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant,
-            state=self._state_for(first, "views"), sources=sources)
+            state=self._state_for(first, "views"), sources=sources, out_dtype=self.out_dtype)
         return out, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
 
     def forward_views_train(self, feats, P, sources=None):
@@ -797,7 +825,7 @@ class Epipolar(nn.Module):
                              img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE,
                              softmax_scale=ep.SOFTMAXSCALE, correct_normalize=ep.USE_CORRECT_NORMALIZE,
                              align_corners=self.align_corners, want_corr=self.emit_corr, want_locs=want_locs,
-                             variant=self.variant),
+                             variant=self.variant, out_dtype=self.out_dtype),
                     grad_keys="other1" in ep.OTHER_GRAD, grad_vals="other2" in ep.OTHER_GRAD)
         out, corr, attn, locs = _ViewsFusionFn.apply(feats, P, sources, opts)
         if not self.emit_attn:

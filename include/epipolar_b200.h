@@ -15,7 +15,8 @@
  * Conventions: plain pointers + sizes, no torch types.  All tensor pointers are DEVICE
  * pointers to float32 unless a name ends in _host, except the feature maps feat_ref / feat_src and the backward's
  * grad_ref / grad_src, whose element type is the params' feat_dtype (EPI_DTYPE_*: float32, bfloat16 or float16; both maps
- * share it).  Every other output stays float32.  The library never allocates persistent
+ * share it), and the forward's `out`, whose element type is the output dtype in bits 8-15 of feat_dtype (EPI_OUT_DTYPE;
+ * float32 when they are zero).  Every other output stays float32.  The library never allocates persistent
  * device memory; the caller passes a workspace.  Every entry point is re-entrant, takes the
  * CUDA stream explicitly, never synchronises the device, and returns 0 on success or a
  * negative EPI_E* code (epi_last_error() gives a thread-local message).
@@ -51,6 +52,10 @@ extern "C" {
 #define EPI_DTYPE_F32 0
 #define EPI_DTYPE_BF16 1
 #define EPI_DTYPE_F16 2
+/* element type of the forward's `out`, in bits 8-15 of EpiFusionParams.feat_dtype: feat_dtype = maps | EPI_OUT_DTYPE(out).
+ * A bfloat16 or float16 `out` is the float32 result rounded once (to nearest even); attn, corr_pos and sample_locs_out stay
+ * float32.  A library that predates the byte refuses a nonzero one with EPI_EINVAL ("unknown feat_dtype"). */
+#define EPI_OUT_DTYPE(d) ((d) << 8)
 
 /* kernel variants (EpiFusionParams.variant) */
 #define EPI_VARIANT_AUTO 0    /* pipelined kernel when the shape allows, else sector / block tiles, else warp */
@@ -70,7 +75,8 @@ typedef struct EpiFusionParams {
     const float *sample_locs_in;  /* optional [K,N,H,W,2] contiguous, 8-byte aligned: normalised grid coords replacing the fused
                                      geometry (parity protocol T1: inject the reference's own locations) */
     /* ---- outputs --------------------------------------------------------------------- */
-    float *out;                   /* [N,C,H,W] logical, strides below, 4-byte aligned */
+    float *out;                   /* [N,C,H,W] logical, strides below, element type EPI_OUT_DTYPE of feat_dtype (float32 unless
+                                     bits 8-15 of feat_dtype say otherwise), aligned to its element size */
     int64_t out_stride[4];
     float *attn;                  /* optional [N,K,H,W] contiguous: softmax weights ("depth", epipolar.py:263) */
     float *corr_pos;              /* optional [N,H,W,2] contiguous, 8-byte aligned: arg-max correspondence, feature px (:237-242) */
@@ -92,7 +98,11 @@ typedef struct EpiFusionParams {
     int32_t z_residual;           /* cfg.EPIPOLAR.ZRESIDUAL (only with z_weight_folded) */
     int32_t add_ref_residual;     /* 1: also add feat_ref (the caller's `ret + feat`, resnet.py:388) */
     int32_t variant;              /* EPI_VARIANT_* */
-    int32_t feat_dtype;           /* EPI_DTYPE_* of feat_ref and feat_src (ABI v3; 0 = float32) */
+    int32_t feat_dtype;           /* bits 0-7: EPI_DTYPE_* of feat_ref and feat_src (ABI v3; 0 = float32).  bits 8-15:
+                                     EPI_OUT_DTYPE(EPI_DTYPE_*) of `out` (0 = float32, the only output type before the byte).  Bits above 15 must
+                                     be zero.  A 16-bit `out` always passes through an fp32 plane in the workspace, which the
+                                     epilogue (z GEMM, fp32 z epilogue or transposition pass) rounds once; the workspace grows by
+                                     that plane where the fused kernel would have stored `out` itself, and nothing else changes. */
     int32_t n_src;                /* source views per reference item, S = max(n_src, 1) (ABI v3; 0 or 1 = one source).  Pair
                                      p = s·N + n (0 <= s < S, 0 <= n < N) fuses reference item n with source item p:
                                      feat_ref / P_ref keep N items; feat_src is logical [S·N,C,H,W] (src_stride), P_src [S·N,3,4];
