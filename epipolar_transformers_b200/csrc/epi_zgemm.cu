@@ -5,15 +5,17 @@
 // restates  finalout = bn(z(out)) [+ out]   /root/reference/modeling/layers/epipolar.py:249-253 (eval-mode BN folded
 // into Wf, bf by epi_fold_z_bn_f32) and  ret + feat   /root/reference/modeling/backbones/resnet.py:388.
 //
-// One CTA per 128 pixels and block of 128 output channels (blockIdx.y); small CTAs (69 KB, one K panel in flight) so that several
-// are resident per SM and their load / MMA / store phases overlap each other:
-// D[128 px, C out] = X[128 px, C]·Wfᵀ with X supplied by the fusion kernel as bf16
-// (hi, lo) planes [N·HW, C] (K-major rows) and Wf split to (hi, lo) while it is staged.  Three MMAs per
-// product (hi·hi + hi·lo + lo·hi), fp32 accumulation in registers (two warpgroups of M=64, N=128), K streamed in 64-channel
-// panels — the X and W panels arrive by TMA (cp.async.bulk.tensor.2d with the 128-byte swizzle the wgmma descriptors expect,
-// completion on an mbarrier); the epilogue adds bias/residuals and writes NCHW in y's type, fp32 or the fp32 result rounded once
-// to bf16 / fp16 (a warp's lanes are 32 consecutive pixels, so every store instruction is one 128-byte line per channel, 64
-// bytes for a 16-bit y).
+// The product is computed transposed, Yᵀ[128 out-ch, 256 px] = (Wf + I)·Xᵀ per CTA (grid: pixel tiles of one item × blocks of
+// 128 output channels), so that an accumulator row is one output channel and its columns are consecutive pixels of one NCHW
+// row: each warp turns its fragments into whole row segments in a slice of the idle ring, with no CTA-wide tile or barrier
+// beyond one named barrier between the two MMA warpgroups.  Both operands are K-major as they lie in memory: the staged weight's
+// (hi, lo) planes [C out][C in] (MMA A, one warpgroup per 64 output channels) and the fused feature's (hi, lo) planes
+// [N·HW, C] (MMA B, N = 256 pixels).  Three MMAs per product (hi·hi + lo·hi + hi·lo), fp32 accumulation in registers.
+// K is streamed in 64-channel panels through a ring of STAGES shared-memory stages: one lane of a ninth warp issues the TMA
+// loads (cp.async.bulk.tensor.2d, 128-byte swizzle, completion on the stage's `full` mbarrier), the warpgroups issue panel q's
+// MMAs before they retire panel q-1's (wgmma.wait_group 1) and hand the stage back through its `empty` mbarrier, and the
+// loader refills it with panel q+1 while panel q multiplies.  The loader has a warp of its own because a loader branch inside
+// the MMA loop would make ptxas serialise the wgmmas (C7518).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -28,22 +30,26 @@ namespace epi {
 using namespace umma;
 
 namespace zg {
-constexpr int NT = 256;
-constexpr uint32_t A_PLANE = 16384;                 // 128 rows x 128 B
-constexpr int NB = 128;                             // output channels per CTA (MMA N)
-constexpr uint32_t B_PLANE = 16384;                 // 128 rows x 128 B
-constexpr uint32_t STAGE = 2 * A_PLANE + 2 * B_PLANE;   // 64 KB: one K panel of (A hi, A lo, W hi, W lo)
-constexpr int OT = 132;                             // epilogue tile pitch (floats)
-constexpr uint32_t TILE_BYTES = NB * OT * 4;        // 67 584 B: the epilogue tile re-uses the stage
-constexpr uint32_t BUF_BYTES = TILE_BYTES > STAGE ? TILE_BYTES : STAGE;
-constexpr uint32_t SMEM_ALLOC = BUF_BYTES + 1024 + 128;     // ~69 KB: up to three CTAs per SM by shared memory (two by registers)
+constexpr int NT = 288;                             // two MMA warpgroups and the loader warp
+constexpr int MO = 128;                             // output channels per CTA (MMA M: 64 per warpgroup)
+constexpr int NP = 256;                             // pixels per CTA (MMA N)
+constexpr uint32_t W_PLANE = MO * 128;              // 16 KB: 128 channel rows x 128 B
+constexpr uint32_t X_PLANE = NP * 128;              // 32 KB: 256 pixel rows x 128 B
+constexpr uint32_t STAGE = 2 * W_PLANE + 2 * X_PLANE;   // 96 KB: one K panel of (W hi, W lo, X hi, X lo)
+constexpr int STAGES = 2;
+constexpr int OP = NP + 8;                         // epilogue slice pitch (floats): two-way bank conflicts at most
+constexpr uint32_t SMEM_ALLOC = STAGES * STAGE + 1024 + 64;     // ~193 KB: one CTA per SM
 
-// 2-D tiled TMA load of a [128 rows x 64 bf16] box into a swizzled panel, completion counted on `bar`
+// 2-D tiled TMA load of a [box rows x 64 bf16] box into a swizzled panel, completion counted on `bar`
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tmap, int c0, int c1, uint64_t *bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
                      umma::smem_u32(smem_dst)),
                  "l"(tmap), "r"(c0), "r"(c1), "r"(umma::smem_u32(bar))
                  : "memory");
+}
+// a bounded wait: a phase that never completes (a lost TMA) traps instead of hanging the stream
+__device__ __forceinline__ void wait_or_trap(uint64_t *bar, uint32_t parity) {
+    for (uint32_t it = 0; !mbar_try_wait(bar, parity); ++it) if (it > (1u << 24)) __trap();
 }
 }  // namespace zg
 
@@ -66,7 +72,7 @@ __device__ __forceinline__ void st4_cs(__half *p, float4 v) {
 
 // TO: element type of y (the fp32 result rounded once)
 template <bool TABLE, typename TO>
-__global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z, const __grid_constant__ CUtensorMap tm_hi,
+__global__ void __launch_bounds__(zg::NT, 1) epi_zgemm_kernel(const ZGemmArgs z, const __grid_constant__ CUtensorMap tm_hi,
                                                               const __grid_constant__ CUtensorMap tm_lo,
                                                               const __grid_constant__ CUtensorMap tw_hi,
                                                               const __grid_constant__ CUtensorMap tw_lo,
@@ -74,118 +80,139 @@ __global__ void __launch_bounds__(zg::NT, 2) epi_zgemm_kernel(const ZGemmArgs z,
     using namespace zg;
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + BUF_BYTES);        // K panel landed (TMA)
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE);  // stage s holds its K panel (TMA)
+    uint64_t *empty = full + STAGES;                                         // every MMA warpgroup is done with stage s
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wg = warp >> 2, t128 = tid & 127;
     const int C = z.C, HW = z.HW, W = z.W;
-    const int tiles = (HW + 127) / 128;
-    const int n = blockIdx.x / tiles, p0 = (blockIdx.x % tiles) * 128;
-    const int nq = (C + 63) / 64;                      // K panels of 64 channels
-    const int oc0 = (int)blockIdx.y * NB;             // this CTA's block of output channels
-    const int CO = min(NB, C - oc0);
+    const int tiles = (HW + NP - 1) / NP;
+    const int n = blockIdx.x / tiles, p0 = (blockIdx.x % tiles) * NP;
+    const int nq = C / 64;                             // K panels of 64 channels
+    const int oc0 = (int)blockIdx.y * MO;             // this CTA's block of output channels
+    const int CO = min(MO, C - oc0);
+    const int nwg = CO > 64 ? 2 : 1;                   // warpgroups with output channels (C = 64 and a last block of 64 use one)
 
-    pdl_launch_dependents();
-    // The bias and the caller's residual (inputs of the whole forward, not products of the previous launches) are fetched into
-    // registers FIRST: their latency is paid under the previous kernel's tail and this kernel's main loop instead of once per
-    // output row of the epilogue (16 dependent round trips per warp).
-    const bool addr = z.ref && z.add_ref;
-    const bool vec = (z.y_stride[3] == 1) && (z.y_stride[2] == W) && (HW % 4 == 0) && (z.y_stride[1] % 4 == 0) && (z.y_stride[0] % 4 == 0) &&
-                     ((reinterpret_cast<uintptr_t>(z.y) & (4 * sizeof(TO) - 1)) == 0) &&
-                     (!addr || ((z.ref_stride[3] == 1) && (z.ref_stride[2] == W) && (z.ref_stride[1] % 4 == 0) && (z.ref_stride[0] % 4 == 0) &&
-                                ((reinterpret_cast<uintptr_t>(z.ref) & (4 * feat_esize(z.ref_dtype) - 1)) == 0)));
-    constexpr int ROWS = NB / (NT / 32);              // output rows per warp
-    float4 res[ROWS];
-    float bias[ROWS];
-    {
-        const int p = p0 + lane * 4;
-#pragma unroll
-        for (int k = 0; k < ROWS; k++) {
-            const int ol = warp + k * (NT / 32);
-            res[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-            bias[k] = ol < CO ? __ldg(z.bf + oc0 + ol) : 0.f;      // folded bias: written long before the staging launch
-            if (addr && vec && p + 3 < HW && ol < CO) {
-                const int64_t i = (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] + (int64_t)(oc0 + ol) * z.ref_stride[1] + p;     // the caller's map, in its type
-                res[k] = z.ref_dtype == kBF16 ? ld4_cs(static_cast<const __nv_bfloat16 *>(z.ref) + i)
-                       : z.ref_dtype == kF16  ? ld4_cs(static_cast<const __half *>(z.ref) + i)
-                                              : ld4_cs(static_cast<const float *>(z.ref) + i);
-            }
-        }
-    }
-    if (tid == 32) { mbar_init(bar, 1); mbar_fence_init(); }
-    if (tid == 64) {
+    // No pdl_launch_dependents(): the next forward's staging launch then starts when this grid completes.  Triggered early,
+    // its persistent CTAs were placed on the SMs this one-CTA-per-SM grid leaves partly free and made the bench.py step
+    // 5-6 µs longer (DESIGN.md §3.3).  This launch itself still starts under the fused kernel's tail (pdl_wait below).
+    if (tid == 0) {
+        for (int s = 0; s < STAGES; s++) { mbar_init(full + s, 1); mbar_init(empty + s, (uint32_t)nwg); }
+        mbar_fence_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tw_lo) : "memory");
     }
     __syncthreads();
-    pdl_wait();                                        // the fused kernel's feature planes
+    pdl_wait();                                        // the fused kernel's feature planes (and the staged weight)
+    // The loader (lane 0 of warp 8) loads K panel q into stage q % STAGES once the MMAs of panel q - STAGES have released it:
+    // W rows oc0 .. +127 (rows past C arrive zero-filled; a C of 64 is one 64-row box) and pixel rows n·HW + p0 .. +255 of the
+    // (hi, lo) planes (rows past N·HW zero-filled, rows of the next item computed and discarded).
+    const uint32_t wrows = (uint32_t)(C < MO ? C : MO);            // W box rows (the tensor map's box)
+    auto load = [&](int q) {
+        const int s = q % STAGES;
+        uint8_t *st = smem + s * STAGE;
+        mbar_arrive_expect_tx(full + s, 2 * wrows * 128u + 2 * X_PLANE);
+        tma_load_2d(st, &tw_hi, q * 64, oc0, full + s);
+        tma_load_2d(st + W_PLANE, &tw_lo, q * 64, oc0, full + s);
+        tma_load_2d(st + 2 * W_PLANE, &tm_hi, q * 64, n * HW + p0, full + s);
+        tma_load_2d(st + 2 * W_PLANE + X_PLANE, &tm_lo, q * 64, n * HW + p0, full + s);
+    };
+    if (warp == 8) {
+        if (lane == 0)
+            for (int q = 0; q < nq; q++) {
+                if (q >= STAGES) wait_or_trap(empty + q % STAGES, (uint32_t)(q / STAGES - 1) & 1u);
+                load(q);
+            }
+        return;
+    }
+    if (wg >= nwg) return;                             // no output channels for this warpgroup (and no barrier left to meet)
 
-    // Main loop: thread 0 issues the TMA loads of a K panel (A: 128 pixel rows x 64 channels of the (hi, lo) planes of x; B: NB output
-    // rows x 64 input channels of the (hi, lo) planes of Wf); warpgroup wg multiplies pixel rows 64 wg .. +63, three MMAs per
-    // 16-channel step, and waits for them before the panel is reloaded.  Output columns >= CO are computed and discarded.
-    const int wg = warp >> 2, t128 = tid & 127;
-    float acc[64];
+    // Main loop: warpgroup wg multiplies output channels oc0 + 64 wg .. +63 by the CTA's 256 pixels.  Every element's sum runs
+    // over K in one fixed order (panel, 16-channel step, hi·hi, lo·hi, hi·lo), whatever the tile, grid or batch.
+    float acc[128];
 #pragma unroll
-    for (int e = 0; e < 64; e++) acc[e] = 0.f;
-    {
-        const uint32_t wrows = (uint32_t)(C < NB ? C : NB);            // W box rows (the tensor map's box)
-        for (int q = 0; q < nq; q++) {
-            if (tid == 0) {
-                mbar_arrive_expect_tx(bar, 2 * A_PLANE + 2 * wrows * 128u);
-                tma_load_2d(smem, &tm_hi, q * 64, n * HW + p0, bar);
-                tma_load_2d(smem + A_PLANE, &tm_lo, q * 64, n * HW + p0, bar);
-                tma_load_2d(smem + 2 * A_PLANE, &tw_hi, q * 64, oc0, bar);
-                tma_load_2d(smem + 2 * A_PLANE + B_PLANE, &tw_lo, q * 64, oc0, bar);
-            }
-            for (uint32_t it = 0; !mbar_try_wait(bar, q & 1); ++it) if (it > (1u << 24)) __trap();
-            const uint32_t sa = smem_u32(smem) + (uint32_t)wg * 8192u, sb = smem_u32(smem) + 2 * A_PLANE;
-            wg_fence();
+    for (int e = 0; e < 128; e++) acc[e] = 0.f;
+    for (int q = 0; q < nq; q++) {
+        const int s = q % STAGES;
+        wait_or_trap(full + s, (uint32_t)(q / STAGES) & 1u);
+        const uint32_t sa = smem_u32(smem + s * STAGE) + (uint32_t)wg * 8192u, sb = smem_u32(smem + s * STAGE) + 2 * W_PLANE;
+        wg_fence();
 #pragma unroll
-            for (int ks = 0; ks < 4; ks++) {
-                const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = desc_add(a_hi, A_PLANE);
-                const uint64_t b_hi = make_smem_desc(sb + ks * 32, 16, 1024), b_lo = desc_add(b_hi, B_PLANE);
-                wgmma_m64n128<0>(acc, a_hi, b_hi);
-                wgmma_m64n128<0>(acc, a_hi, b_lo);
-                wgmma_m64n128<0>(acc, a_lo, b_hi);
-            }
-            wg_commit();
-            wg_wait_all();
-            __syncthreads();                           // both warpgroups are done with the panel
+        for (int ks = 0; ks < 4; ks++) {
+            const uint64_t a_hi = make_smem_desc(sa + ks * 32, 16, 1024), a_lo = desc_add(a_hi, W_PLANE);
+            const uint64_t b_hi = make_smem_desc(sb + ks * 32, 16, 1024), b_lo = desc_add(b_hi, X_PLANE);
+            wgmma_m64n256<0>(acc, a_hi, b_hi);
+            wgmma_m64n256<0>(acc, a_lo, b_hi);
+            wgmma_m64n256<0>(acc, a_hi, b_lo);
         }
+        wg_commit();
+        wg_wait_1();                                   // panel q-1's MMAs have retired; panel q's run on
+        if (q > 0 && t128 == 0) mbar_arrive(empty + (q - 1) % STAGES);
     }
+    wg_wait_all();
 
-    // ---- epilogue ------------------------------------------------------------------------------------------------
-    // phase 1 (accumulator fragments): registers -> shared tile [channel][128 pixels] (the operand stage is free now).
-    //   The ZRESIDUAL needs no pass: the staged weight is Wf + I;
-    // phase 2 (warp <-> channel row, lane <-> 4 consecutive pixels): + bias + caller residual, 512-byte row segments of the NCHW output
-    //   per warp instruction.  Falls back to per-element addressing for strides that are not pixel-contiguous.
-    float *otile = reinterpret_cast<float *>(smem);            // [NB][132] fp32 over the (now idle) stage
+    // ---- epilogue -> NCHW --------------------------------------------------------------------------------------------
+    // Thread t128 holds output channels r and r + 8 (r = acc_row(t128, 0)) at pixel pairs p0 + 8j + 2(t128 & 3), j = 0..31.
+    // Vector path: each warp passes its 16 channel rows x 256 pixels through a private slice of the (now idle) ring, so that
+    // every store instruction writes 512 contiguous bytes of one channel row (for fp32; 256 for a 16-bit y), as full 128-byte
+    // lines: stored straight from the fragments, four lanes cover only 32 bytes of a row, and the partly written lines cost
+    // step time (measured).  The ZRESIDUAL needs no term: the staged weight is Wf + I.  The bias and the caller's residual are
+    // read here, not held across the main loop.  Strides that are not pixel-contiguous take per-element stores from the fragments.
+    const bool addr = z.ref && z.add_ref;
+    const bool vec = (z.y_stride[3] == 1) && (z.y_stride[2] == W) && (HW % 4 == 0) && (z.y_stride[1] % 4 == 0) && (z.y_stride[0] % 4 == 0) &&
+                     ((reinterpret_cast<uintptr_t>(z.y) & (4 * sizeof(TO) - 1)) == 0) &&
+                     (!addr || ((z.ref_stride[3] == 1) && (z.ref_stride[2] == W) && (z.ref_stride[1] % 4 == 0) && (z.ref_stride[0] % 4 == 0) &&
+                                ((reinterpret_cast<uintptr_t>(z.ref) & (4 * feat_esize(z.ref_dtype) - 1)) == 0)));
+    const int64_t qref = addr ? (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] : 0;
+    if (vec) {
+        asm volatile("bar.sync 1, %0;" ::"r"(nwg * 128) : "memory");     // every MMA warpgroup is done reading the ring
+        float *buf = reinterpret_cast<float *>(smem) + (wg * 4 + (warp & 3)) * (16 * OP);   // this warp's [16][OP] slice
 #pragma unroll
-    for (int e = 0; e < 64; e++) {
-        const int col = acc_col(t128, e);
-        if (col < CO) otile[col * OT + wg * 64 + acc_row(t128, e)] = acc[e];
-    }
-    __syncthreads();
-    {
-        const int pp = lane * 4, p = p0 + pp;
+        for (int e = 0; e < 128; e += 2)
+            *reinterpret_cast<float2 *>(buf + acc_row(lane, e) * OP + acc_col(lane, e)) = make_float2(acc[e], acc[e + 1]);
+        __syncwarp();
+        const int rw = wg * 64 + (warp & 3) * 16;      // the warp's first channel row in the CTA's block
+        for (int lr = 0; lr < 16 && rw + lr < CO; lr++) {
+            const int o = oc0 + rw + lr;
+            const float b = __ldg(z.bf + o);           // folded bias: written long before the staging launch
+            TO *yrow = static_cast<TO *>(z.y) + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1];
 #pragma unroll
-        for (int k = 0; k < ROWS; k++) {
-            const int ol = warp + k * (NT / 32);
-            if (ol >= CO) break;
-            const int o = oc0 + ol;
-            const float4 t = *reinterpret_cast<const float4 *>(otile + ol * OT + pp);
-            const float b = bias[k];
-            float y[4] = {t.x + b, t.y + b, t.z + b, t.w + b};
-            if (vec && p + 3 < HW) {
-                st4_cs(static_cast<TO *>(z.y) + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + p,     // written once, read by
-                       make_float4(y[0] + res[k].x, y[1] + res[k].y, y[2] + res[k].z, y[3] + res[k].w));       // nobody here: streaming
-            } else {
-                for (int e = 0; e < 4 && p + e < HW; e++) {
-                    const int py = (p + e) / W, px = (p + e) % W;
-                    float val = y[e];
-                    if (addr) val += ld_feat(z.ref, (int64_t)pair_items(n, z.n_ref, z.n_views, vs).q * z.ref_stride[0] + (int64_t)o * z.ref_stride[1] + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
-                    static_cast<TO *>(z.y)[(int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1] + (int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = from_f32<TO>(val);
+            for (int half = 0; half < 2; half++) {
+                const int pp = half * 128 + lane * 4, p = p0 + pp;
+                if (p >= HW) break;                    // HW % 4 == 0: p < HW covers p + 3
+                const float4 t = *reinterpret_cast<const float4 *>(buf + lr * OP + pp);
+                float4 v = make_float4(t.x + b, t.y + b, t.z + b, t.w + b);
+                if (addr) {
+                    const int64_t i = qref + (int64_t)o * z.ref_stride[1] + p;      // the caller's map, in its type
+                    const float4 rv = z.ref_dtype == kBF16 ? ld4_cs(static_cast<const __nv_bfloat16 *>(z.ref) + i)
+                                    : z.ref_dtype == kF16  ? ld4_cs(static_cast<const __half *>(z.ref) + i)
+                                                           : ld4_cs(static_cast<const float *>(z.ref) + i);
+                    v = make_float4(v.x + rv.x, v.y + rv.y, v.z + rv.z, v.w + rv.w);
                 }
+                st4_cs(yrow + p, v);
+            }
+        }
+        return;
+    }
+    const int r = wg * 64 + acc_row(t128, 0), pc = p0 + ((t128 & 3) << 1);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int ol = r + 8 * h;
+        if (ol >= CO) continue;
+        const int o = oc0 + ol;
+        const float b = __ldg(z.bf + o);
+        TO *yrow = static_cast<TO *>(z.y) + (int64_t)n * z.y_stride[0] + (int64_t)o * z.y_stride[1];
+        const int64_t rrow = qref + (int64_t)o * z.ref_stride[1];
+#pragma unroll
+        for (int j = 0; j < 32; j++) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int p = pc + 8 * j + e;
+                if (p >= HW) continue;
+                const int py = p / W, px = p % W;
+                float val = acc[4 * j + 2 * h + e] + b;
+                if (addr) val += ld_feat(z.ref, rrow + (int64_t)py * z.ref_stride[2] + (int64_t)px * z.ref_stride[3], z.ref_dtype);
+                yrow[(int64_t)py * z.y_stride[2] + (int64_t)px * z.y_stride[3]] = from_f32<TO>(val);
             }
         }
     }
@@ -223,7 +250,7 @@ bool make_plane_map(CUtensorMap *m, const __nv_bfloat16 *base, int rows, int C, 
 
 template <bool TABLE, typename TO>
 static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std::conditional_t<TABLE, ViewSources, NoTable> &vs) {
-    const int tiles = (z.HW + 127) / 128;
+    const int tiles = (z.HW + zg::NP - 1) / zg::NP;
     const auto kern = epi_zgemm_kernel<TABLE, TO>;
     static thread_local bool attr_set = false;
     if (!attr_set) {
@@ -235,13 +262,13 @@ static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std
     struct MapCache { const void *xh, *wh; int rows, C; CUtensorMap m[4]; };
     static thread_local MapCache mc = {nullptr, nullptr, 0, 0, {}};
     if (mc.xh != z.x_hi || mc.wh != z.w_hi || mc.rows != z.N * z.HW || mc.C != z.C) {
-        const int wrows = z.C < zg::NB ? z.C : zg::NB;
-        if (!make_plane_map(&mc.m[0], z.x_hi, z.N * z.HW, z.C, 128) || !make_plane_map(&mc.m[1], z.x_lo, z.N * z.HW, z.C, 128) ||
+        const int wrows = z.C < zg::MO ? z.C : zg::MO;
+        if (!make_plane_map(&mc.m[0], z.x_hi, z.N * z.HW, z.C, zg::NP) || !make_plane_map(&mc.m[1], z.x_lo, z.N * z.HW, z.C, zg::NP) ||
             !make_plane_map(&mc.m[2], z.w_hi, z.C, z.C, wrows) || !make_plane_map(&mc.m[3], z.w_lo, z.C, z.C, wrows))
             return cudaErrorInvalidValue;
         mc.xh = z.x_hi; mc.wh = z.w_hi; mc.rows = z.N * z.HW; mc.C = z.C;
     }
-    return launch_pdl(kern, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::NB - 1) / zg::NB)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3], vs);
+    return launch_pdl(kern, dim3((unsigned)(z.N * tiles), (unsigned)((z.C + zg::MO - 1) / zg::MO)), dim3(zg::NT), (size_t)zg::SMEM_ALLOC, st, z, mc.m[0], mc.m[1], mc.m[2], mc.m[3], vs);
 }
 
 template <typename TO>
