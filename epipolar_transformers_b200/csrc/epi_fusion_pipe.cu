@@ -1084,12 +1084,13 @@ static cudaError_t launch_items(const FusionArgs &a, cudaStream_t st, const Tab 
     void (*kern)(const FusionArgs, const Tab...) =
         lo ? (kpl <= 1 ? epi_fusion_pipe_kernel<1, true, P, Tab...> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, true, P, Tab...> : epi_fusion_pipe_kernel<4, true, P, Tab...>))
            : (kpl <= 1 ? epi_fusion_pipe_kernel<1, false, P, Tab...> : (kpl <= 2 ? epi_fusion_pipe_kernel<2, false, P, Tab...> : epi_fusion_pipe_kernel<4, false, P, Tab...>));
-    static thread_local bool attr_set[6] = {false, false, false, false, false, false};
+    static thread_local DeviceFlags attr_set[6];
     const int ki = (kpl <= 1 ? 0 : (kpl <= 2 ? 1 : 2)) + (lo ? 0 : 3);
-    if (!attr_set[ki]) {
+    const int dev = current_device();
+    if (!attr_set[ki].has(dev)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_alloc<P>());
         if (e != cudaSuccess) return e;
-        attr_set[ki] = true;
+        attr_set[ki].set(dev);
     }
     const int sms = sm_count();
     const int grid = tiles < sms ? tiles : sms;                    // one persistent CTA per SM

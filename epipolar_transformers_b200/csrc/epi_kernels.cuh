@@ -6,15 +6,32 @@
 
 namespace epi {
 
-// SMs of the current device, for persistent grids: queried once per host thread, 132 (an H100 SXM) if the query fails
+// Host-side caches of per-device facts.  cudaFuncSetAttribute and the SM count concern the current device, so a host thread that
+// runs the library on several devices keeps one entry per device; devices from kMaxDevices on are not cached (queried or set on
+// every call).
+constexpr int kMaxDevices = 64;
+inline int current_device() {
+    int dev = 0;
+    return cudaGetDevice(&dev) == cudaSuccess ? dev : 0;
+}
+
+// one bit per device: whether a one-time setting (a kernel's shared-memory attribute) has been applied on that device
+struct DeviceFlags {
+    uint64_t bits = 0;
+    bool has(int dev) const { return dev < kMaxDevices && ((bits >> dev) & 1u); }
+    void set(int dev) { if (dev < kMaxDevices) bits |= 1ull << dev; }
+};
+
+// SMs of the current device, for persistent grids: queried once per host thread and device, 132 (an H100 SXM) if the query fails
 inline int sm_count() {
-    static thread_local int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    static thread_local int sms[kMaxDevices] = {};
+    const int dev = current_device();
+    int n = dev < kMaxDevices ? sms[dev] : 0;
+    if (!n) {
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+        if (dev < kMaxDevices) sms[dev] = n;
     }
-    return sms;
+    return n;
 }
 
 // Device-side view of one fused forward (built from EpiFusionParams by the ABI layer).

@@ -456,12 +456,15 @@ static cudaError_t launch_stage_t(const T *ref, const int64_t ref_stride[4], con
     const size_t smem_order = (size_t)stg::NBIN * 4 + (size_t)H * W * 2;
     const bool multi = n_ref != N || n_views;
     void (*kern)(const StageArgs<T>, const Tab...) = multi ? epi_stage_kernel<T, true, Tab...> : epi_stage_kernel<T, false, Tab...>;
-    static thread_local size_t smem_set[2] = {0, 0};
+    static thread_local size_t smem_set[kMaxDevices][2] = {};           // per device: the attribute applies to the current one
+    const int dev = current_device();
+    size_t uncached[2] = {0, 0};
+    size_t *set = dev < kMaxDevices ? smem_set[dev] : uncached;
     auto ensure = [&](size_t smem) -> cudaError_t {
-        if (smem + 1024 > 48 * 1024 && smem > smem_set[multi]) {        // (+ the kernel's small static arrays)
+        if (smem + 1024 > 48 * 1024 && smem > set[multi]) {             // (+ the kernel's small static arrays)
             cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
-            smem_set[multi] = smem;
+            set[multi] = smem;
         }
         return cudaSuccess;
     };

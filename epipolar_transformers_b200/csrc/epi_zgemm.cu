@@ -252,11 +252,12 @@ template <bool TABLE, typename TO>
 static cudaError_t launch_zgemm_t(const ZGemmArgs &z, cudaStream_t st, const std::conditional_t<TABLE, ViewSources, NoTable> &vs) {
     const int tiles = (z.HW + zg::NP - 1) / zg::NP;
     const auto kern = epi_zgemm_kernel<TABLE, TO>;
-    static thread_local bool attr_set = false;
-    if (!attr_set) {
+    static thread_local DeviceFlags attr_set;
+    const int dev = current_device();
+    if (!attr_set.has(dev)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)zg::SMEM_ALLOC);
         if (e != cudaSuccess) return e;
-        attr_set = true;
+        attr_set.set(dev);
     }
     // tensor maps are a pure function of (pointers, shape): keep the last set per host thread
     struct MapCache { const void *xh, *wh; int rows, C; CUtensorMap m[4]; };

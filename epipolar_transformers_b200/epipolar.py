@@ -691,6 +691,11 @@ class Epipolar(nn.Module):
 
     # -- eval-mode folding of z + BN, cached on parameter versions -------------------------------
     def _folded(self):
+        if torch.cuda.is_current_stream_capturing():
+            # A CUDA graph folds inside itself (one launch per replay, reading the parameters in place): it then holds no
+            # pointer to the cache below, which an eager call frees when a parameter changes, and no wait on an event recorded
+            # outside the capture (which CUDA refuses), and its replays follow in-place parameter updates as eager calls do.
+            return fold_z_bn(self.z, self.bn)
         ts = (self.z.weight, self.z.bias, self.bn.weight, self.bn.bias, self.bn.running_mean, self.bn.running_var)
         key = tuple((t.data_ptr(), t._version) for t in ts if t is not None)
         dev = self.z.weight.device
