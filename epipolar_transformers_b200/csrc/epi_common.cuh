@@ -257,6 +257,11 @@ __device__ __forceinline__ float sdiv(float v, float eps) {       // sign(v)*max
 
 // Endpoints (image coords) of the epipolar line of reference pixel (px,py) clipped to the
 // pixel-centre rectangle; far sentinel when fewer than two valid intersections (:369-405).
+// A pixel whose ray is parallel to the source image plane has zz == 0 (exactly, when the fp32 constants cancel): x2 is
+// then a point at infinity and l2 is not finite (also when a quotient overflows).  Its line is e2 × (zx, zy, zz), the
+// zz → 0 limit of e2 × x2 up to the factor 1/zz; that factor grows without bound, so in the limit the eps clamp of the
+// denominators never acts on a non-zero component, and the homogeneous line is clipped without it.  Every pixel with a
+// finite l2 takes the quotient form unchanged.
 __device__ __forceinline__ void line_endpoints(const PairGeom &g, const GeomCfg &c, float px, float py,
                                                float &sx, float &sy, float &ex, float &ey) {
     float zx = g.M[0] * px + g.M[1] * py + g.M[2];
@@ -264,7 +269,12 @@ __device__ __forceinline__ void line_endpoints(const PairGeom &g, const GeomCfg 
     float zz = g.M[6] * px + g.M[7] * py + g.M[8];
     float x2 = zx / zz, y2 = zy / zz;
     float l0 = g.ey - y2, l1 = x2 - g.ex, l2 = g.ex * y2 - g.ey * x2;    // e2 × x2, both with z = 1
-    float d1 = sdiv(l1, c.eps), d0 = sdiv(l0, c.eps);
+    float clamp = c.eps;
+    if (!(fabsf(l2) <= 3.402823466e38f)) {                               // x2 not finite: e2 × (zx, zy, zz)
+        l0 = g.ey * zz - zy; l1 = zx - g.ex * zz; l2 = g.ex * zy - g.ey * zx;
+        clamp = 0.f;
+    }
+    float d1 = sdiv(l1, clamp), d0 = sdiv(l0, clamp);
     float by1 = -(c.xmin * l0 + l2) / d1;
     float by2 = -(c.xmax * l0 + l2) / d1;
     float bx0 = -(c.ymin * l1 + l2) / d0;

@@ -46,13 +46,14 @@ static void pair_constants(const double *P1, const double *P2, double *M, double
     double z = e2[2]; e2[0] /= z; e2[1] /= z; e2[2] = 1.0;
 }
 
-static double sd(double v) { double a = fabs(v) > EPS_ ? fabs(v) : EPS_; return v > 0 ? a : (v < 0 ? -a : 0.0 * a); }
-static float sdf(float v) { float a = fabsf(v) > (float)EPS_ ? fabsf(v) : (float)EPS_; return v > 0 ? a : (v < 0 ? -a : 0.0f * a); }
+static double sd(double v, double c) { double a = fabs(v) > c ? fabs(v) : c; return v > 0 ? a : (v < 0 ? -a : 0.0 * a); }
+static float sdf(float v, float c) { float a = fabsf(v) > c ? fabsf(v) : c; return v > 0 ? a : (v < 0 ? -a : 0.0f * a); }
 
-/* line clipping (epipolar.py:369-405): endpoints S,E in image coordinates */
-static void clip_d(const double *l, double xmin, double xmax, double ymin, double ymax, double *S, double *E) {
-    double by1 = -(xmin * l[0] + l[2]) / sd(l[1]), by2 = -(xmax * l[0] + l[2]) / sd(l[1]);
-    double bx0 = -(ymin * l[1] + l[2]) / sd(l[0]), bx3 = -(ymax * l[1] + l[2]) / sd(l[0]);
+/* line clipping (epipolar.py:369-405): endpoints S,E in image coordinates; `c` clamps the denominators (EPS_, or 0 for the
+   homogeneous line of a ray parallel to the source image plane, see line_d) */
+static void clip_d(const double *l, double c, double xmin, double xmax, double ymin, double ymax, double *S, double *E) {
+    double by1 = -(xmin * l[0] + l[2]) / sd(l[1], c), by2 = -(xmax * l[0] + l[2]) / sd(l[1], c);
+    double bx0 = -(ymin * l[1] + l[2]) / sd(l[0], c), bx3 = -(ymax * l[1] + l[2]) / sd(l[0], c);
     double cx[4] = {bx0, xmin, xmax, bx3}, cy[4] = {ymin, by1, by2, ymax};
     int ok[4] = {bx0 >= xmin + EPS_ && bx0 < xmax - EPS_, by1 > ymin + EPS_ && by1 <= ymax - EPS_,
                  by2 >= ymin + EPS_ && by2 < ymax - EPS_, bx3 > xmin + EPS_ && bx3 <= xmax - EPS_};
@@ -61,10 +62,10 @@ static void clip_d(const double *l, double xmin, double xmax, double ymin, doubl
     if (ok[0] + ok[1] + ok[2] + ok[3] < 2) { S[0] = E[0] = xmin - FAR_; S[1] = E[1] = ymin - FAR_; }
     else { S[0] = px[0]; S[1] = py[0]; E[0] = px[1]; E[1] = py[1]; }
 }
-static void clip_f(const float *l, float xmin, float xmax, float ymin, float ymax, float *S, float *E) {
+static void clip_f(const float *l, float c, float xmin, float xmax, float ymin, float ymax, float *S, float *E) {
     const float e = (float)EPS_;
-    float by1 = -(xmin * l[0] + l[2]) / sdf(l[1]), by2 = -(xmax * l[0] + l[2]) / sdf(l[1]);
-    float bx0 = -(ymin * l[1] + l[2]) / sdf(l[0]), bx3 = -(ymax * l[1] + l[2]) / sdf(l[0]);
+    float by1 = -(xmin * l[0] + l[2]) / sdf(l[1], c), by2 = -(xmax * l[0] + l[2]) / sdf(l[1], c);
+    float bx0 = -(ymin * l[1] + l[2]) / sdf(l[0], c), bx3 = -(ymax * l[1] + l[2]) / sdf(l[0], c);
     float cx[4] = {bx0, xmin, xmax, bx3}, cy[4] = {ymin, by1, by2, ymax};
     int ok[4] = {bx0 >= xmin + e && bx0 < xmax - e, by1 > ymin + e && by1 <= ymax - e,
                  by2 >= ymin + e && by2 < ymax - e, bx3 > xmin + e && bx3 <= xmax - e};
@@ -72,6 +73,24 @@ static void clip_f(const float *l, float xmin, float xmax, float ymin, float yma
     for (int i = 0; i < 4 && n < 2; i++) if (ok[i]) { px[n] = cx[i]; py[n] = cy[i]; n++; }
     if (ok[0] + ok[1] + ok[2] + ok[3] < 2) { S[0] = E[0] = xmin - (float)FAR_; S[1] = E[1] = ymin - (float)FAR_; }
     else { S[0] = px[0]; S[1] = py[0]; E[0] = px[1]; E[1] = py[1]; }
+}
+
+/* l = e2 × x2 of the point x2 = M p (e2[2] == 1), returns the denominators' clamp: e2 × (x2 / x2[2]) with EPS_, or, where that
+   quotient is not finite (x2[2] == 0: the ray of p is parallel to the source image plane), e2 × x2 of the homogeneous point,
+   the zz -> 0 limit of the quotient form up to a factor 1/zz that grows without bound, so that the clamp never acts (0). */
+static double line_d(const double *e2, const double *x2, double *l) {
+    double x = x2[0] / x2[2], y = x2[1] / x2[2];
+    l[0] = e2[1] - y; l[1] = x - e2[0]; l[2] = e2[0] * y - e2[1] * x;
+    if (isfinite(l[0]) && isfinite(l[1]) && isfinite(l[2])) return EPS_;
+    l[0] = e2[1] * x2[2] - x2[1]; l[1] = x2[0] - e2[0] * x2[2]; l[2] = e2[0] * x2[1] - e2[1] * x2[0];
+    return 0.0;
+}
+static float line_f(const float *e2, const float *x2, float *l) {
+    float x = x2[0] / x2[2], y = x2[1] / x2[2];
+    l[0] = e2[1] - y; l[1] = x - e2[0]; l[2] = e2[0] * y - e2[1] * x;
+    if (isfinite(l[0]) && isfinite(l[1]) && isfinite(l[2])) return (float)EPS_;
+    l[0] = e2[1] * x2[2] - x2[1]; l[1] = x2[0] - e2[0] * x2[2]; l[2] = e2[0] * x2[1] - e2[1] * x2[0];
+    return 0.0f;
 }
 
 int epi_oracle_forward(const float *feat_ref, const float *feat_src, const double *P_ref, const double *P_src,
@@ -116,16 +135,14 @@ int epi_oracle_forward(const float *feat_ref, const float *feat_src, const doubl
                     if (geom_fp32) {
                         float x2[3], l[3], Sf[2], Ef[2];
                         for (int q = 0; q < 3; q++) x2[q] = Mf[q * 3] * pxf + Mf[q * 3 + 1] * pyf + Mf[q * 3 + 2];
-                        x2[0] /= x2[2]; x2[1] /= x2[2]; x2[2] = 1.0f;
-                        l[0] = e2f[1] * x2[2] - e2f[2] * x2[1]; l[1] = e2f[2] * x2[0] - e2f[0] * x2[2]; l[2] = e2f[0] * x2[1] - e2f[1] * x2[0];
-                        clip_f(l, xminf, xmaxf, yminf, ymaxf, Sf, Ef);
+                        float c = line_f(e2f, x2, l);
+                        clip_f(l, c, xminf, xmaxf, yminf, ymaxf, Sf, Ef);
                         S[0] = Sf[0]; S[1] = Sf[1]; E[0] = Ef[0]; E[1] = Ef[1];
                     } else {
                         double x2[3], l[3];
                         for (int q = 0; q < 3; q++) x2[q] = M[q * 3] * pxf + M[q * 3 + 1] * pyf + M[q * 3 + 2];
-                        x2[0] /= x2[2]; x2[1] /= x2[2]; x2[2] = 1.0;
-                        l[0] = e2[1] * x2[2] - e2[2] * x2[1]; l[1] = e2[2] * x2[0] - e2[0] * x2[2]; l[2] = e2[0] * x2[1] - e2[1] * x2[0];
-                        clip_d(l, xminf, xmaxf, yminf, ymaxf, S, E);
+                        double c = line_d(e2, x2, l);
+                        clip_d(l, c, xminf, xmaxf, yminf, ymaxf, S, E);
                     }
                     for (int k = 0; k < K; k++) {
                         double t = (double)k / (double)(K - 1);

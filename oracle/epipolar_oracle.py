@@ -53,7 +53,10 @@ def epipolar_lines(P_ref, P_src, xs, ys, geometry="reference"):
     geometry='reference': x2 = P2 (pinv(P1) p), e2 = P2 [-A1^-1 t1; 1], both divided by their
       third component (epipolar.py:336-350, vision/multiview.py:16-21).
     geometry='hinf': the better-conditioned point on the SAME line x2' = (A2 A1^-1) p and
-      e2 = A2 (-A1^-1 t1) + t2 (SURVEY.md appendix B) — what the CUDA kernel evaluates.
+      e2 = A2 (-A1^-1 t1) + t2 (SURVEY.md appendix B) — what the CUDA kernel evaluates.  Where x2' has no finite
+      quotient (a ray parallel to the source image plane: x2'[2] == 0), the line is e2 × x2' of the homogeneous point, the
+      limit of the quotient form up to a factor that grows without bound; it is scaled so that its smallest non-zero
+      direction component is 1, so the eps clamp of the clipping denominators does not act on it (as in that limit).
     """
     dt = P_ref.dtype
     N = P_ref.shape[0]
@@ -73,9 +76,16 @@ def epipolar_lines(P_ref, P_src, xs, ys, geometry="reference"):
             e2 = P2[:, :3] @ center + P2[:, 3]
         else:
             raise ValueError(geometry)
-        x2 = x2 / x2[2:3]
         e2 = e2 / e2[2]
-        lines[n] = np.cross(np.broadcast_to(e2[:, None], x2.shape), x2, axis=0).T
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+            l = np.cross(np.broadcast_to(e2[:, None], x2.shape), x2 / x2[2:3], axis=0).T
+        if geometry == "hinf":
+            par = ~np.isfinite(l).all(-1)
+            if par.any():
+                lh = np.cross(np.broadcast_to(e2[:, None], (3, int(par.sum()))), x2[:, par], axis=0).T
+                a = np.abs(lh[:, :2])
+                l[par] = lh / np.where(a > 0, a, np.inf).min(-1, keepdims=True)
+        lines[n] = l
     return lines
 
 

@@ -185,6 +185,107 @@ def stereo_rig(N, img_size, yaw=0.0):
     return np.stack(P1).astype(np.float32), np.stack(P2).astype(np.float32)
 
 
+# ---- camera rigs whose epipoles lie inside the maps ----------------------------------------------------------------------
+# 64x64 maps of 256-pixel images (downsample 4, img_scale 1): pixel centres at 4i + 1.5, i < 64.  Cameras are built in float64
+# as KRT = K [R | -R C] and cast to float32 as the dataset code does; centres and intrinsics are dyadic where a case needs exact
+# arithmetic.
+RIG_HW = 64
+
+
+def _cam(pp, R, C, f=256.0):
+    px, py = (pp, pp) if np.isscalar(pp) else pp
+    A = np.array([[f, 0, px], [0, f, py], [0, 0, 1.0]])
+    R = np.asarray(R, np.float64)
+    return A @ np.hstack([R, (-R @ np.asarray(C, np.float64))[:, None]])
+
+
+def _rot_y(a):
+    return np.array([[np.cos(a), 0, np.sin(a)], [0, 1, 0], [-np.sin(a), 0, np.cos(a)]])
+
+
+_FLIP = np.diag([-1.0, 1.0, -1.0])                 # looking down −z: a turn by π about y, exact
+_R90 = np.array([[0, 0, 1.0], [0, 1, 0], [-1, 0, 0]])   # looking down −x: a turn by −π/2 about y, exact
+
+
+def ring_opposite(N=2, img=256, seed=0):
+    """[V=4,N,3,4] float32: a jittered ring of 4·N cameras, view v of item n is camera v·N + n (as the views tests build it),
+    so views v and v + 2 of an item are opposite cameras, both of whose epipoles lie inside the map."""
+    from epipolar_transformers_b200 import synthetic as syn
+    return syn.ring_cameras(4 * N, img, seed=seed, jitter=20.0).reshape(4, N, 3, 4).astype(np.float32)
+
+
+def _pair_rigs():
+    """name -> (P_ref [3,4], P_src [3,4]) float64 before the cast.  The reference camera's principal point is a pixel centre
+    (129.5) or the centre of the map (127.5); the source camera's, (131.25, 126.125), is no pixel centre, so that no epipolar line
+    through e2 meets a corner of the pixel-centre rectangle (a line through a corner is clipped on the thresholds themselves)."""
+    I, pp2 = np.eye(3), (131.25, 126.125)
+    return {
+        # two cameras on the z axis looking at each other, the reference principal point on the centre of pixel (32, 32):
+        # e1 is that pixel
+        "facing": (_cam(129.5, I, (0, 0, -1024)), _cam(pp2, _FLIP, (0, 0, 1024))),
+        # the same with the source centre off the axis: e1 lies between pixel centres
+        "facing_off": (_cam(129.5, I, (0, 0, -1024)), _cam(pp2, _FLIP, (7, -5, 1024))),
+        # the source camera behind the reference camera, looking the same way: e1's third coordinate is negative
+        "behind": (_cam(129.5, I, (0, 0, -1024)), _cam(pp2, I, (0, 0, -2048))),
+        "behind_off": (_cam(129.5, I, (0, 0, -1024)), _cam(pp2, _rot_y(0.02), (37, 21, -2048))),
+        # facing cameras whose e1 is the centre of the pixel-centre rectangle, (127.5, 127.5), between four pixels: the
+        # point the staging kernel's order key measures from
+        "centre": (_cam(127.5, I, (0, 0, -1024)), _cam(pp2, _FLIP, (0, 0, 1024))),
+        # the source camera turned by exactly 90°: M's third row, (−1/256, 0, 129.5/256) in fp32, depends on the reference
+        # intrinsics only, so zz == 0 on all of column 32 (x = 129.5), whose rays are parallel to the source image plane
+        "rig90": (_cam(129.5, I, (0, 0, -2000)), _cam(pp2, _R90, (1000, 0, 1000))),
+        # its near-degenerate twin: turned by a further 1e-6 rad, zz is tiny but not zero
+        "rig90_twin": (_cam(129.5, I, (0, 0, -2000)), _cam(pp2, _R90 @ _rot_y(1e-6), (1000, 0, 1000))),
+    }
+
+
+PAIR_RIGS = list(_pair_rigs())
+
+
+def pair_rig(name):
+    """-> (P_ref, P_src) float32 [N,3,4].  'ring_opposite': the 4·N opposite pairs (v, v + 2) of ring_opposite(N=2), pair
+    v·N + n; otherwise one of PAIR_RIGS (N = 1)."""
+    if name == "ring_opposite":
+        P = ring_opposite()
+        return P.reshape(-1, 3, 4), P[[2, 3, 0, 1]].reshape(-1, 3, 4)
+    P1, P2 = _pair_rigs()[name]
+    return P1[None].astype(np.float32), P2[None].astype(np.float32)
+
+
+def epipoles(P1, P2):
+    """fp64 homogeneous epipoles of one pair: e1 = P1·[C2; 1] (in the reference view), e2 = P2·[C1; 1] (in the source view)."""
+    P1, P2 = np.asarray(P1, np.float64), np.asarray(P2, np.float64)
+    c1 = -np.linalg.solve(P1[:, :3], P1[:, 3]); c2 = -np.linalg.solve(P2[:, :3], P2[:, 3])
+    return P1 @ np.r_[c2, 1.0], P2 @ np.r_[c1, 1.0]
+
+
+def img2feat(v, downsample=4.0):
+    """image coordinate -> feature-pixel coordinate (img_scale 1)"""
+    return (np.asarray(v, np.float64) + 0.5 - downsample / 2) / downsample
+
+
+def e1_distance(P1, P2, H, W, downsample=4.0):
+    """[N,H,W] distance in feature px of every reference pixel centre from e1 (inf where e1 is at infinity)."""
+    d = np.empty((len(P1), H, W))
+    for n in range(len(P1)):
+        e1, _ = epipoles(P1[n], P2[n])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            ex, ey = img2feat(e1[:2] / e1[2], downsample)
+        d[n] = np.hypot(np.arange(W)[None, :] - ex, np.arange(H)[:, None] - ey)
+    return np.nan_to_num(d, nan=np.inf)
+
+
+def rig_cfg(K, C=8, H=RIG_HW, W=RIG_HW):
+    from epipolar_transformers_b200.config import make_cfg
+    return make_cfg(KEYPOINT=dict(HEATMAP_SIZE=(H, W), NFEATS=C), EPIPOLAR=dict(SAMPLESIZE=K, USE_CORRECT_NORMALIZE=True))
+
+
+def loc2feat(locs, H, W):
+    """normalised (USE_CORRECT_NORMALIZE) locations [..., 2] -> feature px"""
+    g = np.asarray(locs, np.float64)
+    return np.stack([(g[..., 0] + 1) * (W - 1) / 2, (g[..., 1] + 1) * (H - 1) / 2], -1)
+
+
 # ---- float64 reference on given locations ------------------------------------------------------------------------------
 FAR_LOC = -312.5          # stands in for a non-finite location in the reference's sampling (it samples nothing either way)
 
