@@ -31,13 +31,19 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_kernel_timing_enable", "epi_kernel_timing_last_ms", "epi_kernel_timing_last3",
            "epi_fusion_backward_deterministic", "epi_fusion_views", "epi_fusion_view_sources_forward_f32",
            "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources",
-           "epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward")
+           "epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward",
+           "epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_heatmaps_workspace_bytes", "epi_fusion_heatmaps_cache_bytes",
+           "epi_fusion_heatmaps")
 # The source-table entry points are new symbols, not a reinterpreted field, so a library without them still runs every other
 # form correctly: load() accepts it, and only a call with a source table needs them (`require_view_sources`).
 VIEW_SOURCES_EXPORTS = ("epi_fusion_view_sources_forward_f32", "epi_fusion_view_sources_workspace_bytes",
                         "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources")
 # The backward of the views form is optional in the same way: only a views-backward call needs it (`require_views_backward`).
 VIEWS_BACKWARD_EXPORTS = ("epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward")
+# So are the heat-map forward and its fold: only a call with a head needs them (`require_heatmaps`).
+HEATMAPS_EXPORTS = ("epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_heatmaps_workspace_bytes",
+                    "epi_fusion_heatmaps_cache_bytes", "epi_fusion_heatmaps")
+HEAD_MAX_JOINTS = 64                # EpiHeadParams.J (include/epipolar_b200.h)
 
 _fp = ctypes.POINTER(ctypes.c_float)
 
@@ -68,6 +74,15 @@ class EpiFusionParams(ctypes.Structure):
     @n_views.setter
     def n_views(self, v):
         self.reserved[0] = v
+
+
+class EpiHeadParams(ctypes.Structure):
+    """Field-for-field mirror of `struct EpiHeadParams` (include/epipolar_b200.h)."""
+    _fields_ = [
+        ("A", ctypes.c_void_p), ("B", ctypes.c_void_p), ("b", ctypes.c_void_p),
+        ("heat", ctypes.c_void_p), ("heat_stride", ctypes.c_int64 * 4),
+        ("J", ctypes.c_int32), ("reserved", ctypes.c_int32 * 3),
+    ]
 
 
 class EpiFusionBwdParams(ctypes.Structure):
@@ -103,7 +118,7 @@ def load():
             "epipolar_transformers_b200: CUDA library %s is missing. Build it with "
             "`python -m epipolar_transformers_b200.build` (needs nvcc). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS and not hasattr(lib, s)]
+    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS + HEATMAPS_EXPORTS and not hasattr(lib, s)]
     if missing:
         # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
         # (a views call would silently run as a one-source call)
@@ -161,6 +176,17 @@ def load():
         lib.epi_fusion_views_backward_workspace_bytes.restype = ctypes.c_size_t
         lib.epi_fusion_views_backward_workspace_bytes.argtypes = views
         lib.epi_fusion_views_backward.restype = ctypes.c_int
+    if all(hasattr(lib, s) for s in HEATMAPS_EXPORTS):
+        heat = [ctypes.POINTER(EpiFusionParams), ctypes.POINTER(EpiHeadParams), ctypes.POINTER(ctypes.c_int32), ctypes.c_int32]
+        lib.epi_fusion_heatmaps_f32.restype = ctypes.c_int
+        lib.epi_fusion_heatmaps_f32.argtypes = heat + [ctypes.c_void_p]
+        lib.epi_fusion_heatmaps_workspace_bytes.restype = ctypes.c_size_t
+        lib.epi_fusion_heatmaps_workspace_bytes.argtypes = heat
+        lib.epi_fusion_heatmaps_cache_bytes.restype = ctypes.c_size_t
+        lib.epi_fusion_heatmaps_cache_bytes.argtypes = heat
+        lib.epi_fusion_heatmaps.restype = ctypes.c_int
+        lib.epi_fold_head_f32.restype = ctypes.c_int
+        lib.epi_fold_head_f32.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 3
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))
@@ -182,6 +208,14 @@ def require_views_backward(lib):
     if missing or lib.epi_fusion_views_backward() != 1:
         raise RuntimeError("libepipolar_b200.so does not export %s, so it has no backward for the views form; rebuild it with "
                            "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_views_backward"]))
+
+
+def require_heatmaps(lib):
+    """Raise unless `lib` has the heat-map forward (epi_fusion_heatmaps())."""
+    missing = [s for s in HEATMAPS_EXPORTS if not hasattr(lib, s)]
+    if missing or lib.epi_fusion_heatmaps() != 1:
+        raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot run the pose head as the forward's epilogue; "
+                           "rebuild it with `python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_heatmaps"]))
 
 
 def check(rc: int, what: str):

@@ -79,7 +79,9 @@ bool src_is_channels_last(const EpiFusionParams *p) {
 enum class Kernel { Pipe, Sector, Tile, Warp };          // fused attention kernel (sector and 4x8 block tiles: epi_fusion_tile_kernel)
 enum class Staging { Pipe, Planes, Nhwc, InPlace };      // feat_src: the pipe's staging launch, bf16 (hi, lo) planes, fp32 channels-last, as is
 enum class RefCopy { None, Before, After };              // fp32 channels-last copy of a low-precision feat_ref, before / after the fused kernel
-enum class Epilogue { Direct, Unstage, ZGemm, ZFp32 };   // who writes `out`: the fused kernel, a transposition pass, the z GEMM / z epilogue
+// who writes `out`: the fused kernel, a transposition pass, the z GEMM / z epilogue; Head: the head kernel writes the heat-maps
+// (epi_fusion_heatmaps_f32 only) from the fused kernel's pixel-major plane
+enum class Epilogue { Direct, Unstage, ZGemm, ZFp32, Head };
 
 // Everything the forward decides, made from the params alone.  Offsets are NONE for the regions the plan does not use.
 struct Plan {
@@ -118,7 +120,7 @@ bool want_tile(const EpiFusionParams *p) {
 // The reference planes are staged once however many sources they are fused with.  One bf16 plane of a map is half its fp32 bytes.
 // The views form stages its V·N items once (`ref_map`): they are both the query and the source planes, and `map` covers the
 // V·S·N pairs' fused features only.
-Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
+Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs, bool head = false) {
     Plan pl;
     const bool views = p->n_views != 0;
     const size_t NP = (size_t)n_pairs(p, vs), px = (size_t)p->H * p->W;
@@ -144,7 +146,8 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         const bool out_direct = p->out_stride[1] == 1 && p->out_stride[3] % 4 == 0 && p->out_stride[2] % 4 == 0 && p->out_stride[0] % 4 == 0 &&
                                 reinterpret_cast<uintptr_t>(p->out) % 16 == 0;
         pl.staging = Staging::Pipe;
-        pl.epilogue = has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32)
+        pl.epilogue = head ? Epilogue::Head
+                    : has_z ? (epi::zgemm_supported(p->C) ? Epilogue::ZGemm : Epilogue::ZFp32)
                             : (out_direct && !out16 ? Epilogue::Direct : Epilogue::Unstage);
         if (lowp && pl.epilogue == Epilogue::ZFp32 && p->add_ref_residual) pl.ref_copy = RefCopy::After;   // the fp32 z epilogue's residual
         pl.cached = p->cache != nullptr;
@@ -158,7 +161,8 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
             if (lo) pl.src_lo = ws.part(map / 2);
         }
         ws.close();
-        // fused feature: bf16 (hi, lo) planes for the z GEMM; fp32, contiguous NCHW for the z epilogue, pixel-major for the transposition
+        // fused feature: bf16 (hi, lo) planes for the z GEMM; fp32, contiguous NCHW for the z epilogue, pixel-major for the
+        // transposition and the head
         if (pl.epilogue == Epilogue::ZGemm) { pl.fused = ws.part(map / 2); pl.fused_lo = ws.take(map / 2); }
         else if (pl.epilogue != Epilogue::Direct) pl.fused = ws.take(map);
         pl.counter = ws.take(256);
@@ -177,7 +181,7 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         // the tile kernel reads bf16 (hi, lo) planes; the warp kernel reads a channels-last fp32 source in place
         const bool tiles = pl.kernel != Kernel::Warp;
         pl.staging = tiles ? Staging::Planes : (!src_is_channels_last(p) || lowp ? Staging::Nhwc : Staging::InPlace);
-        pl.epilogue = has_z ? Epilogue::ZFp32 : out16 ? Epilogue::Unstage : Epilogue::Direct;
+        pl.epilogue = head ? Epilogue::Head : has_z ? Epilogue::ZFp32 : out16 ? Epilogue::Unstage : Epilogue::Direct;
         pl.ref_copy = lowp ? RefCopy::Before : RefCopy::None;        // these kernels read the query (and the residual) as fp32
         // views form: a low-precision map's fp32 copy is the warp kernel's source as it stands, and the sector tiles query the
         // source planes
@@ -185,7 +189,7 @@ Plan make_plan(const EpiFusionParams *p, const epi::ViewSources &vs) {
         if (lowp) pl.ref32 = ws.take(ref_map);
         if (tiles) { pl.src_hi = ws.part(src_map_bytes / 2); pl.src_lo = ws.take(src_map_bytes / 2); }
         else if (pl.staging == Staging::Nhwc) pl.src_nhwc = ws.take(src_map_bytes);
-        if (pl.epilogue != Epilogue::Direct) pl.fused = ws.take(map);      // NCHW for the z epilogue, pixel-major for the transposition
+        if (pl.epilogue != Epilogue::Direct) pl.fused = ws.take(map);      // NCHW for the z epilogue, pixel-major for the transposition / head
         if (tiles) pl.counter = ws.take(256);
         if (pl.kernel == Kernel::Sector) {
             if (!views) { pl.ref_hi = ws.part(ref_map / 2); pl.ref_lo = ws.take(ref_map / 2); }
@@ -227,16 +231,17 @@ const char *read_view_table(const EpiFusionParams *p, const int32_t *sources, in
     return p ? read_table(p->n_views, sources, S, vs, msg, len) : "params is null";
 }
 
-int validate(const EpiFusionParams *p, const epi::ViewSources &vs) {
+// head: a heat-map call, which has no `out` (epi_fusion_heatmaps_f32 checks that it is null)
+int validate(const EpiFusionParams *p, const epi::ViewSources &vs, bool head = false) {
     if (!p) return fail(EPI_EINVAL, "params is null");
     if (p->n_views < 0 || p->n_views == 1) return fail(EPI_EINVAL, "n_views must be 0 or >= 2 (every view against every other)");
     if (p->n_views) {
         if (p->feat_src || p->P_src) return fail(EPI_EINVAL, "n_views >= 2: feat_src and P_src must be null (feat_ref / P_ref hold the views)");
         if (p->n_src > 1) return fail(EPI_EINVAL, "n_views >= 2 needs n_src 0 or 1");
-        if (!p->feat_ref || !p->out) return fail(EPI_EINVAL, "feat_ref/out must be non-null");
+        if (!p->feat_ref || (!p->out && !head)) return fail(EPI_EINVAL, "feat_ref/out must be non-null");
         if (!p->sample_locs_in && !p->P_ref) return fail(EPI_EINVAL, "P_ref required without sample_locs_in");
     } else {
-        if (!p->feat_ref || !p->feat_src || !p->out) return fail(EPI_EINVAL, "feat_ref/feat_src/out must be non-null");
+        if (!p->feat_ref || !p->feat_src || (!p->out && !head)) return fail(EPI_EINVAL, "feat_ref/feat_src/out must be non-null");
         if (!p->sample_locs_in && (!p->P_ref || !p->P_src)) return fail(EPI_EINVAL, "P_ref/P_src required without sample_locs_in");
     }
     if (p->N <= 0 || p->C <= 0 || p->H < 2 || p->W < 2) return fail(EPI_EINVAL, "need N,C >= 1 and H,W >= 2");
@@ -405,11 +410,12 @@ size_t epi_fusion_workspace_bytes(const EpiFusionParams *p) {
 
 namespace {
 
-int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) {
-    int rc = validate(p, vs);
+// h: the head of a heat-map call (epi_fusion_heatmaps_f32, checked there), else null
+int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream, const EpiHeadParams *h = nullptr) {
+    int rc = validate(p, vs, h != nullptr);
     if (rc != EPI_OK) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const Plan pl = make_plan(p, vs);
+    const Plan pl = make_plan(p, vs, h != nullptr);
     void *ws = p->workspace;
     if (pl.workspace_bytes > 0 && (!ws || p->workspace_bytes < pl.workspace_bytes)) return fail(EPI_EWORKSPACE, "workspace too small");
     if (pl.workspace_bytes > 0 && reinterpret_cast<uintptr_t>(ws) % 256 != 0) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
@@ -493,10 +499,11 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
     // where the fused kernel writes
     if (pl.epilogue == Epilogue::ZGemm) {
         a.out_hi = at<__nv_bfloat16>(ws, pl.fused); a.out_lo = at<__nv_bfloat16>(ws, pl.fused_lo);
-    } else if (pl.epilogue != Epilogue::Direct) {    // pixel-major (full 128-byte lines) for the transposition pass, NCHW for the z epilogue
+    } else if (pl.epilogue != Epilogue::Direct) {    // pixel-major (full 128-byte lines) for the transposition pass and the head, NCHW for the z epilogue
         const int64_t nchw_stride[4] = {(int64_t)p->C * p->H * p->W, (int64_t)p->H * p->W, p->W, 1};
         a.out = at<float>(ws, pl.fused);
-        for (int i = 0; i < 4; i++) a.out_stride[i] = pl.epilogue == Epilogue::Unstage ? cl_stride[i] : nchw_stride[i];
+        const bool pm = pl.epilogue == Epilogue::Unstage || pl.epilogue == Epilogue::Head;
+        for (int i = 0; i < 4; i++) a.out_stride[i] = pm ? cl_stride[i] : nchw_stride[i];
     } else {
         a.out = p->out;
         for (int i = 0; i < 4; i++) a.out_stride[i] = p->out_stride[i];
@@ -534,6 +541,14 @@ int forward(const EpiFusionParams *p, const epi::ViewSources &vs, void *stream) 
         z.N = NP; z.n_ref = p->N; z.n_views = V; z.vsrc = vs; z.C = p->C; z.HW = p->H * p->W; z.W = p->W;
         z.z_residual = p->z_residual; z.add_ref = p->add_ref_residual;
         if ((rc = run("z epilogue", epi::launch_z_epilogue(z, od, st)))) return rc;
+    } else if (pl.epilogue == Epilogue::Head) {
+        epi::HeadArgs hd;
+        memset(&hd, 0, sizeof(hd));
+        hd.x = a.out; hd.A = h->A; hd.B = h->B; hd.b = h->b;
+        hd.ref = h->B ? p->feat_ref : nullptr; hd.ref_dtype = dt; hd.heat = h->heat;
+        for (int i = 0; i < 4; i++) { hd.ref_stride[i] = p->ref_stride[i]; hd.heat_stride[i] = h->heat_stride[i]; }
+        hd.N = NP; hd.C = p->C; hd.HW = p->H * p->W; hd.W = p->W; hd.J = h->J; hd.n_ref = p->N; hd.n_views = V;
+        if ((rc = run("head", epi::launch_head(hd, vs, od, st)))) return rc;
     }
     if (g_timing) { cudaEventRecord(g_evB, st); g_timing_valid = 1; }
     g_launches = run.n;
@@ -563,6 +578,72 @@ int epi_fusion_view_sources_forward_f32(const EpiFusionParams *p, const int32_t 
     char msg[128];
     if (const char *why = read_view_table(p, sources_host, S, vs, msg, sizeof(msg))) return fail(EPI_EINVAL, "%s", why);
     return forward(p, vs, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// The head of a heat-map call and the fields of p it replaces.  Returns null, or why they are refused.
+const char *check_head(const EpiFusionParams *p, const EpiHeadParams *h) {
+    if (!p) return "params is null";
+    if (!h) return "head params are null";
+    if (p->out) return "heat-map call: out must be null (heat receives the result; the fused feature is not stored)";
+    if (p->z_weight_folded) return "heat-map call: z_weight_folded must be null (fold z / BN into A and b with epi_fold_head_f32)";
+    if (p->add_ref_residual) return "heat-map call: add_ref_residual must be 0 (B = the head weight adds the caller's residual)";
+    if (!h->A || !h->b || !h->heat) return "heat-map call: A, b and heat must be non-null";
+    if (h->J < 1 || h->J > 64) return "heat-map call: J must be in [1, 64]";
+    if (h->reserved[0] || h->reserved[1] || h->reserved[2]) return "heat-map call: reserved words must be zero";
+    const uintptr_t es = out_dtype(p) == EPI_DTYPE_F32 ? 4 : 2;
+    if (reinterpret_cast<uintptr_t>(h->A) % 4 || reinterpret_cast<uintptr_t>(h->B) % 4 || reinterpret_cast<uintptr_t>(h->b) % 4 ||
+        reinterpret_cast<uintptr_t>(h->heat) % es)
+        return "heat-map call: A, B and b must be 4-byte aligned and heat aligned to its element size";
+    return nullptr;
+}
+
+// The table of a heat-map call: the caller's [V][S] table, or none (NULL with S = 0: the pair, n_src and all-others views forms).
+const char *read_heat_table(const EpiFusionParams *p, const int32_t *sources, int32_t S, epi::ViewSources &vs, char *msg, size_t len) {
+    if (!sources && S == 0) return nullptr;
+    return read_view_table(p, sources, S, vs, msg, len);
+}
+
+// the size queries plan a heat-map call from the shapes alone: J, not the head's pointers
+bool heat_plannable(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources, int32_t S, epi::ViewSources &vs) {
+    char msg[128];
+    return h && h->J >= 1 && h->J <= 64 && !read_heat_table(p, sources, S, vs, msg, sizeof(msg)) && plannable(p, vs);
+}
+
+}  // namespace
+
+extern "C" {
+
+int epi_fusion_heatmaps(void) { return 1; }
+
+size_t epi_fusion_heatmaps_workspace_bytes(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S) {
+    epi::ViewSources vs{};
+    return heat_plannable(p, h, sources_host, S, vs) ? make_plan(p, vs, true).workspace_bytes : 0;
+}
+
+size_t epi_fusion_heatmaps_cache_bytes(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S) {
+    epi::ViewSources vs{};
+    return heat_plannable(p, h, sources_host, S, vs) ? make_plan(p, vs, true).cache_bytes : 0;
+}
+
+int epi_fusion_heatmaps_f32(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S, void *stream) {
+    epi::ViewSources vs{};
+    char msg[128];
+    if (const char *why = check_head(p, h)) return fail(EPI_EINVAL, "%s", why);
+    if (const char *why = read_heat_table(p, sources_host, S, vs, msg, sizeof(msg))) return fail(EPI_EINVAL, "%s", why);
+    return forward(p, vs, stream, h);
+}
+
+int epi_fold_head_f32(const float *Wh, const float *bh, const float *Wf, const float *bf, int32_t z_residual, int32_t J, int32_t C,
+                      float *A_out, float *b_out, void *stream) {
+    if (!Wh || !A_out || !b_out) return fail(EPI_EINVAL, "Wh, A_out and b_out must be non-null");
+    if (J < 1 || C < 1) return fail(EPI_EINVAL, "need J >= 1 and C >= 1");
+    cudaError_t e = epi::launch_fold_head(Wh, bh, Wf, bf, z_residual ? 1 : 0, J, C, A_out, b_out, reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(EPI_ECUDA, "head fold launch failed: %s", cudaGetErrorString(e));
+    return EPI_OK;
 }
 
 size_t epi_fusion_backward_workspace_bytes(const EpiFusionBwdParams *p) {

@@ -161,6 +161,22 @@ cudaError_t launch_z_epilogue(const ZArgs &z, int y_dtype, cudaStream_t st);
 cudaError_t launch_unstage(const float *pm, const void *ref, int ref_dtype, const int64_t ref_stride[4], void *out, int out_dtype,
                            const int64_t out_stride[4], int N, int n_ref, int n_views, const ViewSources &vs, int C, int H, int W,
                            cudaStream_t st);
+// Heat-map epilogue (epi_head.cu): heat[n,j,p] = b[j] + Σ_c (A[j,c]·x[n,p,c] + B[j,c]·ref[q,c,p]), q = pair_items(n, n_ref,
+// n_views, vs).q; x is the fused kernel's pixel-major fp32 plane [N,HW,C]; ref (element type ref_dtype, any strides) and B are
+// null without the caller's residual.  1 <= J <= 64.
+struct HeadArgs {
+    const float *x;
+    const void *ref;        int64_t ref_stride[4];
+    int ref_dtype;
+    const float *A, *B, *b;
+    void *heat;             int64_t heat_stride[4];   // element type: launch_head's heat_dtype
+    int N, C, HW, W, J, n_ref, n_views;
+};
+// heat_dtype (kF32 / kBF16 / kF16): element type of heat, the fp32 sum rounded once
+cudaError_t launch_head(const HeadArgs &h, const ViewSources &vs, int heat_dtype, cudaStream_t st);
+// A = Wh·(Wf + z_res·I) (Wh when Wf is null), b = Wh·bf + bh (null bh / bf: zero), fp64 sums rounded once; Wh [J,C], Wf [C,C]
+cudaError_t launch_fold_head(const float *Wh, const float *bh, const float *Wf, const float *bf, int z_res, int J, int C, float *A,
+                             float *b, cudaStream_t st);
 cudaError_t launch_fold_z_bn(const float *zw, const float *zb, const float *g, const float *b, const float *mean,
                              const float *var, float eps, int C, float *wf, float *bf, cudaStream_t st);
 cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, int J, int H, int W, float radius, float downsample,

@@ -93,7 +93,7 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
                     softmax_scale=0.125, correct_normalize=False, align_corners=False,
                     z_folded=None, z_residual=False, add_ref_residual=False,
                     sample_locs_in=None, want_attn=True, want_corr=True, want_locs=False,
-                    variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32):
+                    variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32, head=None):
     """Functional form of the fused forward.  Returns (out, corr_pos|None, attn|None, sample_locs|None).
 
     feat_ref/feat_src: CUDA [N,C,H,W] (NCHW or channels_last strides), both float32, both bfloat16 or both float16 (what a
@@ -104,23 +104,32 @@ def epipolar_fusion(feat_ref, feat_src, P_ref, P_src, *, K, downsample=4.0, img_
     z_folded: optional (Wf [C,C], bf [C]) from `fold_z_bn` (eval-mode epilogue, epipolar.py:249-253).
     sample_locs_in: optional [K,N,H,W,2] normalised locations replacing the fused geometry.
     state: optional FusionState (persistent workspace + camera-keyed cache); without it scratch is allocated per call.
+    head: optional (weight [J,C] or [J,C,1,1], bias [J] | None), the pose head's 1x1 conv (`final_layer`), or that conv itself,
+      1 <= J <= 64: the call returns (heat [N,J,H,W], corr_pos, attn, sample_locs) with heat = head(z/BN epilogue(fused) +
+      feat_ref if add_ref_residual), of dtype out_dtype, and the fused feature is never stored (`out` must be None).  corr_pos,
+      attn and sample_locs are bit for bit those of the call without a head.  Inference only (`fold_head`, DESIGN.md §3.7).
     """
     lib = _lib.load()
+    if head is not None:
+        _lib.require_heatmaps(lib)
     dcode = _check_feat_pair(feat_ref, feat_src, out, out_dtype)
     if feat_ref.shape != feat_src.shape or feat_ref.device != feat_src.device:
         raise ValueError("feat_ref and feat_src must have the same shape and device")
+    hp = None if head is None else _head_operands(lib, head, feat_ref, feat_src, out, z_folded, z_residual, add_ref_residual)
     return _fusion(lib, dcode, 1, feat_ref, feat_src, P_ref, P_src, K=K, downsample=downsample, img_scale=img_scale,
                    softmax_scale=softmax_scale, correct_normalize=correct_normalize, align_corners=align_corners,
-                   z_folded=z_folded, z_residual=z_residual, add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in,
+                   z_folded=None if hp else z_folded, z_residual=z_residual and not hp,
+                   add_ref_residual=add_ref_residual and not hp, sample_locs_in=sample_locs_in,
                    want_attn=want_attn, want_corr=want_corr, want_locs=want_locs, variant=variant, out=out, state=state,
-                   out_dtype=out_dtype)
+                   out_dtype=out_dtype, head=hp)
 
 
 def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4.0, img_scale=1.0,
                           softmax_scale=0.125, correct_normalize=False, align_corners=False,
                           z_folded=None, z_residual=False, add_ref_residual=False,
                           sample_locs_in=None, want_attn=True, want_corr=True, want_locs=False,
-                          variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32):
+                          variant="auto", out=None, state: Optional[FusionState] = None, out_dtype=torch.float32,
+                          head=None):
     """Fuses every reference item with S source views in one call: the multi-view test path of the reference
     (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239), where each reference batch is fused against every other view.
     Source s of item n gives exactly what `epipolar_fusion(feat_ref, feat_srcs[s], P_ref, P_srcs[s])` gives, but the
@@ -130,9 +139,12 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
     P_ref: [N,3,4]; P_srcs: [S,N,3,4]; sample_locs_in: optional [K,S,N,H,W,2]; out: optional [S,N,C,H,W] of dtype out_dtype
     (float32, or bfloat16 / float16 as in `epipolar_fusion`).
     Every residual (add_ref_residual, also under z) adds feat_ref[n].  Returns
-    (out [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attn [S,N,K,H,W] | None, sample_locs [K,S,N,H,W,2] | None).
+    (out [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attn [S,N,K,H,W] | None, sample_locs [K,S,N,H,W,2] | None); with a `head`
+    (as in `epipolar_fusion`) heat [S,N,J,H,W] in place of out.
     Inference only (no backward for several sources): inputs that require grad under grad mode raise RuntimeError."""
     lib = _lib.load()
+    if head is not None:
+        _lib.require_heatmaps(lib)
     if isinstance(feat_srcs, (list, tuple)):
         if not feat_srcs or not all(isinstance(t, torch.Tensor) for t in feat_srcs):
             raise ValueError("feat_srcs must be a [S,N,C,H,W] tensor or a non-empty sequence of [N,C,H,W] tensors")
@@ -168,12 +180,13 @@ def epipolar_fusion_multi(feat_ref, feat_srcs, P_ref, P_srcs, *, K, downsample=4
     if torch.is_grad_enabled() and (feat_ref.requires_grad or feat_src.requires_grad):
         raise RuntimeError("epipolar_fusion_multi is inference only (several sources have no backward); run it under "
                            "torch.no_grad(), or use epipolar_fusion (one source per call) for gradients")
+    hp = None if head is None else _head_operands(lib, head, feat_ref, feat_src, out4, z_folded, z_residual, add_ref_residual)
     o, corr, attn, locs = _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_srcs, K=K, downsample=downsample,
                                   img_scale=img_scale, softmax_scale=softmax_scale, correct_normalize=correct_normalize,
-                                  align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
-                                  add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
+                                  align_corners=align_corners, z_folded=None if hp else z_folded, z_residual=z_residual and not hp,
+                                  add_ref_residual=add_ref_residual and not hp, sample_locs_in=sample_locs_in, want_attn=want_attn,
                                   want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state,
-                                  out_dtype=out_dtype)
+                                  out_dtype=out_dtype, head=hp)
     return (out if out is not None else o.unflatten(0, (S, N)), None if corr is None else corr.unflatten(0, (S, N)),
             None if attn is None else attn.unflatten(0, (S, N)), None if locs is None else locs.unflatten(1, (S, N)))
 
@@ -207,7 +220,7 @@ def view_source_table(sources, V):
 def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax_scale=0.125, correct_normalize=False,
                           align_corners=False, z_folded=None, z_residual=False, add_ref_residual=False, sample_locs_in=None,
                           want_attn=True, want_corr=True, want_locs=False, variant="auto", out=None,
-                          state: Optional[FusionState] = None, sources=None, out_dtype=torch.float32):
+                          state: Optional[FusionState] = None, sources=None, out_dtype=torch.float32, head=None):
     """Fuses each view of a frame with several other views in one call, staging each view's map once.
 
     sources=None: every view with every other view, the whole multi-view test of the reference (cfg.EPIPOLAR.MULTITEST,
@@ -220,10 +233,13 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
     feats: [V,N,C,H,W], or a sequence of V [N,C,H,W] maps (stacked), V >= 2; P: [V,N,3,4]; sample_locs_in: optional
     [K,V,S,N,H,W,2]; out: optional [V,S,N,C,H,W] of dtype out_dtype (float32, or bfloat16 / float16 as in `epipolar_fusion`).  Reference view v with its j-th source u gives, bit for bit, what
     `epipolar_fusion(feats[v], feats[u], P[v], P[u])` gives; every residual (add_ref_residual, also under z) adds feats[v][n].
-    Returns (out [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attn [V,S,N,K,H,W] | None, sample_locs [K,V,S,N,H,W,2] | None).
+    Returns (out [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attn [V,S,N,K,H,W] | None, sample_locs [K,V,S,N,H,W,2] | None);
+    with a `head` (as in `epipolar_fusion`; its residual adds feats[v][n]) heat [V,S,N,J,H,W] in place of out.
     Inference only: inputs that require grad under grad mode raise RuntimeError.  `epipolar_fusion_views_backward` is its
     backward, and `Epipolar.forward_views_train` the differentiable form."""
     lib = _lib.load()
+    if head is not None:
+        _lib.require_heatmaps(lib)
     if isinstance(feats, (list, tuple)):
         if not all(isinstance(t, torch.Tensor) for t in feats):
             raise ValueError("feats must be a [V,N,C,H,W] tensor or a sequence of V [N,C,H,W] tensors")
@@ -264,12 +280,13 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
     if torch.is_grad_enabled() and feat.requires_grad:
         raise RuntimeError("epipolar_fusion_views is inference only; run it under torch.no_grad(), or use "
                            "Epipolar.forward_views_train (backward: epipolar_fusion_views_backward) for gradients")
+    hp = None if head is None else _head_operands(lib, head, feat, feat, out4, z_folded, z_residual, add_ref_residual)
     o, corr, attn, locs = _fusion(lib, dcode, 1, feat, None, P, None, K=K, downsample=downsample, img_scale=img_scale,
                                   softmax_scale=softmax_scale, correct_normalize=correct_normalize,
-                                  align_corners=align_corners, z_folded=z_folded, z_residual=z_residual,
-                                  add_ref_residual=add_ref_residual, sample_locs_in=sample_locs_in, want_attn=want_attn,
+                                  align_corners=align_corners, z_folded=None if hp else z_folded, z_residual=z_residual and not hp,
+                                  add_ref_residual=add_ref_residual and not hp, sample_locs_in=sample_locs_in, want_attn=want_attn,
                                   want_corr=want_corr, want_locs=want_locs, variant=variant, out=out4, state=state, views=V,
-                                  table=table, out_dtype=out_dtype)
+                                  table=table, out_dtype=out_dtype, head=hp)
     pairs = (V, S, N)
     return (out if out is not None else o.unflatten(0, pairs), None if corr is None else corr.unflatten(0, pairs),
             None if attn is None else attn.unflatten(0, pairs), None if locs is None else locs.unflatten(1, pairs))
@@ -277,12 +294,14 @@ def epipolar_fusion_views(feats, P, *, K, downsample=4.0, img_scale=1.0, softmax
 
 def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, img_scale, softmax_scale, correct_normalize,
             align_corners, z_folded, z_residual, add_ref_residual, sample_locs_in, want_attn, want_corr, want_locs, variant, out,
-            state, views=0, table=None, out_dtype=torch.float32):
+            state, views=0, table=None, out_dtype=torch.float32, head=None):
     """The forward of `epipolar_fusion` (S = 1) and `epipolar_fusion_multi`: feat_ref [N,C,H,W], feat_src / out [S·N,C,H,W],
     P_src [S·N,3,4], sample_locs_in [K,S·N,H,W,2]; outputs have S·N items (pair p = s·N + n).
     views = V >= 2 (`epipolar_fusion_views`): feat_ref [V·N,C,H,W] and P_ref [V·N,3,4] hold the views, feat_src and P_src are
     None, and the outputs have V·S·N items (pair p = (v·S + j)·N + n), S = V−1, or the width of `table` ([V,S] int32 host
-    array from `view_source_table`, which selects the source-table entry points).  out has dtype out_dtype."""
+    array from `view_source_table`, which selects the source-table entry points).  out has dtype out_dtype.
+    head = (A, B | None, b) from `_head_operands`: the heat-map call (epi_fusion_heatmaps_f32); `out` is then None, and the first
+    result is heat [pairs,J,H,W] of dtype out_dtype."""
     NR, C, H, W = feat_ref.shape
     ocode = FEAT_DTYPES[out_dtype]
     N = NR // views if views else NR
@@ -299,7 +318,9 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
         sample_locs_in = _aligned_locs(sample_locs_in.to(device=dev, dtype=torch.float32))
         if tuple(sample_locs_in.shape) != (K, NP, H, W, 2):
             raise ValueError("sample_locs_in must be [K,N,H,W,2]")
-    if out is None and views:                                            # the layout of a single call's empty_like(feat_src)
+    if head is not None:
+        out = torch.empty((NP, head[0].shape[0], H, W), device=dev, dtype=out_dtype)       # heat
+    elif out is None and views:                                          # the layout of a single call's empty_like(feat_src)
         cl = feat_ref.dim() == 4 and feat_ref.is_contiguous(memory_format=torch.channels_last) and not feat_ref.is_contiguous()
         out = torch.empty((NP, C, H, W), device=dev, dtype=out_dtype,
                           memory_format=torch.channels_last if cl else torch.contiguous_format)
@@ -316,7 +337,7 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     key = (dev, S, views, tkey, N, C, H, W, int(K), dcode, ocode, feat_ref.stride(), out.stride(), out.data_ptr() % 16 == 0, src_key,
            z_folded is not None, vcode,
            sample_locs_in is not None, float(downsample), float(img_scale), float(softmax_scale), bool(correct_normalize),
-           bool(align_corners), bool(z_residual), bool(add_ref_residual))
+           bool(align_corners), bool(z_residual), bool(add_ref_residual), head is not None)
     if state is not None and state.key == key:
         p = state.params
     else:
@@ -337,14 +358,24 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
     p.P_ref = P_ref.data_ptr() if sample_locs_in is None else None
     p.P_src = P_src.data_ptr() if sample_locs_in is None and P_src is not None else None
     p.sample_locs_in = sample_locs_in.data_ptr() if sample_locs_in is not None else None
-    p.out = out.data_ptr()
+    p.out = out.data_ptr() if head is None else None
     p.attn = attn.data_ptr() if attn is not None else None
     p.corr_pos = corr.data_ptr() if corr is not None else None
     p.sample_locs_out = locs.data_ptr() if locs is not None else None
     if z_folded is not None:
         wf, bf = z_folded
         p.z_weight_folded = wf.data_ptr(); p.z_bias_folded = bf.data_ptr()
-    if table is None:
+    if head is not None:                                           # the heat-map call: any form, with or without a table
+        h = _lib.EpiHeadParams()
+        A, B, b = head
+        h.A = A.data_ptr(); h.B = B.data_ptr() if B is not None else None; h.b = b.data_ptr()
+        h.heat = out.data_ptr(); h.heat_stride = _strides4(out); h.J = A.shape[0]
+        targs = (ctypes.byref(h),) + ((None, 0) if table is None else
+                                      (table.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), table.shape[1]))
+        cache_bytes = lambda q: lib.epi_fusion_heatmaps_cache_bytes(q, *targs)
+        workspace_bytes = lambda q: lib.epi_fusion_heatmaps_workspace_bytes(q, *targs)
+        forward = lambda q, st: lib.epi_fusion_heatmaps_f32(q, *targs, st)
+    elif table is None:
         cache_bytes, workspace_bytes = lib.epi_fusion_cache_bytes, lib.epi_fusion_workspace_bytes
         forward = lib.epi_fusion_forward_f32
     else:                                                          # the [V,S] host table goes with every call
@@ -369,7 +400,7 @@ def _fusion(lib, dcode, S, feat_ref, feat_src, P_ref, P_src, *, K, downsample, i
             state.ws = ws; state.params = p; state.key = key
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(forward(ctypes.byref(p), ctypes.c_void_p(stream)),
+        _lib.check(forward(ctypes.byref(p), ctypes.c_void_p(stream)), "epi_fusion_heatmaps_f32" if head is not None else
                    "epi_fusion_forward_f32" if table is None else "epi_fusion_view_sources_forward_f32")
     return out, corr, attn, locs
 
@@ -607,6 +638,77 @@ def fold_z_bn(z: nn.Conv2d, bn: nn.BatchNorm2d):
     return wf, bf
 
 
+def head_weights(head):
+    """(weight [J,C], bias [J] | None) of a pose head: a 1x1 nn.Conv2d (stride 1, no padding, one group, like `final_layer`,
+    resnet.py:421) or a (weight [J,C] or [J,C,1,1], bias [J] | None) pair.  Anything else raises ValueError."""
+    if isinstance(head, nn.Conv2d):
+        if (head.kernel_size != (1, 1) or head.stride != (1, 1) or head.dilation != (1, 1) or head.groups != 1 or
+                tuple(head.padding) != (0, 0)):
+            raise ValueError("the head must be a 1x1 nn.Conv2d with stride 1, no padding and one group (got %r)" % (head,))
+        weight, bias = head.weight, head.bias
+    elif isinstance(head, (tuple, list)) and len(head) == 2:
+        weight, bias = head
+    else:
+        raise ValueError("head must be a 1x1 nn.Conv2d or a (weight, bias) pair (got %s)" % type(head).__name__)
+    if not isinstance(weight, torch.Tensor) or not (weight.dim() == 2 or (weight.dim() == 4 and weight.shape[2:] == (1, 1))):
+        raise ValueError("the head weight must be [J,C] or [J,C,1,1]")
+    weight = weight.flatten(1)
+    J = weight.shape[0]
+    if not 1 <= J <= _lib.HEAD_MAX_JOINTS:
+        raise ValueError("the head must have 1 to %d output channels (got %d)" % (_lib.HEAD_MAX_JOINTS, J))
+    if bias is not None and (not isinstance(bias, torch.Tensor) or tuple(bias.shape) != (J,)):
+        raise ValueError("the head bias must be None or [J]")
+    return weight, bias
+
+
+def fold_head(weight, bias=None, z_folded=None, z_residual=False):
+    """(A [J,C], b [J]) of the heat-map epilogue, computed on the device (one launch, no host sync): A = Wh·(Wf + z_residual·I),
+    b = Wh·bf + bh, each element summed in fp64 and rounded once to float32; without z_folded (a layer without z) A = Wh and
+    b = bh.  weight [J,C] (or [J,C,1,1]) and bias [J] | None are read as their float32 values; z_folded = `fold_z_bn`'s (Wf, bf)."""
+    lib = _lib.load()
+    _lib.require_heatmaps(lib)
+    weight, bias = head_weights((weight, bias))
+    J, C = weight.shape
+    dev = weight.device
+    if not weight.is_cuda:
+        raise RuntimeError("the head weight is on %s: the heat-map epilogue has no CPU implementation" % dev)
+    f32 = lambda t: None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous()
+    wh, bh = f32(weight), f32(bias)
+    wf, bf = (None, None) if z_folded is None else map(f32, z_folded)
+    if wf is not None and tuple(wf.shape) != (C, C):
+        raise ValueError("z_folded's weight must be [C,C] with C = %d, the head's input channels" % C)
+    A = torch.empty((J, C), device=dev, dtype=torch.float32)
+    b = torch.empty((J,), device=dev, dtype=torch.float32)
+    ptr = lambda t: None if t is None else t.data_ptr()
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(lib.epi_fold_head_f32(wh.data_ptr(), ptr(bh), ptr(wf), ptr(bf), int(bool(z_residual and wf is not None)), J, C,
+                                         A.data_ptr(), b.data_ptr(), ctypes.c_void_p(stream)), "epi_fold_head_f32")
+    return A, b
+
+
+class _Folded(tuple):
+    """(A, B, b) that `Epipolar._head_folded` folded and checked: the functional forms take it as their `head` as it stands."""
+
+
+def _head_operands(lib, head, feat_ref, feat_src, out, z_folded, z_residual, add_ref_residual):
+    """(A, B | None, b) of a functional heat-map call: z / BN folded into the head, B = the head weight with the caller's
+    residual.  Refuses `out` and gradients (the heat-map forward has no backward)."""
+    _lib.require_heatmaps(lib)
+    if out is not None:
+        raise ValueError("a call with a head returns heat-maps: out must be None (the fused feature is not stored)")
+    if isinstance(head, _Folded):
+        return tuple(head)
+    weight, bias = head_weights(head)
+    if weight.shape[1] != feat_ref.shape[1]:
+        raise ValueError("the head takes %d channels, the maps have %d" % (weight.shape[1], feat_ref.shape[1]))
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (feat_ref, feat_src, weight, bias)):
+        raise RuntimeError("the heat-map forward is inference only (it has no backward); run it under torch.no_grad()")
+    A, b = fold_head(weight, bias, z_folded, z_residual)
+    B = weight.detach().to(dtype=torch.float32).contiguous() if add_ref_residual else None
+    return A, B, b
+
+
 def sample_locs(P_ref, P_src, H, W, K, downsample=4.0, img_scale=1.0, correct_normalize=False):
     """Device grid2sample_locs (epipolar.py:323-418): [K,N,H,W,2] normalised (x,y)."""
     lib = _lib.load()
@@ -679,6 +781,7 @@ class Epipolar(nn.Module):
             self.z = nn.Conv2d(nf // ep.BOTTLENECK, nf, kernel_size=1, stride=1, padding=0, bias=True)
             self.bn = ZeroInitBN(nf)
         self._fold_cache = None
+        self._head_cache = None
         self._states = {}            # device -> FusionState (persistent workspace + camera-keyed cache)
         # carries the dtype the module is cast to, which `out` takes; no elements and not persistent, so the state_dict keys
         # stay the reference's
@@ -706,6 +809,46 @@ class Epipolar(nn.Module):
             ev.record(cur)
             self._fold_cache = (key, folded, ev, {cur.cuda_stream})
         _, folded, ev, seen = self._fold_cache
+        if cur.cuda_stream not in seen:          # a consumer on another stream must not read the fold before it is written
+            cur.wait_event(ev)
+            seen.add(cur.cuda_stream)
+        return folded
+
+    # -- eval-mode folding of z + BN + the pose head into the heat-map epilogue, cached like _folded ---------------
+    def _head_folded(self, head, feat):
+        """(A, B, b) of the heat-map call for `head` (1x1 nn.Conv2d or (weight, bias)): z / BN (eval) folded into the head, and
+        B = the head weight, which adds the caller's residual `ret + feat` (resnet.py:388).  Refuses gradients, and training
+        mode with z."""
+        lib = _lib.load()
+        _lib.require_heatmaps(lib)
+        weight, bias = head_weights(head)
+        has_z = "z" in self.cfg.EPIPOLAR.PARAMETERIZED
+        if has_z and self.training:
+            raise RuntimeError("the heat-map forward folds the z projection's BatchNorm with its running statistics: call "
+                               "module.eval() first")
+        params = [weight, bias] + ([self.z.weight, self.z.bias, self.bn.weight, self.bn.bias] if has_z else [])
+        if torch.is_grad_enabled() and (feat.requires_grad or any(t is not None and t.requires_grad for t in params)):
+            raise RuntimeError("the heat-map forward is inference only (it has no backward); run it under torch.no_grad()")
+        if weight.shape[1] != feat.shape[-3]:
+            raise ValueError("the head takes %d channels, the maps have %d" % (weight.shape[1], feat.shape[-3]))
+        zres = bool(self.cfg.EPIPOLAR.ZRESIDUAL) and has_z
+
+        def fold():
+            A, b = fold_head(weight, bias, self._folded() if has_z else None, zres)
+            return A, weight.detach().to(dtype=torch.float32).contiguous(), b
+
+        if torch.cuda.is_current_stream_capturing():
+            return fold()                        # inside the graph, for the reason _folded gives
+        ts = [weight, bias] + ([self.z.weight, self.z.bias, self.bn.weight, self.bn.bias, self.bn.running_mean,
+                                self.bn.running_var] if has_z else [])
+        key = (zres,) + tuple((t.data_ptr(), t._version) for t in ts if t is not None)
+        cur = torch.cuda.current_stream(weight.device)
+        if self._head_cache is None or self._head_cache[0] != key:
+            folded = fold()
+            ev = torch.cuda.Event()
+            ev.record(cur)
+            self._head_cache = (key, folded, ev, {cur.cuda_stream})
+        _, folded, ev, seen = self._head_cache
         if cur.cuda_stream not in seen:          # a consumer on another stream must not read the fold before it is written
             cur.wait_event(ev)
             seen.add(cur.cuda_stream)
@@ -761,16 +904,46 @@ class Epipolar(nn.Module):
             finalout = out
         return finalout, corr, attn, (locs.transpose(0, 1) if want_locs else None)
 
-    def forward_multi(self, feat1, feats2, P1, P2s):
+    def forward_heatmaps(self, feat1, feat2, P1, P2, head):
+        """The eval step of the pose network from this layer on, `head(fused_other_feat(feat1, feat2, P1, P2, self)[0])`
+        (resnet.py:385-388,421), with the 1x1 head as the fused forward's epilogue: the fused feature is never stored.
+        head: the 1x1 nn.Conv2d `final_layer` (or a (weight [J,C], bias [J]) pair), 1 <= J <= 64.  Returns (heat [N,J,H,W] in the
+        module's dtype, corr_pos, attention, sample_locs) as `forward` returns them (bit for bit).  z / BN and the head are
+        folded once per parameter version (`fold_head`).  Inference only: gradients and training mode with z raise
+        RuntimeError."""
+        cfg = self.cfg
+        ep = cfg.EPIPOLAR
+        hp = self._head_folded(head, feat1)
+        want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+        heat, corr, attn, locs = epipolar_fusion(
+            feat1, feat2, P1, P2, K=self.sample_size, downsample=self.downsample,
+            img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE, softmax_scale=ep.SOFTMAXSCALE,
+            correct_normalize=ep.USE_CORRECT_NORMALIZE, align_corners=self.align_corners, want_attn=self.emit_attn,
+            want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant, state=self._state_for(feat1, "single-heat"),
+            out_dtype=self.out_dtype, head=_Folded(hp))
+        return heat, corr, attn, (locs.transpose(0, 1) if want_locs else None)
+
+    def forward_multi(self, feat1, feats2, P1, P2s, head=None):
         """`forward` of one reference batch against S source views in one fused call (the MULTITEST path,
         modeling/model.py:213-239).  feat1 [N,C,H,W], feats2 [S,N,C,H,W] or a sequence of S [N,C,H,W] maps, P1 [N,3,4],
         P2s [S,N,3,4].  Returns what S calls of `forward` return, stacked over the sources:
         (finalout [S,N,C,H,W], corr_pos [S,N,H,W,2] | None, attention [S,N,K,H,W] | None, sample_locs [S,N,K,H,W,2] | None).
         Inference only.  With the z projection the module must be in eval mode: training-mode BatchNorm would take its
-        batch statistics over all S·N items, which S separate calls do not."""
+        batch statistics over all S·N items, which S separate calls do not.
+        head: as in `forward_heatmaps`; then heat [S,N,J,H,W] = head(finalout + feat1) in place of finalout."""
         cfg = self.cfg
         ep = cfg.EPIPOLAR
         has_z = "z" in ep.PARAMETERIZED
+        if head is not None:
+            hp = self._head_folded(head, feat1)
+            want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+            heat, corr, attn, locs = epipolar_fusion_multi(
+                feat1, feats2, P1, P2s, K=self.sample_size, downsample=self.downsample,
+                img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE, softmax_scale=ep.SOFTMAXSCALE,
+                correct_normalize=ep.USE_CORRECT_NORMALIZE, align_corners=self.align_corners, want_attn=self.emit_attn,
+                want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant, state=self._state_for(feat1, "multi-heat"),
+                out_dtype=self.out_dtype, head=_Folded(hp))
+            return heat, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
         if has_z and self.training:
             raise RuntimeError("Epipolar.forward_multi with the z projection needs eval mode: training-mode BatchNorm statistics "
                                "over S*N items differ from S separate forward calls")
@@ -785,17 +958,29 @@ class Epipolar(nn.Module):
             state=self._state_for(feat1, "multi"), out_dtype=self.out_dtype)
         return out, corr, attn, (locs.permute(1, 2, 0, 3, 4, 5) if want_locs else None)
 
-    def forward_views(self, feats, P, sources=None):
+    def forward_views(self, feats, P, sources=None, head=None):
         """`forward` of every view of a frame against several other views in one fused call.  feats [V,N,C,H,W] or a
         sequence of V [N,C,H,W] maps, P [V,N,3,4].  sources=None: every other view (the whole MULTITEST path,
         modeling/model.py:213-239), S = V−1 and u = j + (j >= v); a [V,S] host table (see `epipolar_fusion_views`): u =
         sources[v][j].  Returns what `forward(feats[v], feats[u], P[v], P[u])` returns for reference view v and its j-th source
         u, stacked as (finalout [V,S,N,C,H,W], corr_pos [V,S,N,H,W,2] | None, attention [V,S,N,K,H,W] | None,
         sample_locs [V,S,N,K,H,W,2] | None).  Inference only.  With the z projection the module must be in eval mode, for the
-        reason `forward_multi` gives."""
+        reason `forward_multi` gives.
+        head: as in `forward_heatmaps`; then heat [V,S,N,J,H,W] = head(finalout + feats[v]) in place of finalout."""
         cfg = self.cfg
         ep = cfg.EPIPOLAR
         has_z = "z" in ep.PARAMETERIZED
+        if head is not None:
+            first = feats[0] if isinstance(feats, (list, tuple)) and feats else feats
+            hp = self._head_folded(head, first)
+            want_locs = bool(cfg.VIS.EPIPOLAR_LINE)
+            heat, corr, attn, locs = epipolar_fusion_views(
+                feats, P, K=self.sample_size, downsample=self.downsample,
+                img_scale=cfg.DATASETS.IMAGE_RESIZE * cfg.DATASETS.PREDICT_RESIZE, softmax_scale=ep.SOFTMAXSCALE,
+                correct_normalize=ep.USE_CORRECT_NORMALIZE, align_corners=self.align_corners, want_attn=self.emit_attn,
+                want_corr=self.emit_corr, want_locs=want_locs, variant=self.variant, state=self._state_for(first, "views-heat"),
+                sources=sources, out_dtype=self.out_dtype, head=_Folded(hp))
+            return heat, corr, attn, (locs.permute(1, 2, 3, 0, 4, 5, 6) if want_locs else None)
         if has_z and self.training:
             raise RuntimeError("Epipolar.forward_views with the z projection needs eval mode: training-mode BatchNorm statistics "
                                "over V*(V-1)*N items differ from separate forward calls")
@@ -858,7 +1043,16 @@ def fused_other_feat(feat, other_features, KRT, other_KRT, sampler: Epipolar, ca
     return ret, corr_pos, depth, locs
 
 
-def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma, downsample):
+def _fused_tail(tail, fuse_head):
+    """fuse_head=True needs `tail` to be the 1x1 head itself (an nn.Conv2d that `head_weights` accepts)."""
+    if fuse_head:
+        if not isinstance(tail, nn.Conv2d):
+            raise ValueError("fuse_head=True needs tail to be the 1x1 nn.Conv2d head (got %s)" % type(tail).__name__)
+        head_weights(tail)
+    return fuse_head
+
+
+def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma, downsample, fuse_head=False):
     """The multi-view test of the reference (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239) from the fusion layer on:
     every reference item is fused with each of the S other views, each fusion goes through the rest of the network and the
     peak finder, and every joint keeps the location of the source whose peak scores highest (torch.max over the sources, then
@@ -867,7 +1061,13 @@ def multitest(sampler: Epipolar, tail, feat, other_feats, KRT, other_KRTs, sigma
     feat [N,C,H,W] (the reference views' features at the merge point), other_feats [S,N,C,H,W] or S [N,C,H,W] maps, KRT
     [N,3,4], other_KRTs [S,N,3,4]; tail: everything after the merge point ([B,C,H,W] -> heat-maps [B,J,h,w]; `final_layer`
     for MERGE='late'); sigma = cfg.KEYPOINT.SIGMA, downsample as for find_tensor_peak_batch.
-    Returns (locs [N,J,2], scores [N,J], source index [N,J]); the reference's final `squeeze()` is left to the caller."""
+    Returns (locs [N,J,2], scores [N,J], source index [N,J]); the reference's final `squeeze()` is left to the caller.
+    fuse_head=True: tail must be the 1x1 nn.Conv2d head (else ValueError), and runs as the fused forward's epilogue
+    (`Epipolar.forward_multi(head=)`), so the fused feature is never stored."""
+    if _fused_tail(tail, fuse_head):
+        with torch.no_grad():
+            heat, _, _, _ = sampler.forward_multi(feat, other_feats, KRT, other_KRTs, head=tail)
+            return find_tensor_peak_best(heat, sigma, downsample)
     with torch.no_grad():
         ret, _, _, _ = sampler.forward_multi(feat, other_feats, KRT, other_KRTs)
         x = ret if sampler.fuse_ref_residual else ret + feat          # getOtherFeat's `ret + feat` (resnet.py:388), per source
@@ -888,7 +1088,7 @@ def _table_on(table, dev):
     return t
 
 
-def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample, sources=None):
+def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample, sources=None, fuse_head=False):
     """The reference's multi-view test (cfg.EPIPOLAR.MULTITEST, modeling/model.py:213-239) for every view of a frame at once:
     each view v is the reference in turn, is fused with each of its sources, each fusion goes through the rest of the
     network and the peak finder, and every joint keeps the location of the source whose peak scores highest.  All V·S
@@ -898,14 +1098,22 @@ def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample, sour
     as for `multitest`.  sources=None: every other view (S = V−1); a [V,S] host table (e.g. `multiview.nearest_view_table`
     with topk = S): the sources it names, a cheaper test over each view's S nearest cameras.  Returns per view
     (locs [V,N,J,2], scores [V,N,J], source view [V,N,J]): the source is the camera index u of the winning view, not its
-    position j among the view's sources."""
+    position j among the view's sources.
+    fuse_head=True: tail must be the 1x1 nn.Conv2d head (else ValueError), and runs as the fused forward's epilogue
+    (`Epipolar.forward_views(head=)`), so the V·S·N fused features are never stored."""
+    fuse_head = _fused_tail(tail, fuse_head)
     with torch.no_grad():
         if isinstance(feats, (list, tuple)):
             feats = torch.stack(list(feats))
-        ret, _, _, _ = sampler.forward_views(feats, KRT, sources=sources)
-        V, S, N = ret.shape[0], ret.shape[1], ret.shape[2]
-        x = ret if sampler.fuse_ref_residual else ret + feats[:, None]    # getOtherFeat's `ret + feat` of reference view v
-        heat = tail(x.flatten(0, 2))                                       # [V·S·N, J, h, w]
+        if fuse_head:
+            heat, _, _, _ = sampler.forward_views(feats, KRT, sources=sources, head=tail)
+            V, S, N = heat.shape[0], heat.shape[1], heat.shape[2]
+            heat = heat.flatten(0, 2)                                      # [V·S·N, J, h, w]
+        else:
+            ret, _, _, _ = sampler.forward_views(feats, KRT, sources=sources)
+            V, S, N = ret.shape[0], ret.shape[1], ret.shape[2]
+            x = ret if sampler.fuse_ref_residual else ret + feats[:, None]    # getOtherFeat's `ret + feat` of reference view v
+            heat = tail(x.flatten(0, 2))                                       # [V·S·N, J, h, w]
         # [S, V·N, J, h, w]: source slot j of every (view, item)
         heat = heat.unflatten(0, (V, S, N)).transpose(0, 1).flatten(1, 2)
         locs, scores, j = find_tensor_peak_best(heat, sigma, downsample)
@@ -917,7 +1125,7 @@ def multitest_views(sampler: Epipolar, tail, feats, KRT, sigma, downsample, sour
         return locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), table.gather(1, j.flatten(1)).view_as(j)
 
 
-def standard_views_test(sampler: Epipolar, tail, feats, KRT, sources, sigma, downsample):
+def standard_views_test(sampler: Epipolar, tail, feats, KRT, sources, sigma, downsample, fuse_head=False):
     """The reference's standard (non-MULTITEST) test from one backbone pass: each view v is the reference once, fused with
     the one source view sources[v][0] (its nearest camera, data/datasets/multiview_h36m.py:231-238), and the fusion goes
     through getOtherFeat's residual (modeling/backbones/resnet.py:377-388), the rest of the network and the peak finder
@@ -927,15 +1135,23 @@ def standard_views_test(sampler: Epipolar, tail, feats, KRT, sources, sigma, dow
     sampler: the Epipolar layer; tail: everything after the merge point ([B,C,H,W] -> heat-maps [B,J,h,w]); feats
     [V,N,C,H,W] or V [N,C,H,W] maps (the views' features at the merge point); KRT [V,N,3,4]; sources: a [V,1] host table
     (`multiview.nearest_view_table(..., topk=1)`); sigma = cfg.KEYPOINT.SIGMA, downsample as for find_tensor_peak_batch.
-    Returns per view (locs [V,N,J,2], scores [V,N,J], corr_pos [V,N,H,W,2] | None, attention [V,N,K,H,W] | None)."""
+    Returns per view (locs [V,N,J,2], scores [V,N,J], corr_pos [V,N,H,W,2] | None, attention [V,N,K,H,W] | None).
+    fuse_head=True: tail must be the 1x1 nn.Conv2d head (else ValueError), and runs as the fused forward's epilogue
+    (`Epipolar.forward_views(head=)`), so the fused features are never stored."""
+    fuse_head = _fused_tail(tail, fuse_head)
     with torch.no_grad():
         if isinstance(feats, (list, tuple)):
             feats = torch.stack(list(feats))
         V, N = feats.shape[0], feats.shape[1]
         if view_source_table(sources, V).shape[1] != 1:
             raise ValueError("the standard test fuses each view with one source: sources must be [V,1]")
-        ret, corr, attn, _ = sampler.forward_views(feats, KRT, sources=sources)
-        x = ret[:, 0] if sampler.fuse_ref_residual else ret[:, 0] + feats     # getOtherFeat's `ret + feat`
-        locs, scores = find_tensor_peak_batch(tail(x.flatten(0, 1)), sigma, downsample)
+        if fuse_head:
+            heat, corr, attn, _ = sampler.forward_views(feats, KRT, sources=sources, head=tail)
+            heat = heat[:, 0].flatten(0, 1)
+        else:
+            ret, corr, attn, _ = sampler.forward_views(feats, KRT, sources=sources)
+            x = ret[:, 0] if sampler.fuse_ref_residual else ret[:, 0] + feats     # getOtherFeat's `ret + feat`
+            heat = tail(x.flatten(0, 1))
+        locs, scores = find_tensor_peak_batch(heat, sigma, downsample)
         return (locs.unflatten(0, (V, N)), scores.unflatten(0, (V, N)), None if corr is None else corr[:, 0],
                 None if attn is None else attn[:, 0])

@@ -238,6 +238,45 @@ size_t epi_fusion_views_backward_workspace_bytes(const EpiFusionBwdParams *p, in
 /* 1: this library has the views backward above (a library built before it lacks this symbol). */
 int epi_fusion_views_backward(void);
 
+/* ---- heat-maps: the pose head's 1×1 conv as the forward's epilogue ------------------------------------------------------
+ * The eval step of the pose network after the fusion layer is  final_layer(ret + feat)  (/root/reference/modeling/backbones/
+ * resnet.py:388,421).  With X the pre-z fused feature, (Wf, bf) the z / BN fold (epi_fold_z_bn_f32), R the caller's residual
+ * feat_ref of the pair's query item and (Wh [J,C], bh [J]) the head:
+ *   heat = Wh·(Wf·X + bf + z_res·X + R) + bh = A·X + B·R + b,   A = Wh·(Wf + z_res·I),  B = Wh,  b = Wh·bf + bh
+ * (without z: A = Wh, b = bh; without the caller's residual: B = 0).  The fused feature is never written to `out`. */
+typedef struct EpiHeadParams {
+    const float *A;               /* [J,C] row-major, 4-byte aligned (epi_fold_head_f32) */
+    const float *B;               /* [J,C] row-major: the head weight Wh, adding the caller's residual feat_ref; or NULL (none) */
+    const float *b;               /* [J] */
+    void *heat;                   /* [pairs,J,H,W] logical, any element strides below, element type EPI_OUT_DTYPE of feat_dtype
+                                     (float32 unless bits 8-15 of feat_dtype say otherwise), aligned to its element size */
+    int64_t heat_stride[4];
+    int32_t J;                    /* joints, 1 <= J <= 64 */
+    int32_t reserved[3];          /* must be zero */
+} EpiHeadParams;
+
+/* Fold z / BN and the head into (A, b) of EpiHeadParams on the device: A = Wh·(Wf + z_residual·I), b = Wh·bf + bh, each element
+ * summed in fp64 and rounded once to fp32.  Wh [J,C] row-major; bh [J] or NULL (zero); Wf [C,C] (epi_fold_z_bn_f32) or NULL
+ * (A = Wh, b = bh: a layer without z); bf [C] or NULL (zero).  A_out [J,C], b_out [J].  One launch; never synchronises, so it
+ * can be captured in a CUDA graph.  EPI_EINVAL for a NULL Wh / A_out / b_out, J < 1 or C < 1. */
+int epi_fold_head_f32(const float *Wh, const float *bh, const float *Wf, const float *bf, int32_t z_residual, int32_t J, int32_t C,
+                      float *A_out, float *b_out, void *stream);
+
+/* The forward of any form (pair, n_src, n_views, or the views form with a source table: sources_host a [V][S] host table as in
+ * epi_fusion_view_sources_forward_f32, or NULL with S = 0 for none) with the head as its epilogue: h->heat receives, per pair,
+ * A·X + B·R + b; attn, corr_pos and sample_locs_out are what the same call without the head writes, bit for bit.  The fused kernel
+ * stores X as an fp32 pixel-major plane in the workspace, and one more launch applies the head: every heat element is an fp32 sum
+ * over c = 0 .. C−1 in one fixed order (b, then A[j,c]·X[c] and B[j,c]·R[c] for increasing c), so each pair's heat is bit for bit
+ * that of the pair-form call on that pair, and a 16-bit heat is the fp32 heat rounded once.  EPI_EINVAL (with a message) for a
+ * non-NULL out, z_weight_folded or nonzero add_ref_residual (A, B and b express them), a NULL h / A / b / heat, J < 1 or J > 64,
+ * nonzero reserved words, and every refusal of the form it runs. */
+int epi_fusion_heatmaps_f32(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S, void *stream);
+/* Workspace / cache bytes of that call (0 when the params, the head or the table cannot be planned). */
+size_t epi_fusion_heatmaps_workspace_bytes(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S);
+size_t epi_fusion_heatmaps_cache_bytes(const EpiFusionParams *p, const EpiHeadParams *h, const int32_t *sources_host, int32_t S);
+/* 1: this library has the heat-map entry points above (a library built before them lacks this symbol). */
+int epi_fusion_heatmaps(void);
+
 /* Only the geometry: sample locations [K,N,H,W,2] for (P_ref,P_src)  (grid2sample_locs). */
 int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_locs_out, int32_t N,
                         int32_t H, int32_t W, int32_t K, float downsample, float img_scale, float eps,
