@@ -14,10 +14,11 @@ from .epipolar import (Epipolar, FusionState, ZeroInitBN, epipolar_fusion, epipo
                        epipolar_fusion_views_backward, fold_z_bn, fold_head, head_weights, sample_locs, fused_other_feat, multitest, multitest_views, standard_views_test, view_source_table)
 from .host_pipeline import HostStreamer, bind_host_to_gpu
 from .peaks import find_tensor_peak_batch, find_tensor_peak_best
+from .triangulate import triangulate_views
 from . import multiview, synthetic
 
 __all__ = ["Epipolar", "FusionState", "HostStreamer", "bind_host_to_gpu", "ZeroInitBN", "epipolar_fusion", "fold_z_bn", "fold_head", "head_weights", "sample_locs", "fused_other_feat", "find_tensor_peak_batch",
            "epipolar_fusion_multi", "multitest", "find_tensor_peak_best", "epipolar_fusion_views", "epipolar_fusion_views_backward", "multitest_views",
-           "standard_views_test", "view_source_table",
+           "standard_views_test", "view_source_table", "triangulate_views",
            "Node", "default_cfg", "make_cfg", "get_global_cfg", "set_global_cfg",
            "cfg_h36m_r50_256", "cfg_h36m_r152_384", "multiview", "synthetic"]

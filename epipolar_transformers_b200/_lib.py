@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libepipolar_b200.so")
 
 EPI_ABI_VERSION = 3
 EPI_DTYPE_F32, EPI_DTYPE_BF16, EPI_DTYPE_F16 = 0, 1, 2
+EPI_DTYPE_F64 = 3                   # the cameras of epi_triangulate_dlt_f64 only
 
 
 def EPI_OUT_DTYPE(d):
@@ -33,7 +34,7 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources",
            "epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward",
            "epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_heatmaps_workspace_bytes", "epi_fusion_heatmaps_cache_bytes",
-           "epi_fusion_heatmaps")
+           "epi_fusion_heatmaps", "epi_triangulate_dlt_f64", "epi_triangulate")
 # The source-table entry points are new symbols, not a reinterpreted field, so a library without them still runs every other
 # form correctly: load() accepts it, and only a call with a source table needs them (`require_view_sources`).
 VIEW_SOURCES_EXPORTS = ("epi_fusion_view_sources_forward_f32", "epi_fusion_view_sources_workspace_bytes",
@@ -43,6 +44,9 @@ VIEWS_BACKWARD_EXPORTS = ("epi_fusion_views_backward_f32", "epi_fusion_views_bac
 # So are the heat-map forward and its fold: only a call with a head needs them (`require_heatmaps`).
 HEATMAPS_EXPORTS = ("epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_heatmaps_workspace_bytes",
                     "epi_fusion_heatmaps_cache_bytes", "epi_fusion_heatmaps")
+# And the triangulation: only `triangulate_views` needs it (`require_triangulate`).
+TRIANGULATE_EXPORTS = ("epi_triangulate_dlt_f64", "epi_triangulate")
+TRIANGULATE_MAX_VIEWS = 64          # epi_triangulate_dlt_f64's V (include/epipolar_b200.h)
 HEAD_MAX_JOINTS = 64                # EpiHeadParams.J (include/epipolar_b200.h)
 
 _fp = ctypes.POINTER(ctypes.c_float)
@@ -118,7 +122,8 @@ def load():
             "epipolar_transformers_b200: CUDA library %s is missing. Build it with "
             "`python -m epipolar_transformers_b200.build` (needs nvcc). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    missing = [s for s in EXPORTS if s not in VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS + HEATMAPS_EXPORTS and not hasattr(lib, s)]
+    optional = VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS + HEATMAPS_EXPORTS + TRIANGULATE_EXPORTS
+    missing = [s for s in EXPORTS if s not in optional and not hasattr(lib, s)]
     if missing:
         # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
         # (a views call would silently run as a one-source call)
@@ -187,6 +192,11 @@ def load():
         lib.epi_fusion_heatmaps.restype = ctypes.c_int
         lib.epi_fold_head_f32.restype = ctypes.c_int
         lib.epi_fold_head_f32.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 3
+    if all(hasattr(lib, s) for s in TRIANGULATE_EXPORTS):
+        lib.epi_triangulate_dlt_f64.restype = ctypes.c_int
+        lib.epi_triangulate_dlt_f64.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32, ctypes.c_double] + [ctypes.c_int32] * 3 + \
+            [ctypes.c_void_p] * 3
+        lib.epi_triangulate.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))
@@ -216,6 +226,14 @@ def require_heatmaps(lib):
     if missing or lib.epi_fusion_heatmaps() != 1:
         raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot run the pose head as the forward's epilogue; "
                            "rebuild it with `python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_fusion_heatmaps"]))
+
+
+def require_triangulate(lib):
+    """Raise unless `lib` has the DLT triangulation (epi_triangulate())."""
+    missing = [s for s in TRIANGULATE_EXPORTS if not hasattr(lib, s)]
+    if missing or lib.epi_triangulate() != 1:
+        raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot triangulate joints; rebuild it with "
+                           "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_triangulate"]))
 
 
 def check(rc: int, what: str):

@@ -1,5 +1,6 @@
 // epi_abi.cu — the extern "C" boundary declared in include/epipolar_b200.h.
 // Validates arguments, plans the forward (kernels, staging, workspace and cache regions) and launches the plan on the caller's stream.
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 
@@ -796,6 +797,27 @@ int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32
     cudaError_t e = epi::launch_peaks_best(heat, locs, scores, src_index, S, B, J, H, W, radius, downsample, threshold, int_div,
                                            reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(EPI_ECUDA, "peak kernel launch failed: %s", cudaGetErrorString(e));
+    return EPI_OK;
+}
+
+int epi_triangulate(void) { return 1; }
+
+int epi_triangulate_dlt_f64(const float *locs, const float *scores, const void *P, int32_t P_dtype, double conf_thres, int32_t V,
+                            int32_t N, int32_t J, double *X, int32_t *n_used, void *stream) {
+    if (!locs || !scores || !P || !X || !n_used) return fail(EPI_EINVAL, "locs, scores, P, X and n_used must be non-null");
+    if (V < 2 || V > 64) return fail(EPI_EINVAL, "V must be in [2, 64] (the selected views are a 64-bit mask)");
+    if (N < 1 || J < 1) return fail(EPI_EINVAL, "need N >= 1 and J >= 1");
+    if ((int64_t)N * J > INT32_MAX) return fail(EPI_EINVAL, "N * J must be <= 2^31 - 1 (one thread per problem, counted in int32)");
+    if (P_dtype != EPI_DTYPE_F32 && P_dtype != EPI_DTYPE_F64) return fail(EPI_EINVAL, "P_dtype must be EPI_DTYPE_F32 or EPI_DTYPE_F64");
+    if (!std::isfinite(conf_thres)) return fail(EPI_EINVAL, "conf_thres must be finite");
+    if (conf_thres > 1000.0) return fail(EPI_EINVAL, "conf_thres must be <= 1000 (the view selection steps down from it by 0.05)");
+    const uintptr_t pa = P_dtype == EPI_DTYPE_F64 ? 8 : 4;
+    if (reinterpret_cast<uintptr_t>(locs) % 8 || reinterpret_cast<uintptr_t>(X) % 8 || reinterpret_cast<uintptr_t>(P) % pa ||
+        reinterpret_cast<uintptr_t>(scores) % 4 || reinterpret_cast<uintptr_t>(n_used) % 4)
+        return fail(EPI_EINVAL, "locs, X and a float64 P must be 8-byte aligned, scores, n_used and a float32 P 4-byte aligned");
+    cudaError_t e = epi::launch_triangulate(locs, scores, P, P_dtype == EPI_DTYPE_F64, conf_thres, V, N, J, X, n_used,
+                                            reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(EPI_ECUDA, "triangulation launch failed: %s", cudaGetErrorString(e));
     return EPI_OK;
 }
 

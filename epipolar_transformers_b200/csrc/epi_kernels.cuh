@@ -184,6 +184,9 @@ cudaError_t launch_peaks(const float *heat, float *locs, float *scores, int B, i
 // heat [S,B,J,H,W]: per (b, j) the peak of the source with the highest score (first source on a tie); src_index may be null
 cudaError_t launch_peaks_best(const float *heat, float *locs, float *scores, int *src_index, int S, int B, int J, int H, int W,
                               float radius, float downsample, float threshold, int int_div, cudaStream_t st);
+// locs [V,N,J,2], scores [V,N,J], P [V,N,3,4] (float64 when P_f64, else float32) -> X [N,J,3], n_used [N,J]: one thread per (n, j)
+cudaError_t launch_triangulate(const float *locs, const float *scores, const void *P, bool P_f64, double conf_thres, int V, int N,
+                               int J, double *X, int *n_used, cudaStream_t st);
 cudaError_t launch_sample_locs(const float *P_ref, const float *P_src, float *locs, int N, const GeomCfg &gc, cudaStream_t st);
 
 }  // namespace epi

@@ -52,6 +52,8 @@ extern "C" {
 #define EPI_DTYPE_F32 0
 #define EPI_DTYPE_BF16 1
 #define EPI_DTYPE_F16 2
+/* float64: only the cameras of epi_triangulate_dlt_f64 take it */
+#define EPI_DTYPE_F64 3
 /* element type of the forward's `out`, in bits 8-15 of EpiFusionParams.feat_dtype: feat_dtype = maps | EPI_OUT_DTYPE(out).
  * A bfloat16 or float16 `out` is the float32 result rounded once (to nearest even); attn, corr_pos and sample_locs_out stay
  * float32.  A library that predates the byte refuses a nonzero one with EPI_EINVAL ("unknown feat_dtype"). */
@@ -297,6 +299,27 @@ int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_
  * epi_find_peaks_f32's result bit for bit. */
 int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32_t *src_index, int32_t S, int32_t B, int32_t J,
                             int32_t H, int32_t W, float radius, float downsample, float threshold, int32_t int_div, void *stream);
+
+/* Linear (DLT) triangulation of every (frame, joint) in one launch: the reference's KEYPOINT.TRIANGULATION = 'pymvg' mode
+ * (vision/triangulation.py, triangulate_pymvg, and pymvg's find3d, with zero distortion).  For the problem (n, j):
+ *   1. views: t = conf_thres in fp64; repeat { sel = {v : scores[v,n,j] > (float)t}; stop if t < -1; if |sel| <= 1,
+ *      t = t - 0.05 (fp64) and repeat; else stop }.  The compare is float32, as numpy compares a float32 array with a Python
+ *      float; a NaN score is never selected.
+ *   2. A: per selected view, in increasing view order, the rows x·M[2] - M[0] and y·M[2] - M[1] in fp64, M = P[v,n], (x, y) =
+ *      locs[v,n,j].
+ *   3. X[n,j] = w[:3] / w[3], w the right singular vector of A's smallest singular value (Givens QR of A's rows into a 4x4 R,
+ *      then one-sided Jacobi on R, all in fp64; AᵀA is never formed).
+ * n_used[n,j] = |sel| (0 .. V).  X is NaN when |sel| < 2 or a selected view has a non-finite location or camera entry;
+ * w[3] = 0 gives the IEEE quotient.  locs [V,N,J,2] (image px, any resizing already applied), scores [V,N,J] and P [V,N,3,4] are
+ * contiguous; P is float32 (P_dtype = EPI_DTYPE_F32) or float64 (EPI_DTYPE_F64).  One launch on `stream`; never synchronises,
+ * so it can be captured in a CUDA graph.  EPI_EINVAL (with a message) for a NULL pointer, V < 2 or V > 64, N < 1, J < 1,
+ * N·J > 2^31 - 1, an unknown P_dtype, a non-finite conf_thres or one above 1000 (step 1 would count down from it for
+ * (conf_thres + 1) / 0.05 passes), and locs, X or a float64 P not 8-byte aligned or scores, n_used or a float32 P not 4-byte
+ * aligned. */
+int epi_triangulate_dlt_f64(const float *locs, const float *scores, const void *P, int32_t P_dtype, double conf_thres, int32_t V,
+                            int32_t N, int32_t J, double *X, int32_t *n_used, void *stream);
+/* 1: this library has epi_triangulate_dlt_f64 (a library built before it lacks this symbol). */
+int epi_triangulate(void);
 
 /* Fold conv1x1 z + eval BatchNorm into (Wf, bf) on the device, no host sync:
  *   Wf[o,c] = s[o]·Wz[o,c],  bf[o] = s[o]·(bz[o] − mean[o]) + beta[o],  s = gamma/sqrt(var+bn_eps). */
