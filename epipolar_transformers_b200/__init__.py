@@ -15,10 +15,12 @@ from .epipolar import (Epipolar, FusionState, ZeroInitBN, epipolar_fusion, epipo
 from .host_pipeline import HostStreamer, bind_host_to_gpu
 from .peaks import find_tensor_peak_batch, find_tensor_peak_best
 from .triangulate import triangulate_views
+from .rpsm import H36M_PARENTS, crop_affine, limb_lengths, rpsm_pairwise, rpsm_views
 from . import multiview, synthetic
 
 __all__ = ["Epipolar", "FusionState", "HostStreamer", "bind_host_to_gpu", "ZeroInitBN", "epipolar_fusion", "fold_z_bn", "fold_head", "head_weights", "sample_locs", "fused_other_feat", "find_tensor_peak_batch",
            "epipolar_fusion_multi", "multitest", "find_tensor_peak_best", "epipolar_fusion_views", "epipolar_fusion_views_backward", "multitest_views",
            "standard_views_test", "view_source_table", "triangulate_views",
+           "rpsm_views", "rpsm_pairwise", "limb_lengths", "crop_affine", "H36M_PARENTS",
            "Node", "default_cfg", "make_cfg", "get_global_cfg", "set_global_cfg",
            "cfg_h36m_r50_256", "cfg_h36m_r152_384", "multiview", "synthetic"]

@@ -34,7 +34,8 @@ EXPORTS = ("epi_version", "epi_last_error", "epi_fusion_workspace_bytes", "epi_f
            "epi_fusion_view_sources_workspace_bytes", "epi_fusion_view_sources_cache_bytes", "epi_fusion_view_sources",
            "epi_fusion_views_backward_f32", "epi_fusion_views_backward_workspace_bytes", "epi_fusion_views_backward",
            "epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_heatmaps_workspace_bytes", "epi_fusion_heatmaps_cache_bytes",
-           "epi_fusion_heatmaps", "epi_triangulate_dlt_f64", "epi_triangulate")
+           "epi_fusion_heatmaps", "epi_triangulate_dlt_f64", "epi_triangulate", "epi_rpsm_f32", "epi_rpsm_workspace_bytes",
+           "epi_rpsm_pairwise_pack", "epi_rpsm")
 # The source-table entry points are new symbols, not a reinterpreted field, so a library without them still runs every other
 # form correctly: load() accepts it, and only a call with a source table needs them (`require_view_sources`).
 VIEW_SOURCES_EXPORTS = ("epi_fusion_view_sources_forward_f32", "epi_fusion_view_sources_workspace_bytes",
@@ -47,6 +48,9 @@ HEATMAPS_EXPORTS = ("epi_fold_head_f32", "epi_fusion_heatmaps_f32", "epi_fusion_
 # And the triangulation: only `triangulate_views` needs it (`require_triangulate`).
 TRIANGULATE_EXPORTS = ("epi_triangulate_dlt_f64", "epi_triangulate")
 TRIANGULATE_MAX_VIEWS = 64          # epi_triangulate_dlt_f64's V (include/epipolar_b200.h)
+# And the recursive pictorial structure: only `rpsm_views` and `rpsm_pairwise` need it (`require_rpsm`).
+RPSM_EXPORTS = ("epi_rpsm_f32", "epi_rpsm_workspace_bytes", "epi_rpsm_pairwise_pack", "epi_rpsm")
+RPSM_MAX_VIEWS, RPSM_MAX_JOINTS, RPSM_MAX_NBINS, RPSM_MAX_RECUR_NBINS, RPSM_MAX_DEPTH = 64, 32, 16, 4, 32
 HEAD_MAX_JOINTS = 64                # EpiHeadParams.J (include/epipolar_b200.h)
 
 _fp = ctypes.POINTER(ctypes.c_float)
@@ -109,6 +113,19 @@ class EpiFusionBwdParams(ctypes.Structure):
     ]
 
 
+class EpiRpsmParams(ctypes.Structure):
+    """Field-for-field mirror of `struct EpiRpsmParams` (include/epipolar_b200.h)."""
+    _fields_ = [
+        ("heat", ctypes.c_void_p), ("P", ctypes.c_void_p), ("crop", ctypes.c_void_p), ("root", ctypes.c_void_p),
+        ("limb_length", ctypes.c_void_p), ("pairwise", ctypes.c_void_p), ("parents", ctypes.POINTER(ctypes.c_int32)),
+        ("pose", ctypes.c_void_p), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
+        ("V", ctypes.c_int32), ("N", ctypes.c_int32), ("J", ctypes.c_int32), ("h", ctypes.c_int32), ("w", ctypes.c_int32),
+        ("first_nbins", ctypes.c_int32), ("recur_nbins", ctypes.c_int32), ("recur_depth", ctypes.c_int32),
+        ("align_corners", ctypes.c_int32), ("image_size", ctypes.c_float * 2), ("grid_size", ctypes.c_double),
+        ("tolerance", ctypes.c_double),
+    ]
+
+
 _lib = None
 
 
@@ -122,7 +139,7 @@ def load():
             "epipolar_transformers_b200: CUDA library %s is missing. Build it with "
             "`python -m epipolar_transformers_b200.build` (needs nvcc). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
-    optional = VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS + HEATMAPS_EXPORTS + TRIANGULATE_EXPORTS
+    optional = VIEW_SOURCES_EXPORTS + VIEWS_BACKWARD_EXPORTS + HEATMAPS_EXPORTS + TRIANGULATE_EXPORTS + RPSM_EXPORTS
     missing = [s for s in EXPORTS if s not in optional and not hasattr(lib, s)]
     if missing:
         # e.g. a library built before EpiFusionBwdParams.deterministic or EpiFusionParams.n_views, which would ignore the field
@@ -197,6 +214,15 @@ def load():
         lib.epi_triangulate_dlt_f64.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32, ctypes.c_double] + [ctypes.c_int32] * 3 + \
             [ctypes.c_void_p] * 3
         lib.epi_triangulate.restype = ctypes.c_int
+    if all(hasattr(lib, s) for s in RPSM_EXPORTS):
+        lib.epi_rpsm_f32.restype = ctypes.c_int
+        lib.epi_rpsm_f32.argtypes = [ctypes.POINTER(EpiRpsmParams), ctypes.c_void_p]
+        lib.epi_rpsm_workspace_bytes.restype = ctypes.c_size_t
+        lib.epi_rpsm_workspace_bytes.argtypes = [ctypes.POINTER(EpiRpsmParams)]
+        lib.epi_rpsm_pairwise_pack.restype = ctypes.c_int
+        lib.epi_rpsm_pairwise_pack.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32, ctypes.c_double,
+                                               ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p]
+        lib.epi_rpsm.restype = ctypes.c_int
     v = lib.epi_version()
     if v != EPI_ABI_VERSION:
         raise RuntimeError("libepipolar_b200.so ABI version %d != expected %d" % (v, EPI_ABI_VERSION))
@@ -234,6 +260,14 @@ def require_triangulate(lib):
     if missing or lib.epi_triangulate() != 1:
         raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot triangulate joints; rebuild it with "
                            "`python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_triangulate"]))
+
+
+def require_rpsm(lib):
+    """Raise unless `lib` has the recursive pictorial structure (epi_rpsm())."""
+    missing = [s for s in RPSM_EXPORTS if not hasattr(lib, s)]
+    if missing or lib.epi_rpsm() != 1:
+        raise RuntimeError("libepipolar_b200.so does not export %s, so it cannot run the recursive pictorial structure; rebuild "
+                           "it with `python -m epipolar_transformers_b200.build --force`" % (missing or ["epi_rpsm"]))
 
 
 def check(rc: int, what: str):

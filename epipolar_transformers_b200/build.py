@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libepipolar_b200.so")
 STAMP = LIB + ".flags"          # the nvcc flags LIB was built with: a library built for another architecture is rebuilt
-SOURCES = ["epi_abi.cu", "epi_aux.cu", "epi_fusion_warp.cu", "epi_fusion_tile.cu", "epi_fusion_pipe.cu", "epi_fusion_bwd.cu", "epi_stage.cu", "epi_peaks.cu", "epi_zgemm.cu", "epi_umma_selftest.cu", "epi_head.cu", "epi_triangulate.cu"]
+SOURCES = ["epi_abi.cu", "epi_aux.cu", "epi_fusion_warp.cu", "epi_fusion_tile.cu", "epi_fusion_pipe.cu", "epi_fusion_bwd.cu", "epi_stage.cu", "epi_peaks.cu", "epi_zgemm.cu", "epi_umma_selftest.cu", "epi_head.cu", "epi_triangulate.cu", "epi_rpsm.cu"]
 HEADERS = ["epi_common.cuh", "epi_kernels.cuh", "epi_umma.cuh", os.path.join("..", "..", "include", "epipolar_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -800,6 +800,129 @@ int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32
     return EPI_OK;
 }
 
+namespace {
+
+// torch.linspace(-size/2, size/2, n) in float32, as its CPU kernel computes it: each half one fused multiply-add
+void rpsm_linspace(double size, int n, float *g) {
+    const float start = (float)(-size / 2), end = (float)(size / 2);
+    const float step = (end - start) / (float)(n - 1);
+    for (int i = 0; i < n; i++) g[i] = i < n / 2 ? std::fma(step, (float)i, start) : std::fma(-step, (float)(n - 1 - i), end);
+}
+
+bool rpsm_size_ok(double v) { return std::isfinite(v) && v > 0.0 && v <= 3.0e38; }
+
+// parents[J] -> the tree (one root, every joint reaching it); false with g_err set otherwise
+int rpsm_tree(const int32_t *parents, int J, epi::RpsmTree &t) {
+    memset(&t, 0, sizeof(t));
+    t.J = J;
+    t.E = J - 1;
+    t.root = -1;
+    for (int j = 0; j < J; j++) {
+        const int p = parents[j];
+        if (p == -1) {
+            if (t.root >= 0) return fail(EPI_EINVAL, "parents has more than one root (-1)");
+            t.root = j;
+        } else if (p < 0 || p >= J || p == j) {
+            return fail(EPI_EINVAL, "parents[j] must be -1 (the root) or another joint's index in [0, J)");
+        }
+        t.parent[j] = (signed char)p;
+    }
+    if (t.root < 0) return fail(EPI_EINVAL, "parents has no root (-1)");
+    int e = 0;
+    for (int j = 0; j < J; j++) {
+        int d = 0;
+        for (int k = j; parents[k] != -1; k = parents[k])
+            if (++d >= J) return fail(EPI_EINVAL, "parents is not a tree (a cycle does not reach the root)");
+        t.depth[j] = (signed char)d;
+        t.max_depth = d > t.max_depth ? d : t.max_depth;
+        t.edge[j] = (signed char)(j == t.root ? -1 : e++);
+    }
+    int k = 0;
+    for (int d = 0; d <= t.max_depth; d++)
+        for (int j = 0; j < J; j++)
+            if (t.depth[j] == d) t.bfs[k++] = (signed char)j;
+    return EPI_OK;
+}
+
+size_t rpsm_energy_bytes(const EpiRpsmParams *p) {
+    const size_t B = (size_t)p->first_nbins * p->first_nbins * p->first_nbins;
+    return align_up((size_t)p->N * p->J * B * sizeof(float));
+}
+
+}  // namespace
+
+int epi_rpsm(void) { return 1; }
+
+size_t epi_rpsm_workspace_bytes(const EpiRpsmParams *p) {
+    if (!p || p->N < 1 || p->J < 1 || p->J > epi::kRpsmMaxJoints || p->first_nbins < 2 || p->first_nbins > epi::kRpsmMaxNbins0)
+        return 0;
+    const size_t B = (size_t)p->first_nbins * p->first_nbins * p->first_nbins;
+    return rpsm_energy_bytes(p) + align_up((size_t)p->N * (p->J - 1) * B * sizeof(int16_t));
+}
+
+int epi_rpsm_f32(const EpiRpsmParams *p, void *stream) {
+    if (!p) return fail(EPI_EINVAL, "params must be non-null");
+    if (!p->heat || !p->P || !p->crop || !p->root || !p->limb_length || !p->pairwise || !p->parents || !p->pose || !p->workspace)
+        return fail(EPI_EINVAL, "heat, P, crop, root, limb_length, pairwise, parents, pose and workspace must be non-null");
+    if (p->V < 2 || p->V > 64) return fail(EPI_EINVAL, "V must be in [2, 64]");
+    if (p->N < 1) return fail(EPI_EINVAL, "need N >= 1");
+    if (p->J < 1 || p->J > epi::kRpsmMaxJoints) return fail(EPI_EINVAL, "J must be in [1, 32]");
+    if (p->first_nbins < 2 || p->first_nbins > epi::kRpsmMaxNbins0) return fail(EPI_EINVAL, "first_nbins must be in [2, 16]");
+    if (p->recur_nbins < 2 || p->recur_nbins > epi::kRpsmMaxNbinsR) return fail(EPI_EINVAL, "recur_nbins must be in [2, 4]");
+    if (p->recur_depth < 0 || p->recur_depth > epi::kRpsmMaxDepth) return fail(EPI_EINVAL, "recur_depth must be in [0, 32]");
+    if (p->h < 2 || p->w < 2) return fail(EPI_EINVAL, "the heat-maps need h >= 2 and w >= 2");
+    if (!rpsm_size_ok(p->grid_size) || !rpsm_size_ok(p->tolerance))
+        return fail(EPI_EINVAL, "grid_size and tolerance must be finite and positive");
+    if (!rpsm_size_ok(p->image_size[0]) || !rpsm_size_ok(p->image_size[1]))
+        return fail(EPI_EINVAL, "image_size must be finite and positive");
+    const void *f32[] = {p->heat, p->P, p->crop, p->root, p->limb_length, p->pairwise, p->pose};
+    for (const void *q : f32)
+        if (reinterpret_cast<uintptr_t>(q) % 4) return fail(EPI_EINVAL, "heat, P, crop, root, limb_length, pairwise and pose must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(p->workspace) % 256) return fail(EPI_EINVAL, "workspace must be 256-byte aligned");
+    if (p->workspace_bytes < epi_rpsm_workspace_bytes(p)) return fail(EPI_EINVAL, "workspace_bytes is smaller than epi_rpsm_workspace_bytes()");
+    epi::RpsmTree t;
+    if (int rc = rpsm_tree(p->parents, p->J, t)) return rc;
+    epi::RpsmArgs a;
+    memset(&a, 0, sizeof(a));
+    a.heat = p->heat; a.P = p->P; a.crop = p->crop; a.root = p->root; a.limb = p->limb_length; a.mask = p->pairwise;
+    a.energy = static_cast<float *>(p->workspace);
+    a.state = at<int16_t>(p->workspace, rpsm_energy_bytes(p));
+    a.pose = p->pose;
+    a.V = p->V; a.N = p->N; a.h = p->h; a.w = p->w;
+    a.n0 = p->first_nbins; a.B = a.n0 * a.n0 * a.n0; a.nr = p->recur_nbins; a.depth = p->recur_depth; a.align = p->align_corners ? 1 : 0;
+    a.img0 = p->image_size[0]; a.img1 = p->image_size[1]; a.tol = (float)p->tolerance;
+    rpsm_linspace(p->grid_size, a.n0, a.g0);
+    double size = p->grid_size / p->first_nbins;          // the reference's cur_grd_size, a Python float
+    for (int r = 0; r < a.depth; r++) {
+        rpsm_linspace(size, a.nr, a.gr[r]);
+        size = size / p->recur_nbins;
+    }
+    int n = 0;
+    cudaError_t e = epi::launch_rpsm(a, t, reinterpret_cast<cudaStream_t>(stream), &n);
+    if (e != cudaSuccess) return fail(EPI_ECUDA, "rpsm launch failed: %s", cudaGetErrorString(e));
+    g_launches = n;
+    return EPI_OK;
+}
+
+int epi_rpsm_pairwise_pack(const float *dense, const float *limb_length, int32_t E, int32_t nbins, double grid_size,
+                           double tolerance, uint32_t *packed, void *stream) {
+    if ((dense == nullptr) == (limb_length == nullptr)) return fail(EPI_EINVAL, "give exactly one of dense and limb_length");
+    if (!packed) return fail(EPI_EINVAL, "packed must be non-null");
+    if (E < 0 || E > epi::kRpsmMaxJoints - 1) return fail(EPI_EINVAL, "E must be in [0, 31]");
+    if (nbins < 2 || nbins > epi::kRpsmMaxNbins0) return fail(EPI_EINVAL, "nbins must be in [2, 16]");
+    if (!rpsm_size_ok(grid_size)) return fail(EPI_EINVAL, "grid_size must be finite and positive");
+    if (limb_length && !rpsm_size_ok(tolerance)) return fail(EPI_EINVAL, "tolerance must be finite and positive");
+    if (reinterpret_cast<uintptr_t>(packed) % 4 || reinterpret_cast<uintptr_t>(dense) % 4 || reinterpret_cast<uintptr_t>(limb_length) % 4)
+        return fail(EPI_EINVAL, "dense, limb_length and packed must be 4-byte aligned");
+    if (E == 0) return EPI_OK;
+    float g0[epi::kRpsmMaxNbins0];
+    rpsm_linspace(grid_size, nbins, g0);
+    cudaError_t e = epi::launch_rpsm_pack(dense, limb_length, E, nbins, g0, (float)tolerance, packed,
+                                          reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) return fail(EPI_ECUDA, "rpsm pairwise pack launch failed: %s", cudaGetErrorString(e));
+    return EPI_OK;
+}
+
 int epi_triangulate(void) { return 1; }
 
 int epi_triangulate_dlt_f64(const float *locs, const float *scores, const void *P, int32_t P_dtype, double conf_thres, int32_t V,

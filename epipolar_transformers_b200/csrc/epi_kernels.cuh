@@ -189,4 +189,32 @@ cudaError_t launch_triangulate(const float *locs, const float *scores, const voi
                                int J, double *X, int *n_used, cudaStream_t st);
 cudaError_t launch_sample_locs(const float *P_ref, const float *P_src, float *locs, int N, const GeomCfg &gc, cudaStream_t st);
 
+// ---- recursive pictorial structure (epi_rpsm.cu) ----
+constexpr int kRpsmMaxJoints = 32, kRpsmMaxNbins0 = 16, kRpsmMaxNbinsR = 4, kRpsmMaxDepth = 32;
+// The tree and the level grids, built and checked on the host; passed by value.
+struct RpsmTree {
+    int J, E, root, max_depth;
+    signed char parent[kRpsmMaxJoints];   // -1 at the root
+    signed char edge[kRpsmMaxJoints];     // edge index of joint j as a child (the e-th non-root joint); -1 at the root
+    signed char depth[kRpsmMaxJoints];
+    signed char bfs[kRpsmMaxJoints];      // joints by ascending depth, the root first
+};
+struct RpsmArgs {
+    const float *heat, *P, *crop, *root, *limb;   // [V,N,J,h,w], [V,N,3,4], [V,N,2,3], [N,3], [N,E]
+    const uint32_t *mask;                         // level-0 pairwise, [E, B, ceil(B/32)], row = parent bin
+    float *energy;                                // workspace: level-0 energies [N, J, B]
+    int16_t *state;                               // workspace: level-0 arg-max states [N, E, B]
+    float *pose;                                  // [N, J, 3]
+    int V, N, h, w, n0, B, nr, depth, align;
+    float img0, img1, tol;
+    float g0[kRpsmMaxNbins0];                     // level-0 1-D grid (linspace), before the centre is added
+    float gr[kRpsmMaxDepth][kRpsmMaxNbinsR];      // recursion r's 1-D grid
+};
+// launches: 1 unary + tree.max_depth max-product + 1 recursion kernel; returns the count in *launches
+cudaError_t launch_rpsm(const RpsmArgs &a, const RpsmTree &t, cudaStream_t st, int *launches);
+// packed [E, B, ceil(B/32)] bits: dense[e, p, k] != 0 (dense non-null), or |dist(X_p, X_k)| within tol of limb[e] on the
+// level-0 grid g0 centred at the origin
+cudaError_t launch_rpsm_pack(const float *dense, const float *limb, int E, int n0, const float *g0, float tol, uint32_t *packed,
+                             cudaStream_t st);
+
 }  // namespace epi

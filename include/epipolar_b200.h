@@ -321,6 +321,49 @@ int epi_triangulate_dlt_f64(const float *locs, const float *scores, const void *
 /* 1: this library has epi_triangulate_dlt_f64 (a library built before it lacks this symbol). */
 int epi_triangulate(void);
 
+/* The reference's recursive pictorial-structure model (KEYPOINT.TRIANGULATION = 'rpsm', modeling/pictorial_cuda.py) for N
+ * frames at once.  The tree is the host array parents[J] (the root -1, every other joint its parent's index); a joint's
+ * children are taken in ascending index, and edge e is the e-th non-root joint (limb_length's and the mask's edge order).
+ * Level 0 is a cube of first_nbins^3 = B bins of side grid_size around root[n], one grid for all joints, its pairwise term the
+ * caller's packed 0/1 mask; recursion r = 1..recur_depth puts recur_nbins^3 bins of side grid_size / first_nbins /
+ * recur_nbins^(r-1) around each joint's current estimate, its pairwise term |dist + 1e-9 - limb_length| < tolerance.  The
+ * arithmetic, operation by operation, is in csrc/epi_rpsm.cu's header; the pose is the chosen bins' float32 coordinates. */
+typedef struct EpiRpsmParams {
+    const float *heat;          /* [V,N,J,h,w] heat-maps */
+    const float *P;             /* [V,N,3,4] original-image cameras (origK @ RT) */
+    const float *crop;          /* [V,N,2,3] crop affine of each view (get_affine_transform(center, scale, 0, image_size)) */
+    const float *root;          /* [N,3] centre of the level-0 cube */
+    const float *limb_length;   /* [N,E] limb lengths (E = J - 1), used by the recursions */
+    const uint32_t *pairwise;   /* [E,B,ceil(B/32)] level-0 mask, bit k of row p = parent bin p may take child bin k */
+    const int32_t *parents;     /* HOST array [J] */
+    float *pose;                /* [N,J,3] output */
+    void *workspace;            /* epi_rpsm_workspace_bytes(), 256-byte aligned */
+    size_t workspace_bytes;
+    int32_t V, N, J, h, w;
+    int32_t first_nbins, recur_nbins, recur_depth, align_corners;
+    float image_size[2];        /* IMAGE_SIZE (x, y) in pixels */
+    double grid_size;           /* GRID_SIZE (mm); the level sizes are divided in fp64 */
+    double tolerance;           /* LIMB_LENGTH_TOLERANCE (mm), compared in float32 */
+} EpiRpsmParams;
+
+/* Bytes of workspace for `p`: the level-0 energies (N·J·B float32) and arg-max states (N·E·B int16). */
+size_t epi_rpsm_workspace_bytes(const EpiRpsmParams *p);
+/* pose for every frame; 2 + (the tree's depth) launches on `stream` whatever N is (epi_last_launch_count()); never
+ * synchronises, so it can be captured in a CUDA graph.  EPI_EINVAL (with a message) for a NULL pointer, V outside [2, 64],
+ * N < 1, J outside [1, 32] or a parents array that is not one tree, first_nbins outside [2, 16], recur_nbins outside [2, 4],
+ * recur_depth outside [0, 32], h or w < 2, a non-finite or non-positive grid_size, tolerance or image size, a float pointer
+ * not 4-byte aligned, a workspace not 256-byte aligned or smaller than epi_rpsm_workspace_bytes(). */
+int epi_rpsm_f32(const EpiRpsmParams *p, void *stream);
+/* The packed level-0 mask [E, B, ceil(B/32)] (B = nbins^3, bits past B zero) on the device, from either a dense [E,B,B]
+ * float32 mask (bit = entry != 0; limb_length NULL) or limb lengths [E] (dense NULL) on the level-0 grid centred at the
+ * origin, with the recursions' rule |dist + 1e-9 - limb_length| < tolerance.  One launch on `stream`.  EPI_EINVAL for both or
+ * neither source, a NULL or misaligned packed, E outside [0, 31], nbins outside [2, 16], a non-finite or non-positive
+ * grid_size or (limb lengths) tolerance. */
+int epi_rpsm_pairwise_pack(const float *dense, const float *limb_length, int32_t E, int32_t nbins, double grid_size,
+                           double tolerance, uint32_t *packed, void *stream);
+/* 1: this library has the epi_rpsm_* entry points (a library built before them lacks this symbol). */
+int epi_rpsm(void);
+
 /* Fold conv1x1 z + eval BatchNorm into (Wf, bf) on the device, no host sync:
  *   Wf[o,c] = s[o]·Wz[o,c],  bf[o] = s[o]·(bz[o] − mean[o]) + beta[o],  s = gamma/sqrt(var+bn_eps). */
 int epi_fold_z_bn_f32(const float *z_weight, const float *z_bias, const float *bn_weight,
