@@ -52,6 +52,7 @@ TRIANGULATE_MAX_VIEWS = 64          # epi_triangulate_dlt_f64's V (include/epipo
 RPSM_EXPORTS = ("epi_rpsm_f32", "epi_rpsm_workspace_bytes", "epi_rpsm_pairwise_pack", "epi_rpsm")
 RPSM_MAX_VIEWS, RPSM_MAX_JOINTS, RPSM_MAX_NBINS, RPSM_MAX_RECUR_NBINS, RPSM_MAX_DEPTH = 64, 32, 16, 4, 32
 HEAD_MAX_JOINTS = 64                # EpiHeadParams.J (include/epipolar_b200.h)
+PEAKS_MAX_R = 23169                 # EPI_PEAKS_MAX_R: the largest R = int(radius + 0.5) of the peak finders (include/epipolar_b200.h)
 
 _fp = ctypes.POINTER(ctypes.c_float)
 

@@ -3,6 +3,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <string>
 
 #include "../../include/epipolar_b200.h"
 #include "epi_kernels.cuh"
@@ -777,11 +778,28 @@ int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_lo
     return EPI_OK;
 }
 
+namespace {
+
+// The arguments both peak finders share.  One warp per (b, j), its index counted in int32; R = (int)(radius + 0.5f) in the kernel,
+// whose window loop counts to (2R+1)^2 + 31 in int.
+int peaks_args(int64_t BJ, int32_t H, int32_t W, float radius) {
+    if (BJ <= 0 || H < 2 || W < 2 || !(radius > 0.f)) return fail(EPI_EINVAL, "bad shape or radius");
+    if (!std::isfinite(radius)) return fail(EPI_EINVAL, "radius must be finite");
+    if (radius >= (float)(EPI_PEAKS_MAX_R + 1) || (int)(radius + 0.5f) > EPI_PEAKS_MAX_R)
+        return fail(EPI_EINVAL, "radius too large: R = int(radius + 0.5) must be at most EPI_PEAKS_MAX_R = %s",
+                    std::to_string(EPI_PEAKS_MAX_R).c_str());
+    if ((int)(radius + 0.5f) < 1) return fail(EPI_EINVAL, "radius must round to at least 1");
+    if (BJ > INT32_MAX / 32) return fail(EPI_EINVAL, "B * J too large (one warp per joint, counted in int32)");
+    return EPI_OK;
+}
+
+}  // namespace
+
 int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_t B, int32_t J, int32_t H, int32_t W,
                        float radius, float downsample, float threshold, int32_t int_div, void *stream) {
     if (!heatmaps || !locs || !scores) return fail(EPI_EINVAL, "null pointer");
-    if (B <= 0 || J <= 0 || H < 2 || W < 2 || !(radius > 0.f)) return fail(EPI_EINVAL, "bad shape or radius");
-    if ((int)(radius + 0.5f) < 1) return fail(EPI_EINVAL, "radius must round to at least 1");
+    if (B <= 0 || J <= 0) return fail(EPI_EINVAL, "bad shape or radius");
+    if (int rc = peaks_args((int64_t)B * J, H, W, radius)) return rc;
     cudaError_t e = epi::launch_peaks(heatmaps, locs, scores, B, J, H, W, radius, downsample, threshold, int_div,
                                       reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(EPI_ECUDA, "peak kernel launch failed: %s", cudaGetErrorString(e));
@@ -791,9 +809,8 @@ int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_
 int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32_t *src_index, int32_t S, int32_t B, int32_t J,
                             int32_t H, int32_t W, float radius, float downsample, float threshold, int32_t int_div, void *stream) {
     if (!heat || !locs || !scores) return fail(EPI_EINVAL, "null pointer");
-    if (S <= 0 || B <= 0 || J <= 0 || H < 2 || W < 2 || !(radius > 0.f)) return fail(EPI_EINVAL, "bad shape or radius");
-    if ((int)(radius + 0.5f) < 1) return fail(EPI_EINVAL, "radius must round to at least 1");
-    if ((int64_t)B * J > INT32_MAX / 32) return fail(EPI_EINVAL, "B * J too large (one warp per joint, counted in int32)");
+    if (S <= 0 || B <= 0 || J <= 0) return fail(EPI_EINVAL, "bad shape or radius");
+    if (int rc = peaks_args((int64_t)B * J, H, W, radius)) return rc;
     cudaError_t e = epi::launch_peaks_best(heat, locs, scores, src_index, S, B, J, H, W, radius, downsample, threshold, int_div,
                                            reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return fail(EPI_ECUDA, "peak kernel launch failed: %s", cudaGetErrorString(e));

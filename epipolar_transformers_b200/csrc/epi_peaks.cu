@@ -3,12 +3,12 @@
 // Restates /root/reference/modeling/backbones/basic_batch.py:17-63, which the caller runs once per batch item in a Python
 // loop (modeling/backbones/resnet.py:423-428), for a whole [B, J, H, W] stack of heat-maps in ONE launch, one warp per
 // (item, joint):
-//   score, index = max over the flattened map (first maximum)                                            (:24)
+//   score, index = max over the flattened map: the first NaN if there is one (torch.max), else the first maximum (:24)
 //   index_w = index % W ; index_h = index / W   — TRUE division under torch >= 1.5 (the semantics of the torch
 //       installed here, which is what the golden vectors freeze), integer division under the torch < 1.4 the repo
 //       names in its README: `int_div` selects it                                                     (:25-26)
 //   (2R+1)^2 bilinear samples (zero padding, align_corners=False) of the window [index -+ radius] laid out by
-//   F.affine_grid(align_corners=False), R = int(radius + 0.5); values <= threshold -> 0                   (:30-50)
+//   F.affine_grid(align_corners=False), R = int(radius + 0.5); values <= threshold -> 0, NaN kept          (:30-50)
 //   x = Σ sub·X / (Σ sub + eps) + index_w, y likewise with Y ; X, Y = arange(-radius, radius + 1e-4, radius / R)  (:52-57)
 //   pix2coord: v·downsample + downsample/2 − 0.5                                                         (:59-61)
 #include "epi_kernels.cuh"
@@ -21,18 +21,20 @@ __device__ __forceinline__ void peak_of(const float *__restrict__ m, int H, int 
                                         int int_div, float &out_x, float &out_y, float &out_score) {
     const int lane = threadIdx.x & 31;
     const int HW = H * W;
-    // ---- arg-max, first maximum (NaN never wins, like a plain comparison scan) ----
+    // ---- arg-max as torch.max computes it: NaN beats any number and the lowest index wins among NaNs; otherwise the
+    // first maximum.  A map of -inf alone records nothing and takes index 0, torch.max's first maximum. ----
     float best = -INFINITY;
     int bi = 0x7fffffff;
-    for (int i = lane; i < HW; i += 32) {
+    for (int i = lane; i < HW; i += 32) {                                // increasing i: the first NaN / maximum stays
         const float v = __ldg(m + i);
-        if (v > best) { best = v; bi = i; }
+        if (v > best || (v != v && best == best)) { best = v; bi = i; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        const bool onan = ov != ov, bnan = best != best;
+        if (onan ? (!bnan || oi < bi) : (!bnan && (ov > best || (ov == best && oi < bi)))) { best = ov; bi = oi; }
     }
     if (bi == 0x7fffffff) bi = 0;
     const float index_w = (float)(bi % W);
@@ -61,7 +63,7 @@ __device__ __forceinline__ void peak_of(const float *__restrict__ m, int H, int 
             if (xa && yb) v += (1.f - wx) * wy * __ldg(m + (y0 + 1) * W + x0);
             if (xb && yb) v += wx * wy * __ldg(m + (y0 + 1) * W + x0 + 1);
         }
-        if (!(v > threshold)) v = 0.f;                                   // F.threshold(sub, threshold, 0)
+        if (v <= threshold) v = 0.f;                                     // F.threshold(sub, threshold, 0): NaN is kept
         sum += v;
         sx = fmaf(v, -radius + step * (float)ix, sx);
         sy = fmaf(v, -radius + step * (float)iy, sy);
@@ -94,7 +96,8 @@ __global__ void __launch_bounds__(128) epi_peaks_kernel(const float *__restrict_
 }
 
 // Multi-view test (modeling/model.py:229-234): heat [S,B,J,H,W]; warp (b, j) runs the single-source peak of every source and
-// keeps the first one with the highest score — strict `>`, so a tie keeps the earlier source like torch.max.
+// keeps the one torch.max over the sources picks: the first NaN score if there is one, else the first highest score (strict
+// `>`, so a tie keeps the earlier source).
 __global__ void __launch_bounds__(128) epi_peaks_best_kernel(const float *__restrict__ heat, float *__restrict__ locs,
                                                              float *__restrict__ scores, int *__restrict__ src_index, int S, int BJ,
                                                              int H, int W, float radius, float downsample, float threshold,
@@ -106,7 +109,7 @@ __global__ void __launch_bounds__(128) epi_peaks_best_kernel(const float *__rest
     for (int s = 0; s < S; s++) {
         float x, y, score;
         peak_of(heat + ((size_t)s * BJ + warp) * H * W, H, W, radius, downsample, threshold, int_div, x, y, score);
-        if (s == 0 || score > bs) { bx = x; by = y; bs = score; bsrc = s; }
+        if (s == 0 || (score != score ? bs == bs : score > bs)) { bx = x; by = y; bs = score; bsrc = s; }
     }
     if (lane == 0) {
         locs[2 * warp] = bx;

@@ -288,15 +288,20 @@ int epi_sample_locs_f32(const float *P_ref, const float *P_src, float *sample_lo
  * /root/reference/modeling/backbones/resnet.py:423-428 over modeling/backbones/basic_batch.py:17-63):
  * heatmaps [B,J,H,W] contiguous -> locs [B,J,2] (x, y in image coordinates, pix2coord applied) and scores [B,J].
  * radius = cfg.KEYPOINT.SIGMA; threshold 1e-6 in the reference; int_div = 1 reproduces torch < 1.4's integer `index / W`,
- * 0 the true division of current torch (what the reference computes under the torch installed with this library). */
+ * 0 the true division of current torch (what the reference computes under the torch installed with this library).
+ * Non-finite values follow torch: the arg-max is the first NaN if the map holds one, else the first maximum; the threshold
+ * zeroes values <= threshold and keeps NaN, so a NaN or a zero bilinear weight times ±inf in the window gives a NaN location.
+ * EPI_EINVAL for a radius that is not finite and > 0, one whose R = int(radius + 0.5) is outside 1 .. EPI_PEAKS_MAX_R (the
+ * (2R+1)^2-sample window is counted in int32), or B·J > INT32_MAX / 32 (one warp per joint, counted in int32). */
+#define EPI_PEAKS_MAX_R 23169
 int epi_find_peaks_f32(const float *heatmaps, float *locs, float *scores, int32_t B, int32_t J, int32_t H, int32_t W,
                        float radius, float downsample, float threshold, int32_t int_div, void *stream);
 
 /* The best-source selection of the reference's multi-view test (modeling/model.py:229-234: torch.max over the sources' peak
  * scores, then gather of their locations): heat [S,B,J,H,W] contiguous -> for every (b, j) the peak of the source with the
  * highest score, locs [B,J,2], scores [B,J] and optionally (src_index != NULL) that source's index [B,J] as int32.  Each source's
- * peak is computed exactly as epi_find_peaks_f32 computes it; a tie keeps the first source (torch.max).  S = 1 returns
- * epi_find_peaks_f32's result bit for bit. */
+ * peak is computed exactly as epi_find_peaks_f32 computes it, with the same refusals; as torch.max, the first source with a NaN
+ * score wins, else the first with the highest score.  S = 1 returns epi_find_peaks_f32's result bit for bit. */
 int epi_find_peaks_best_f32(const float *heat, float *locs, float *scores, int32_t *src_index, int32_t S, int32_t B, int32_t J,
                             int32_t H, int32_t W, float radius, float downsample, float threshold, int32_t int_div, void *stream);
 

@@ -6,12 +6,15 @@ from __future__ import annotations
 import numpy as np
 
 
-def find_tensor_peak_batch(heatmap, radius, downsample, threshold=0.000001, int_div=False, dtype=np.float32):
-    """heatmap [J,H,W] -> (locs [J,2], score [J])."""
+def find_tensor_peak_batch(heatmap, radius, downsample, threshold=0.000001, int_div=False, dtype=np.float32, window=False):
+    """heatmap [J,H,W] -> (locs [J,2], score [J]), and with window=True also the thresholded window sub [J,S,S].
+
+    Non-finite values follow the reference: the arg-max is the first NaN if there is one (torch.max), the threshold keeps
+    NaN (F.threshold zeroes only v <= threshold), and a zero bilinear weight times ±inf is NaN."""
     heatmap = np.asarray(heatmap, dtype)
     J, H, W = heatmap.shape
     flat = heatmap.reshape(J, -1)
-    index = flat.argmax(1)                                                   # first maximum (:24)
+    index = flat.argmax(1)                                                   # first NaN, else first maximum (:24)
     score = flat[np.arange(J), index]
     index_w = (index % W).astype(dtype)                                      # :25
     index_h = (index // W).astype(dtype) if int_div else (index.astype(dtype) / dtype(W))   # :26 (true division in torch >= 1.5)
@@ -34,10 +37,11 @@ def find_tensor_peak_batch(heatmap, radius, downsample, threshold=0.000001, int_
             inb = ((yy >= 0) & (yy < H))[:, :, None] & ((xx >= 0) & (xx < W))[:, None, :]
             v = heatmap[np.arange(J)[:, None, None], np.clip(yy, 0, H - 1)[:, :, None], np.clip(xx, 0, W - 1)[:, None, :]]
             sub += np.where(inb, v, dtype(0)) * (wyy[:, :, None] * wxx[:, None, :]).astype(dtype)
-    sub = np.where(sub > dtype(threshold), sub, dtype(0))                    # F.threshold (:50)
+    sub = np.where(sub <= dtype(threshold), dtype(0), sub)                   # F.threshold keeps NaN (:50)
     X = (dtype(-radius) + dtype(radius * 1.0 / R) * np.arange(S, dtype=dtype))                # arange(-r, r+1e-4, r/R) (:52-53)
     sum_region = sub.reshape(J, -1).sum(1) + dtype(np.finfo(float).eps)
     x = (sub * X[None, None, :]).reshape(J, -1).sum(1) / sum_region + index_w
     y = (sub * X[None, :, None]).reshape(J, -1).sum(1) / sum_region + index_h
     p2c = lambda v: v * dtype(downsample) + dtype(downsample / 2.0) - dtype(0.5)              # vision/multiview.py:154-157
-    return np.stack([p2c(x), p2c(y)], 1), score
+    locs = np.stack([p2c(x), p2c(y)], 1)
+    return (locs, score, sub) if window else (locs, score)
